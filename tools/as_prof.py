@@ -1,5 +1,11 @@
-"""Phase timers of mlpg_fwd_as_kernel on the cfg2 batch.  Needs a debug build:
-   NNK_NVCC_EXTRA=-DNNK_AS_PROF python -m nnmnkwii_b200.build   (rebuild without it afterwards)"""
+"""Phase timers of mlpg_fwd_as_kernel: per-CTA clock64 cycles of every assembler and solver phase on the three
+MLPG workloads the benchmark reports (configs[1], T=1000 forward, T=1000 gradient).  Needs a library built with
+the counters, e.g. next to the normal one:
+
+    NNK_NVCC_EXTRA=-DNNK_AS_PROF NNK_LIB_OUT=/tmp/libnnk_prof.so python -m nnmnkwii_b200.build
+    NNK_LIB_PATH=/tmp/libnnk_prof.so python tools/as_prof.py
+
+(the build stamps its flags, so the next plain build recompiles every object)."""
 import ctypes
 import os
 import sys
@@ -12,41 +18,67 @@ sys.path.insert(0, ROOT)
 import bench  # noqa: E402
 from nnmnkwii_b200 import _device as dev, _lib, paramgen as G  # noqa: E402
 
-lens, means, variances = bench.make_batch(0)
+if not hasattr(_lib.lib, "nnk_as_prof_read"):
+    sys.exit("%s was built without -DNNK_AS_PROF" % _lib.LIB_PATH)
+NA = int(os.environ.get("NA", "3"))  # assembler warps per CTA of the build (NNK_AS_NA)
 device = torch.device("cuda", 0)
-layout = G.merlin_layout()
-n_rows = int(lens.sum())
-off = torch.from_numpy(np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)).to(device)
-d_m, d_v = torch.from_numpy(means).to(device), torch.from_numpy(variances).to(device)
-d_out = torch.zeros((n_rows, 63), dtype=torch.float32, device=device)
-order = torch.from_numpy(np.argsort(-lens, kind="stable").astype(np.int32)).to(device)
-chains = dev.chains_on_device(layout.chains, device)
 wc = _lib.make_windows(bench.WINDOWS)
 
+# configs[1]: the benchmark's batch (Merlin layout, 63 chains = 2 groups per utterance)
+lens, means, variances = bench.make_batch(0)
+layout = G.merlin_layout()
+off = torch.from_numpy(np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)).to(device)
+d_m, d_v = torch.from_numpy(means).to(device), torch.from_numpy(variances).to(device)
+d_out = torch.zeros((int(lens.sum()), 63), dtype=torch.float32, device=device)
+order = torch.from_numpy(np.argsort(-lens, kind="stable").astype(np.int32)).to(device)
+chains = dev.chains_on_device(layout.chains, device)
 
-def step():
+
+def cfg2():
     dev.run_mlpg("fwd", means=d_m, variances=d_v, rhs=None, out=d_out, offsets=off, lengths=None, order=order,
                  chains=chains, n_chain=layout.n_chain, max_T=int(lens.max()), windows_c=wc, in_ld=187, var_ld=187,
                  go_ld=0, out_ld=63, dtype_code=_lib.NNK_F32, go_f64=0, n_utt=len(lens), device=device, check=False)
 
 
-NA = int(os.environ.get("NA", "3"))
+# the T=1000 shapes of bench.bench_extras: 256 utterances, static_dim 60, per-frame variances
+B2, T2, sd2 = 256, 1000, 60
+g = torch.Generator(device=device).manual_seed(0)
+ch2 = dev.chains_on_device(dev.simple_chains(sd2), device)
+off2 = torch.arange(B2 + 1, dtype=torch.int64, device=device) * T2
+m2 = torch.rand(B2 * T2, 3 * sd2, device=device, generator=g)
+v2 = torch.rand(B2 * T2, 3 * sd2, device=device, generator=g) + 0.1
+go2 = torch.randn(B2 * T2, sd2, device=device, generator=g)
+y2 = torch.zeros(B2 * T2, sd2, device=device)
+g2 = torch.zeros(B2 * T2, 3 * sd2, device=device)
+
+
+def t1000(mode, rhs, o, out_ld):
+    dev.run_mlpg(mode, means=m2, variances=v2, rhs=rhs, out=o, offsets=off2, lengths=None, order=None, chains=ch2,
+                 n_chain=sd2, max_T=T2, windows_c=wc, in_ld=3 * sd2, var_ld=3 * sd2, go_ld=sd2, out_ld=out_ld,
+                 dtype_code=_lib.NNK_F32, go_f64=0, n_utt=B2, device=device, check=False)
+
+
+cases = (("configs[1]", cfg2, len(lens) * 2),
+         ("T1000 forward", lambda: t1000("fwd", None, y2, sd2), B2 * 2),
+         ("T1000 gradient", lambda: t1000("grad", go2, g2, 3 * sd2), B2 * 2))
+names = ["A wait pb_empty", "A wait input TMA", "A convert+assemble+publish", None,
+         "S wait pb_full", "S eliminate", "S wait scratch TMA", "S backward"]
 buf = (ctypes.c_ulonglong * 16)()
-for _ in range(3):
-    step()
-_lib.lib.nnk_as_prof_read(buf)
-e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-e0.record()
-step()
-e1.record()
-torch.cuda.synchronize()
-_lib.lib.nnk_as_prof_read(buf)
-ms = e0.elapsed_time(e1)
-n_cta = len(lens) * 2
-names = ["A wait pb_empty", "A wait input TMA", "A convert+assemble+publish", "-", "S wait pb_full", "S eliminate", "S wait scratch TMA", "S backward"]
-print("step %.3f ms; per-CTA average cycles (assemblers: per warp, 2 warps):" % ms)
+print("%s, per-CTA average cycles (assemblers: per warp, %d warps; solver: one warp)" % (torch.cuda.get_device_name(0), NA))
+print("  %-28s" % "" + "".join("%16s" % c[0] for c in cases))
+cols, times = [], []
+for _, fn, n_cta in cases:
+    for _ in range(3):
+        fn()
+    _lib.lib.nnk_as_prof_read(buf)  # synchronises and clears the counters
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    fn()
+    e1.record()
+    _lib.lib.nnk_as_prof_read(buf)
+    times.append(e0.elapsed_time(e1))
+    cols.append([buf[i] / (n_cta * (NA if i < 4 else 1)) for i in range(8)])
 for i, nm in enumerate(names):
-    if nm == "-":
-        continue
-    div = n_cta * (NA if i < 4 else 1)
-    print("  %-28s %10.0f" % (nm, buf[i] / div))
+    if nm:
+        print("  %-28s" % nm + "".join("%16.0f" % c[i] for c in cols))
+print("  %-28s" % "launch ms (instrumented)" + "".join("%16.3f" % t for t in times))
