@@ -264,6 +264,45 @@ int nnk_gmm_logprob(const nnk_gmm_t* gmm, const double* x, int64_t x_ld, int32_t
 int nnk_gmm_map(const nnk_gmm_t* gmm, const double* x, int64_t x_ld, int32_t T, const double* lp, int32_t mode, double* E,
                 double* Dv, int32_t* mix, void* stream);
 
+/* ---- GMM training: EM for full-covariance mixtures (sklearn.mixture.GaussianMixture.fit) ----------------
+ * N frames of D features (D <= 128), K components (K <= 128); all parameters are float64 device arrays,
+ * X is float32 (widened on load) or float64.  One EM iteration is
+ *   nnk_gmm_em_estep   : resp (N, K) = exp(log_resp) from weights / means / prec_chol, *lower_bound = mean of the
+ *                        per-frame log-likelihood (sklearn's _e_step + _compute_lower_bound);
+ *   nnk_gmm_em_mstep   : from resp: means (K, D), covariances (K, D, D) with reg_covar on the diagonal and, per
+ *                        weight_norm, weights = nk / N (0, sklearn's _initialize), nk / sum nk (1, its _m_step) or
+ *                        left alone (2);
+ *   nnk_gmm_em_factor  : factor != 0: prec_chol = L^-T with covariances = L L^T (sklearn's
+ *                        _compute_precision_cholesky); factor == 0: prec_chol is the caller's.  Either way it
+ *                        derives the per-component constants the next nnk_gmm_em_estep reads from the workspace,
+ *                        so it must run after any change of weights, means or prec_chol.
+ * A non-positive Cholesky pivot sets *status (zeroed by the caller) to 1 and leaves prec_chol undefined.
+ * Every reduction runs in a fixed order: identical inputs give bit-identical outputs.  All three take their
+ * scratch from `workspace` (>= nnk_gmm_em_workspace_bytes(N, D, K); 0 = unsupported sizes), which carries
+ * state from nnk_gmm_em_factor to nnk_gmm_em_estep and from nnk_gmm_em_mstep's statistics to its covariances. */
+typedef struct nnk_gmm_em_args {
+  const void* X;              /* device (N, x_ld) frames                                               */
+  int64_t N, x_ld;
+  int32_t dtype;              /* NNK_F32 / NNK_F64 of X                                                */
+  int32_t D, K;
+  int32_t weight_norm;        /* nnk_gmm_em_mstep: 0 = nk / N, 1 = nk / sum(nk), 2 = keep weights      */
+  int32_t factor;             /* nnk_gmm_em_factor: 1 = factor covariances, 0 = prec_chol given        */
+  double reg_covar;
+  double* resp;               /* device (N, K)                                                         */
+  double* weights;            /* device (K)                                                            */
+  double* means;              /* device (K, D)                                                         */
+  double* covariances;        /* device (K, D, D)                                                      */
+  double* prec_chol;          /* device (K, D, D) upper factors U, U U^T = covariance^-1               */
+  double* lower_bound;        /* device (1)                                                            */
+  int32_t* status;            /* device (1)                                                            */
+  void* workspace;
+  size_t workspace_bytes;
+} nnk_gmm_em_args_t;
+size_t nnk_gmm_em_workspace_bytes(int64_t N, int32_t D, int32_t K);
+int nnk_gmm_em_estep(const nnk_gmm_em_args_t* args, void* stream);
+int nnk_gmm_em_mstep(const nnk_gmm_em_args_t* args, void* stream);
+int nnk_gmm_em_factor(const nnk_gmm_em_args_t* args, void* stream);
+
 /* ---- sharded batches (SURVEY.md 8e; the reference has no multi-device path) ------------------------
  * Copies n_seg row segments (whole utterances) between two row-major device matrices:
  * dst[dst_row[s] + r, 0:cols] = src[src_row[s] + r, 0:cols] for r < len[s].  Used to bring the

@@ -66,6 +66,29 @@ class NnkGmm(ctypes.Structure):
     ]
 
 
+class NnkGmmEmArgs(ctypes.Structure):
+    _fields_ = [
+        ("X", ctypes.c_void_p),
+        ("N", ctypes.c_int64),
+        ("x_ld", ctypes.c_int64),
+        ("dtype", ctypes.c_int32),
+        ("D", ctypes.c_int32),
+        ("K", ctypes.c_int32),
+        ("weight_norm", ctypes.c_int32),
+        ("factor", ctypes.c_int32),
+        ("reg_covar", ctypes.c_double),
+        ("resp", ctypes.c_void_p),
+        ("weights", ctypes.c_void_p),
+        ("means", ctypes.c_void_p),
+        ("covariances", ctypes.c_void_p),
+        ("prec_chol", ctypes.c_void_p),
+        ("lower_bound", ctypes.c_void_p),
+        ("status", ctypes.c_void_p),
+        ("workspace", ctypes.c_void_p),
+        ("workspace_bytes", ctypes.c_size_t),
+    ]
+
+
 class NnkDtwArgs(ctypes.Structure):
     _fields_ = [
         ("X", ctypes.c_void_p),
@@ -104,6 +127,7 @@ EXPORTS = [
     "nnk_uv_band_profile", "nnk_uv_band_extract", "nnk_uv_apply", "nnk_uv_apply_toeplitz", "nnk_uv_apply_factored",
     "nnk_dtw_align", "nnk_dtw_workspace_bytes", "nnk_gather_rows", "nnk_trim_lengths", "nnk_delta_features",
     "nnk_metric_workspace_bytes", "nnk_frame_metric", "nnk_f0_metric", "nnk_segment_copy", "nnk_gmm_logprob", "nnk_gmm_map",
+    "nnk_gmm_em_workspace_bytes", "nnk_gmm_em_estep", "nnk_gmm_em_mstep", "nnk_gmm_em_factor",
     "nnk_peer_alloc", "nnk_peer_free", "nnk_peer_export", "nnk_peer_open", "nnk_peer_close", "nnk_peer_copy",
 ]
 
@@ -174,6 +198,11 @@ def _load():
     L.nnk_gmm_logprob.argtypes = [ctypes.POINTER(NnkGmm), vp, i64, i32, vp, vp]
     L.nnk_gmm_map.restype = ctypes.c_int
     L.nnk_gmm_map.argtypes = [ctypes.POINTER(NnkGmm), vp, i64, i32, vp, i32, vp, vp, vp, vp]
+    L.nnk_gmm_em_workspace_bytes.restype = ctypes.c_size_t
+    L.nnk_gmm_em_workspace_bytes.argtypes = [i64, i32, i32]
+    for name in ("nnk_gmm_em_estep", "nnk_gmm_em_mstep", "nnk_gmm_em_factor"):
+        getattr(L, name).restype = ctypes.c_int
+        getattr(L, name).argtypes = [ctypes.POINTER(NnkGmmEmArgs), vp]
     L.nnk_segment_copy.restype = ctypes.c_int
     L.nnk_segment_copy.argtypes = [vp, vp, i32, i64, i64, i64, vp, vp, vp, i32, i32, vp]
     return L

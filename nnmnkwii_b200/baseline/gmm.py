@@ -7,6 +7,9 @@ frame); here the mixture posteriors, the per-frame affine maps and the variances
 whole utterance -- or a whole batch of utterances -- on the GPU in float64 and handed to the MLPG
 kernels without leaving the device.
 
+``GaussianMixture`` fits the joint GMM itself: scikit-learn's estimator with its EM iterations run by the
+float64 kernels of csrc/nnk_gmm_em.cu (C ABI ``nnk_gmm_em_*``).
+
 The per-mixture matrices ``A[m] = covarYX[m] covarXX[m]^-1`` are formed once (the reference re-solves
 per frame, gmm.py:113-115, 231-233).  Posteriors, arg-max mixture, affine map and variances run in the
 float64 kernels of csrc/nnk_gmm.cu (C ABI ``nnk_gmm_logprob`` / ``nnk_gmm_map``): no (frames, mixtures,
@@ -16,6 +19,7 @@ import ctypes
 
 import numpy as np
 from scipy import linalg
+from sklearn.mixture import GaussianMixture as _SkGaussianMixture
 
 from ..paramgen import mlpg_batch
 
@@ -197,4 +201,287 @@ class MLPG(MLPGBase):
         return [y[off[i]:off[i + 1]] for i in range(len(lens))]
 
 
-__all__ = ["MLPGBase", "MLPG"]
+_EM_MAX_FEATURES = 128
+_EM_MAX_COMPONENTS = 128
+_ILL_DEFINED = ("Fitting the mixture model failed because some components have ill-defined empirical covariance "
+                "(for instance caused by singleton or collapsed samples). Try to decrease the number of components, "
+                "increase reg_covar, or scale the input data.")
+
+
+class _EmState(object):
+    """Device buffers of one fit: the frames, the responsibilities, the parameters, the workspace of
+    csrc/nnk_gmm_em.cu and the filled ``nnk_gmm_em_args_t``."""
+
+    def __init__(self, X, K, reg_covar):
+        import torch
+
+        from .. import _device as dev
+        from .. import _lib
+        self.X, self.device = X, X.device
+        N, D = X.shape
+        f64 = dict(dtype=torch.float64, device=X.device)
+        self.resp = torch.empty((N, K), **f64)
+        self.weights = torch.empty(K, **f64)
+        self.means = torch.empty((K, D), **f64)
+        self.covariances = torch.empty((K, D, D), **f64)
+        self.prec_chol = torch.empty((K, D, D), **f64)
+        self.lower_bound = torch.zeros(1, **f64)
+        self.status = torch.zeros(1, dtype=torch.int32, device=X.device)
+        nbytes = _lib.lib.nnk_gmm_em_workspace_bytes(N, D, K)
+        self.ws = dev.workspace(X.device, nbytes)
+        a = _lib.NnkGmmEmArgs()
+        a.X, a.N, a.x_ld, a.dtype, a.D, a.K = X.data_ptr(), N, X.stride(0), dev.torch_dtype_code(X.dtype), D, K
+        a.reg_covar = float(reg_covar)
+        for name in ("resp", "weights", "means", "covariances", "prec_chol", "lower_bound", "status"):
+            setattr(a, name, getattr(self, name).data_ptr())
+        a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws.numel()
+        self.args = a
+        self.stream = dev.current_stream_ptr(X.device)
+
+    def _call(self, name):
+        from .. import _lib
+        _lib.check(getattr(_lib.lib, name)(ctypes.byref(self.args), self.stream), name)
+
+    def estep(self):
+        self._call("nnk_gmm_em_estep")
+
+    def mstep(self, weight_norm):
+        self.args.weight_norm = weight_norm
+        self._call("nnk_gmm_em_mstep")
+
+    def factor(self, factor):
+        self.args.factor = int(factor)
+        self._call("nnk_gmm_em_factor")
+
+    def put(self, name, array):
+        import torch
+        getattr(self, name).copy_(torch.from_numpy(np.ascontiguousarray(array, dtype=np.float64)))
+
+    def check_status(self):
+        """Synchronises: raises sklearn's ValueError if a Cholesky pivot was not positive."""
+        if int(self.status.item()):
+            raise ValueError(_ILL_DEFINED)
+
+
+def _as_frames(X):
+    """(N, D) frames for the device: numpy / array-likes are validated like sklearn and uploaded; CUDA
+    tensors stay where they are.  Returns (device tensor, host float64 array or None)."""
+    import torch
+
+    from .. import _device as dev
+    from sklearn.utils import check_array
+    dev.require_cuda()
+    if isinstance(X, torch.Tensor) and X.is_cuda:
+        if X.ndim != 2:
+            raise ValueError("Expected 2D array, got %dD tensor instead" % X.ndim)
+        if X.dtype not in (torch.float32, torch.float64):
+            X = X.to(torch.float64)
+        if X.shape[0] < 2:
+            raise ValueError("Found array with %d sample(s) (shape=%s) while a minimum of 2 is required by "
+                             "GaussianMixture." % (X.shape[0], tuple(X.shape)))
+        if not bool(torch.isfinite(X).all()):
+            raise ValueError("Input X contains NaN or infinity.")
+        if X.shape[1] == 0 or X.stride(1) != 1 or X.stride(0) < X.shape[1]:
+            X = X.contiguous()
+        return X, None
+    if isinstance(X, torch.Tensor):
+        X = X.numpy()
+    Xh = check_array(X, dtype=[np.float64, np.float32], ensure_min_samples=2, estimator="GaussianMixture")
+    return torch.from_numpy(np.ascontiguousarray(Xh)).to(torch.device("cuda", torch.cuda.current_device())), Xh
+
+
+def _host_f64(t):
+    return t.detach().cpu().numpy().astype(np.float64, copy=True)
+
+
+class GaussianMixture(_SkGaussianMixture):
+    """``sklearn.mixture.GaussianMixture`` whose EM runs on the GPU (csrc/nnk_gmm_em.cu).
+
+    Same constructor, same fitted attributes (float64 NumPy arrays: ``weights_``, ``means_``,
+    ``covariances_``, ``precisions_cholesky_``, ``precisions_``, ``converged_``, ``n_iter_``,
+    ``lower_bound_``, ``lower_bounds_``), so scikit-learn's own ``predict``, ``predict_proba``, ``score``,
+    ``sample``, ``bic``, pickling and this module's ``MLPG`` / ``MLPGBase`` work on the result.
+
+    ``fit`` / ``fit_predict`` follow scikit-learn 1.9's ``BaseMixture.fit_predict`` step for step
+    (``n_init``, ``warm_start``, ``max_iter=0``, the ``tol`` stop, ``ConvergenceWarning``, the final E-step
+    whose arg-max gives the labels).  The initial responsibilities (``init_params`` in {"kmeans",
+    "k-means++", "random", "random_from_data"}) come from scikit-learn on the host with the same
+    ``random_state`` consumption, so the same seed gives the same start; the initial parameters are then
+    computed from them on the device.  Only ``covariance_type="full"`` is supported, with at most 128
+    features and 128 components.
+
+    ``X`` may be a NumPy array or a torch CUDA tensor, float32 or float64; a CUDA tensor is copied to
+    the host only when a host initialiser ("kmeans", "k-means++") needs it, and ``fit_predict`` then
+    returns the labels as a CUDA tensor.  The arithmetic is always float64.  Note that scikit-learn 1.9
+    itself fits float32 data in float32, so on float32 input the two differ; this class matches
+    scikit-learn run on the same data widened to float64 (to about 1e-10 relative: the summation order
+    of the reductions differs in the last bits).
+    """
+
+    def _check_sizes(self, D):
+        if self.covariance_type != "full":
+            raise NotImplementedError("nnmnkwii_b200 GaussianMixture fits covariance_type='full' only (got %r)"
+                                      % (self.covariance_type,))
+        if D > _EM_MAX_FEATURES:
+            raise ValueError("GaussianMixture on the GPU supports at most %d features (got %d)" % (_EM_MAX_FEATURES, D))
+        if self.n_components > _EM_MAX_COMPONENTS:
+            raise ValueError("GaussianMixture on the GPU supports at most %d components (got %d)"
+                             % (_EM_MAX_COMPONENTS, self.n_components))
+
+    def _initial_resp(self, n_samples, host_X, random_state):
+        """The responsibilities scikit-learn's ``_initialize_parameters`` derives, computed the same way
+        (same RandomState calls), in float64."""
+        from sklearn import cluster
+        from sklearn.cluster import kmeans_plusplus
+        K = self.n_components
+        resp = np.zeros((n_samples, K), dtype=np.float64)
+        if self.init_params == "kmeans":
+            label = cluster.KMeans(n_clusters=K, n_init=1, random_state=random_state).fit(host_X()).labels_
+            resp[np.arange(n_samples), label] = 1
+        elif self.init_params == "random":
+            resp = np.asarray(random_state.uniform(size=(n_samples, K)), dtype=np.float64)
+            resp /= np.sum(resp, axis=1)[:, np.newaxis]
+        elif self.init_params == "random_from_data":
+            indices = random_state.choice(n_samples, size=K, replace=False)
+            for col, index in enumerate(indices):
+                resp[index, col] = 1
+        elif self.init_params == "k-means++":
+            _, indices = kmeans_plusplus(host_X(), K, random_state=random_state)
+            resp[indices, np.arange(K)] = 1
+        return resp
+
+    def _device_initialize(self, st, n_samples, host_X, random_state):
+        """sklearn's ``GaussianMixture._initialize_parameters`` + ``_initialize``; returns whether the
+        device covariances are valid (they are not when ``precisions_init`` is given)."""
+        from sklearn.mixture._gaussian_mixture import _compute_precision_cholesky_from_precisions
+        from sklearn.utils._array_api import get_namespace
+        compute_resp = self.weights_init is None or self.means_init is None or self.precisions_init is None
+        if compute_resp:
+            st.put("resp", self._initial_resp(n_samples, host_X, random_state))
+            st.mstep(0 if self.weights_init is None else 2)
+        if self.weights_init is not None:
+            st.put("weights", self.weights_init)
+        if self.means_init is not None:
+            st.put("means", self.means_init)
+        if self.precisions_init is None:
+            st.factor(True)
+            st.check_status()
+            return True
+        prec = np.asarray(self.precisions_init, dtype=np.float64)
+        st.put("prec_chol", _compute_precision_cholesky_from_precisions(prec, self.covariance_type,
+                                                                         xp=get_namespace(prec)[0]))
+        st.factor(False)
+        return False
+
+    def fit_predict(self, X, y=None):
+        """Estimate the model parameters with EM on the GPU and return the labels of ``X``.
+
+        Mirrors ``sklearn.mixture.GaussianMixture.fit_predict`` (see the class docstring)."""
+        import warnings
+
+        import torch
+        from sklearn.exceptions import ConvergenceWarning
+        from sklearn.utils import check_random_state
+        from sklearn.utils._array_api import get_namespace
+
+        self._validate_params()
+        Xd, Xh = _as_frames(X)
+        n_samples, D = Xd.shape
+        self._check_sizes(D)
+        if n_samples < self.n_components:
+            raise ValueError("Expected n_samples >= n_components but got n_components = %d, n_samples = %d"
+                             % (self.n_components, n_samples))
+        self.n_features_in_ = D
+        if hasattr(self, "feature_names_in_"):
+            del self.feature_names_in_
+        shape_only = np.empty((0, D))  # sklearn's _check_parameters reads X.shape only
+        self._check_parameters(shape_only, xp=get_namespace(shape_only)[0])
+
+        cache = {}
+
+        def host_X():
+            if "X" not in cache:
+                cache["X"] = np.asarray(Xh, dtype=np.float64) if Xh is not None else _host_f64(Xd)
+            return cache["X"]
+
+        st = _EmState(Xd, self.n_components, self.reg_covar)
+        do_init = not (self.warm_start and hasattr(self, "converged_"))
+        n_init = self.n_init if do_init else 1
+        max_lower_bound = -np.inf
+        best_lower_bounds = []
+        best = None
+        self.converged_ = False
+        random_state = check_random_state(self.random_state)
+        cov_valid = False
+        if not do_init:  # warm start: continue from the fitted attributes
+            st.put("weights", self.weights_)
+            st.put("means", self.means_)
+            st.put("prec_chol", self.precisions_cholesky_)
+            if getattr(self, "covariances_", None) is not None:
+                st.put("covariances", self.covariances_)
+                cov_valid = True
+            st.factor(False)
+
+        def snapshot():
+            return (st.weights.clone(), st.means.clone(), st.covariances.clone() if cov_valid else None,
+                    st.prec_chol.clone())
+
+        for init in range(n_init):
+            self._print_verbose_msg_init_beg(init)
+            if do_init:
+                cov_valid = self._device_initialize(st, n_samples, host_X, random_state)
+            lower_bound = -np.inf if do_init else self.lower_bound_
+            current_lower_bounds = []
+            if self.max_iter == 0:
+                best = snapshot()
+                best_n_iter = 0
+            else:
+                converged = False
+                for n_iter in range(1, self.max_iter + 1):
+                    prev_lower_bound = lower_bound
+                    st.estep()
+                    st.mstep(1)
+                    st.factor(True)
+                    cov_valid = True
+                    st.check_status()
+                    lower_bound = float(st.lower_bound.item())
+                    current_lower_bounds.append(lower_bound)
+                    change = lower_bound - prev_lower_bound
+                    self._print_verbose_msg_iter_end(n_iter, change)
+                    if abs(change) < self.tol:
+                        converged = True
+                        break
+                self._print_verbose_msg_init_end(lower_bound, converged)
+                if lower_bound > max_lower_bound or max_lower_bound == -np.inf:
+                    max_lower_bound = lower_bound
+                    best = snapshot()
+                    best_n_iter = n_iter
+                    best_lower_bounds = current_lower_bounds
+                    self.converged_ = converged
+
+        if not self.converged_ and self.max_iter > 0:
+            warnings.warn("Best performing initialization did not converge. Try different init parameters, or "
+                          "increase max_iter, tol, or check for degenerate data.", ConvergenceWarning)
+
+        w, m, c, pc = best
+        # like sklearn's _get_parameters: without a covariance estimate (precisions_init, max_iter=0) the
+        # attribute keeps whatever it was, and is missing on a fresh estimator
+        cov_host = _host_f64(c) if c is not None else self.covariances_
+        self._set_parameters((_host_f64(w), _host_f64(m), cov_host, _host_f64(pc)))
+        self.n_iter_ = best_n_iter
+        self.lower_bound_ = max_lower_bound
+        self.lower_bounds_ = best_lower_bounds
+
+        # final E-step with the kept parameters: labels consistent with fit(X).predict(X)
+        st.weights.copy_(w)
+        st.means.copy_(m)
+        st.prec_chol.copy_(pc)
+        st.factor(False)
+        st.estep()
+        labels = torch.argmax(st.resp, dim=1)
+        if Xh is None:
+            return labels
+        return labels.cpu().numpy()
+
+
+__all__ = ["MLPGBase", "MLPG", "GaussianMixture"]

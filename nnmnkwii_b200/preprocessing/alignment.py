@@ -201,12 +201,20 @@ class IterativeDTWAligner(object):
     """Align feature matrices iteratively using GMM-based feature conversion (alignment.py:79-190).
 
     Per iteration: DTW of the converted source against the target (GPU), joint-GMM fit on the
-    aligned (zero padded) frames (scikit-learn, host, as in the reference), frame-wise GMM mapping
-    of the source.  Finally the ORIGINAL source is gathered along the last paths.
+    aligned (zero padded) frames, frame-wise GMM mapping of the source.  Finally the ORIGINAL source
+    is gathered along the last paths.
+
+    ``gmm`` (additive) picks who fits the joint GMM: ``"sklearn"`` (default, scikit-learn on the host,
+    as in the reference) or ``"device"`` (:class:`nnmnkwii_b200.baseline.gmm.GaussianMixture`, EM on the
+    GPU in float64, same ``n_components``, ``max_iter`` and ``random_state``).  The two are not
+    bit-identical: scikit-learn fits float32 frames in float32, and even on float64 frames the
+    summation order differs in the last bits.
     """
 
     def __init__(self, n_iter=3, dist=_default_dist, radius=1, max_iter_gmm=100, n_components_gmm=16, verbose=0,
-                 random_state=None):
+                 random_state=None, gmm="sklearn"):
+        if gmm not in ("sklearn", "device"):
+            raise ValueError("gmm must be 'sklearn' or 'device' (got %r)" % (gmm,))
         self.n_iter = n_iter
         self.dist = dist
         self.radius = radius
@@ -214,13 +222,17 @@ class IterativeDTWAligner(object):
         self.n_components_gmm = n_components_gmm
         self.verbose = verbose
         self.random_state = random_state  # additive: the reference leaves the GMM unseeded
+        self.gmm = gmm
 
     def transform(self, XY):
         import torch
-        from sklearn.mixture import GaussianMixture
 
         from . import trim_zeros_frames
         from ..baseline.gmm import MLPG
+        if self.gmm == "device":
+            from ..baseline.gmm import GaussianMixture
+        else:
+            from sklearn.mixture import GaussianMixture
 
         X, Y = XY
         assert X.ndim == 3 and Y.ndim == 3
