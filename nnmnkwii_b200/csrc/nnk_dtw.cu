@@ -979,9 +979,19 @@ static size_t dtw_fused_smem(int max_tx, int max_ty, int D) {
   const size_t groups = (size_t)(max_tx + 31) / 32;
   return sizeof(double) * ((size_t)max_ty * dp + (size_t)DTW_NBR * DTW_CW) + sizeof(int) * 2 * (groups + 1) + 16;
 }
-// the fused kernel serves frames of 8..39 dimensions whose Y series fits shared memory as float64
-static bool dtw_fused_ok(int max_tx, int max_ty, int D, size_t max_smem) {
-  return D >= 8 && D < 40 && dtw_fused_smem(max_tx, max_ty, D) <= max_smem;
+// the fused kernel serves frames of 8..39 dimensions whose Y series fits shared memory as float64;
+// max_dyn is the dynamic shared memory a block may request: the opt-in limit less the kernel's static part
+static bool dtw_fused_ok(int max_tx, int max_ty, int D, size_t max_dyn) {
+  return D >= 8 && D < 40 && dtw_fused_smem(max_tx, max_ty, D) <= max_dyn;
+}
+template <typename T>
+static const void* dtw_fused_fn(int nb8) {
+  switch (nb8) {
+    case 1: return (const void*)dtw_fused_kernel<T, 1>;
+    case 2: return (const void*)dtw_fused_kernel<T, 2>;
+    case 3: return (const void*)dtw_fused_kernel<T, 3>;
+    default: return (const void*)dtw_fused_kernel<T, 4>;
+  }
 }
 static bool dtw_force_two_pass() {
   static int v = -1;
@@ -1119,7 +1129,13 @@ extern "C" int nnk_dtw_align(const nnk_dtw_args_t* a, void* stream) {
   int dev = 0, max_smem = 0;
   NNK_CUDA_CHECK(cudaGetDevice(&dev));
   NNK_CUDA_CHECK(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  if (full && !dtw_force_two_pass() && dtw_fused_ok(a->max_tx, a->max_ty, a->D, (size_t)max_smem)) {
+  size_t fused_dyn = 0;  // dynamic shared memory the fused instance for this D may request
+  if (full && a->D >= 8 && a->D < 40) {
+    cudaFuncAttributes fa;
+    NNK_CUDA_CHECK(cudaFuncGetAttributes(&fa, a->dtype == NNK_F64 ? dtw_fused_fn<double>(a->D / 8) : dtw_fused_fn<float>(a->D / 8)));
+    fused_dyn = (size_t)max_smem > fa.sharedSizeBytes ? (size_t)max_smem - fa.sharedSizeBytes : 0;
+  }
+  if (full && !dtw_force_two_pass() && dtw_fused_ok(a->max_tx, a->max_ty, a->D, fused_dyn)) {
     DtwFusedParams f;
     f.X = a->X; f.Y = a->Y; f.x_pair_stride = a->x_pair_stride; f.y_pair_stride = a->y_pair_stride;
     f.x_ld = a->x_ld; f.y_ld = a->y_ld; f.D = a->D; f.len_x = a->len_x; f.len_y = a->len_y; f.order = a->order;

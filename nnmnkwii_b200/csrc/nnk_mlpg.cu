@@ -365,7 +365,8 @@ static int launch_mlpg(const nnk_mlpg_args_t& a, cudaStream_t st) {
   size_t items_cap = per_item ? a.workspace_bytes / per_item : 0;
   int utt_per_launch = (int)(items_cap / (size_t)p.n_groups);
   if (utt_per_launch < 1) { set_error("workspace too small: need >= %zu bytes", per_item * p.n_groups); return NNK_ERR_WORKSPACE; }
-  // forward solves go through the TMA-staged kernel unless the rows are too wide for its ring
+  // forward solves go through a staged kernel unless the rows are too wide for its rings: the warp-specialised
+  // kernel when as_geometry fits, else the single-warp TMA kernel when tma_geometry fits
   TmaGeom geom;
   size_t smem_bytes = 0;
   constexpr int ES = (int)sizeof(Tin);
@@ -381,8 +382,7 @@ static int launch_mlpg(const nnk_mlpg_args_t& a, cudaStream_t st) {
                       as_geometry<TT, NA, NSA, ND, TTB_AS, NSB_AS>(GRAD ? a.go_ld * 4 : a.in_ld * ES, a.var_ld * ES, GRAD, L,
                                                                    NT, as_geom, as_smem);
   const bool staged = !force_direct_loads() && (a.win.nw == NW) &&
-                      ((MODE == MODE_FWD && tma_geometry<TT, NS, TTB>(a.in_ld, a.var_ld, ES, NT, geom, smem_bytes)) ||
-                       (GRAD && paired));
+                      (paired || (MODE == MODE_FWD && tma_geometry<TT, NS, TTB>(a.in_ld, a.var_ld, ES, NT, geom, smem_bytes)));
   for (int u0 = 0; u0 < a.n_utt; u0 += utt_per_launch) {
     const int nu = (a.n_utt - u0 < utt_per_launch) ? a.n_utt - u0 : utt_per_launch;
     p.urank0 = u0;

@@ -1,0 +1,231 @@
+"""Host-side mirrors of the kernel-selection rules of the MLPG, UnitVarianceMLPG and DTW launchers, and a
+profiler helper that names the CUDA kernels a call launched.
+
+The mirrors restate, in Python, the size thresholds of the launchers (`pick_instance`, `as_geometry`,
+`tma_geometry` in csrc/nnk_mlpg*.cu*, `dtw_fused_smem` / `dtw_smem_bytes` / `dtw_fast_cells_bound` /
+`dtw_exact_chunk` in csrc/nnk_dtw.cu).  The tests of tests/test_kernel_variants_*_gpu.py pick their shapes
+from them and then assert, with the profiler, that the kernel the mirror predicts is the one that ran: a
+later change to a geometry function makes those tests fail instead of silently moving their coverage."""
+import re
+
+import numpy as np
+
+NNK_MAX_WIN = NNK_MAX_HALF = 4
+
+
+# ---- which kernels ran ---------------------------------------------------------------------------------------
+def profiled(fn, family=r"\b(mlpg|uv|dtw|fastdtw|trim_len)_\w*kernel\b", attempts=3):
+    """Run ``fn()`` under torch.profiler (CUDA activity) and return ``(result, error, kernel_names)``.
+
+    ``error`` is the exception ``fn`` raised (None if it returned).  CUPTI records the launches of the
+    ctypes library as well as torch's own, but now and then a profile comes back without the records of
+    a call; ``fn`` (every call here is repeatable) is then run again, at most ``attempts`` times, until the
+    profile holds a kernel of ``family``.  Fails (never skips) when no such name was collected."""
+    import torch
+    from torch.autograd import DeviceType
+    from torch.profiler import ProfilerActivity, profile
+
+    for _ in range(attempts):
+        torch.cuda.synchronize()
+        out = err = None
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            try:
+                out = fn()
+            except Exception as e:  # noqa: BLE001 -- handed back to the caller
+                err = e
+            torch.cuda.synchronize()
+        names = [e.name for e in prof.events() if e.device_type == DeviceType.CUDA]
+        if launched(names, family):
+            return out, err, names
+    raise AssertionError("the profiler collected no kernel names of %r in %d attempts: %s" % (family, attempts, names))
+
+
+def launched(names, pattern):
+    """Names matching the regular expression ``pattern``."""
+    rx = re.compile(pattern)
+    return [n for n in names if rx.search(n)]
+
+
+# ---- MLPG ------------------------------------------------------------------------------------------------------
+def pick_instance(windows):
+    """(NW, L, U) of the template instance `pick_instance` (csrc/nnk_mlpg.cu) chooses."""
+    nw = len(windows)
+    L = max(int(w[0]) for w in windows)
+    U = max(int(w[1]) for w in windows)
+    assert 1 <= nw <= NNK_MAX_WIN and L <= NNK_MAX_HALF and U <= NNK_MAX_HALF
+    if nw == 1 and L == 0 and U == 0:
+        return 1, 0, 0
+    if nw <= 3 and L <= 1 and U <= 1:
+        return 3, 1, 1
+    if nw <= 3 and L <= 2 and U <= 2:
+        return 3, 2, 2
+    return NNK_MAX_WIN, NNK_MAX_HALF, NNK_MAX_HALF
+
+
+def _r16(n):
+    return (n + 32 + 15) // 16 * 16
+
+
+def as_geometry_fits(row_bytes_m, row_bytes_v, grad, half_l, nt):
+    """`as_geometry<TT=4, NA=3, NSA=1, ND=6, TTB=8, NSB=grad ? 4 : 8>` of csrc/nnk_mlpg_as.cuh."""
+    TT, NA, NSA, ND, TTB = 4, 3, 1, 6, 8
+    NSB = 4 if grad else 8
+    ld = max(row_bytes_m, row_bytes_v)
+    sb_in = _r16((TT + nt - 1) * ld)
+    sb_ws = TTB * nt * 32 * 8
+    sb_var = _r16((TTB + half_l) * row_bytes_v) if grad else 0
+    ring_a = (NSA * 2 * sb_in + 127) // 128 * 128
+    pbb = ND * TT * (nt + 1) * 32 * 8
+    bwd = NSB * (sb_ws + sb_var)
+    if NA * ring_a + pbb < bwd:
+        ring_a = ((bwd - pbb) // NA + 127) // 128 * 128
+    return 512 + NA * ring_a + pbb <= 100 * 1024
+
+
+def tma_geometry_fits(in_ld, var_ld, es, nt):
+    """`tma_geometry<TT=4, NS=4, TTB=4>` of csrc/nnk_mlpg_tma.cuh."""
+    TT, NS, TTB = 4, 4, 4
+    ld = max(in_ld, var_ld)
+    sb_in = _r16(TT * ld * es)
+    sb_ws = TTB * nt * 32 * 8
+    return 128 + max(NS * 2 * sb_in, NS * sb_ws) <= 40 * 1024
+
+
+AS, TMA, DIRECT = "mlpg_fwd_as_kernel", "mlpg_fwd_tma_kernel", "mlpg_kernel"
+
+
+def mlpg_kernel_for(mode, windows, D, es, var_global=False, go_ld=None, go_f64=False):
+    """Name of the kernel `launch_mlpg` runs for a single-stream call: mode "fwd" (in_ld = D) or "grad"
+    (go_ld = columns of grad_output, static_dim for paramgen.mlpg_grad)."""
+    NW, L, U = pick_instance(windows)
+    nt = L + U + 1
+    var_ld = 0 if var_global else D
+    if mode == "fwd":
+        paired = nt <= 5 and as_geometry_fits(D * es, var_ld * es, False, L, nt)
+        staged = len(windows) == NW and (paired or tma_geometry_fits(D, var_ld, es, nt))
+    else:
+        go_ld = D // len(windows) if go_ld is None else go_ld
+        paired = (not go_f64) and nt <= 5 and as_geometry_fits(go_ld * 4, var_ld * es, True, L, nt)
+        staged = len(windows) == NW and paired
+    if not staged:
+        return DIRECT
+    return AS if paired else TMA
+
+
+def staged_limit(mode, windows, es, var_global=False):
+    """Widest row D (columns of the means) that still runs a staged kernel; D + 1 runs `mlpg_kernel`."""
+    last = None
+    for D in range(len(windows), 4097):
+        if mlpg_kernel_for(mode, windows, D, es, var_global) != DIRECT:
+            last = D
+        elif last is not None:
+            return last
+    raise AssertionError("no staged-kernel limit below 4096 columns")
+
+
+# ---- DTW -------------------------------------------------------------------------------------------------------
+DTW_FR, DTW_CW = 512, 128
+DTW_NBR = DTW_FR // 32 + 1
+FD_PD, FD_MAXW = 7, 24
+
+
+def max_smem_optin(device=0):
+    import torch
+    return int(torch.cuda.get_device_properties(device).shared_memory_per_block_optin)
+
+
+def _dtw_dp(D):
+    dp = (D + 1) & ~1
+    if ((dp >> 1) & 1) == 0:
+        dp += 2
+    return dp
+
+
+def dtw_fused_smem(max_tx, max_ty, D):
+    groups = (max_tx + 31) // 32
+    return 8 * (max_ty * _dtw_dp(D) + DTW_NBR * DTW_CW) + 4 * 2 * (groups + 1) + 16
+
+
+# static shared memory of every dtw_fused_kernel instance (ptxas -v: 16 bytes, the back-track's `s_n`): a
+# block may request the opt-in limit less this much dynamic shared memory
+DTW_FUSED_STATIC_SMEM = 16
+
+
+def dtw_fused_ok(max_tx, max_ty, D, max_smem):
+    return 8 <= D < 40 and dtw_fused_smem(max_tx, max_ty, D) <= max_smem - DTW_FUSED_STATIC_SMEM
+
+
+def dtw_fused_ty_limit(max_tx, D, max_smem):
+    """Largest padded Ty the fused exact kernel takes at this D."""
+    fixed = dtw_fused_smem(max_tx, 0, D)
+    return (max_smem - DTW_FUSED_STATIC_SMEM - fixed) // (8 * _dtw_dp(D))
+
+
+def dtw_dp_bucket(max_tx):
+    """MC of the `dtw_dp_kernel<MC>` the two-pass exact path launches."""
+    mc = (max_tx + 255) // 256
+    return 4 if mc <= 4 else 8 if mc <= 8 else 16
+
+
+def dtw_exact_chunk(n_pairs, max_tx, max_ty):
+    per = max_tx * max_ty * 9
+    return max(1, min(n_pairs, (2 << 30) // per))
+
+
+def _dtw_smem_bytes(max_tx, bp_cap):
+    return 8 * (FD_PD + 1) * 32 + 4 * (max_tx * 2 + (max_tx + 1) + 2 * (max_tx // 2 + 1)) + bp_cap + 16
+
+
+def fast_cells_bound(max_tx, max_ty, radius):
+    r2 = 2 * radius + 1
+    return 4 * r2 * ((max_tx + max_ty) // 2 + r2 + 2) + 64
+
+
+def fastdtw_caps(max_tx, max_ty, radius, max_smem):
+    """(smem_bp_cap, cost_cap) of `nnk_dtw_align`'s FastDTW launch."""
+    bound = fast_cells_bound(max_tx, max_ty, radius)
+    if _dtw_smem_bytes(max_tx, bound) > max_smem // 4:
+        base = _dtw_smem_bytes(max_tx, 0)
+        assert base + 1024 <= max_smem
+        bound = max_smem // 4 - base if max_smem // 4 > base + 1024 else 1024
+    return bound, fast_cells_bound(max_tx, max_ty, radius)
+
+
+def fastdtw_levels(x, y, radius, kind):
+    """Per level of FastDTW, finest first: (window cells, most rows active on one anti-diagonal).
+
+    Windows come from `oracle.expand_window` of the oracle's path one level coarser, exactly as
+    `fastdtw_kernel` builds them; the sum of the cells is what the kernel reports as `cells`."""
+    import oracle
+    xs, ys = [np.asarray(x, np.float64)], [np.asarray(y, np.float64)]
+    while len(xs[-1]) >= radius + 2 and len(ys[-1]) >= radius + 2:
+        a, b = xs[-1], ys[-1]  # __reduce_by_half
+        na, nb = len(a) // 2, len(b) // 2
+        xs.append((a[0:2 * na:2] + a[1:2 * na:2]) / 2)
+        ys.append((b[0:2 * nb:2] + b[1:2 * nb:2]) / 2)
+    out = []
+    for lev in range(len(xs)):
+        Tx, Ty = len(xs[lev]), len(ys[lev])
+        if lev == len(xs) - 1:
+            lo, hi = np.zeros(Tx, np.int64), np.full(Tx, Ty, np.int64)
+        else:
+            _, pi, pj, _ = oracle.fastdtw(xs[lev + 1], ys[lev + 1], radius=radius, kind=kind)
+            lo, hi = oracle.expand_window(pi, pj, Tx, Ty, radius)
+            lo, hi = lo.astype(np.int64), hi.astype(np.int64)
+        ncells = int(np.maximum(0, hi - lo).sum())
+        # the kernel's count: row i enters on anti-diagonal k = i + lo[i]; the lowest row still active
+        # there is the first r with r + hi[r] > k (binary search over [0, i])
+        end = np.arange(Tx) + hi
+        wmax = 0
+        for i in range(Tx):
+            k = i + lo[i]
+            a, b = 0, i
+            while a < b:
+                m = (a + b) >> 1
+                if end[m] > k:
+                    b = m
+                else:
+                    a = m + 1
+            wmax = max(wmax, i - a + 1)
+        out.append((ncells, wmax))
+    return out
