@@ -45,8 +45,8 @@ def test_gmm_kernels_at_voice_conversion_size():
     """The fused GMM kernels (log-posteriors, arg-max map, posterior mean) at a realistic size --
     32 mixtures over 72-dim (static + delta) frames, two dims that do not fill the last lane group --
     against the reference's own per-frame algebra written out in NumPy float64 (gmm.py:97-121, 219-244)."""
-    from scipy.special import logsumexp
     from nnmnkwii_b200.baseline.gmm import MLPG, MLPGBase
+    from test_kernel_variants_gmm_gpu import gmm_map_reference
     for M, dim, T in ((32, 72, 333), (3, 5, 17), (7, 96, 40)):
         rng = np.random.default_rng(M * 1000 + dim)
         A = rng.standard_normal((M, 2 * dim, 2 * dim)) / np.sqrt(2 * dim)
@@ -56,17 +56,7 @@ def test_gmm_kernels_at_voice_conversion_size():
                                     covariance_type="full")
         src = rng.standard_normal((T, dim))
         base = MLPGBase(gmm)
-        # reference algebra, frame by frame
-        lp = np.empty((T, M))
-        Em = np.empty((T, M, dim))
-        for m in range(M):
-            d = src - base.src_means[m]
-            sol = np.linalg.solve(base.covarXX[m], d.T).T
-            lp[:, m] = (np.log(base.weights[m]) - 0.5 * (d * sol).sum(1) - 0.5 * np.linalg.slogdet(base.covarXX[m])[1]
-                        - 0.5 * dim * np.log(2 * np.pi))
-            Em[:, m] = base.tgt_means[m] + sol @ base.covarYX[m].T
-        post = np.exp(lp - logsumexp(lp, axis=1, keepdims=True))
-        want = np.einsum("tm,tmi->ti", post, Em)
+        lp, Em, want, Dm = gmm_map_reference(base, src)  # reference algebra, frame by frame
         assert rel_err(base.transform(src), want) < 1e-9
         conv = MLPG(gmm, windows=[(0, 0, np.array([1.0]))] * 1)
         conv.static_dim = dim // 2  # force the E / D path (feature_dim != static_dim)
@@ -75,7 +65,5 @@ def test_gmm_kernels_at_voice_conversion_size():
         E, Dv = conv._means_vars(x, c)
         mix = lp.argmax(1)
         assert rel_err(E.cpu().numpy(), Em[np.arange(T), mix]) < 1e-9
-        Dm = np.stack([np.diag(base.covarYY[m]) - np.diag(base.covarYX[m]) / np.diag(base.covarXX[m]) * np.diag(base.covarXY[m])
-                       for m in range(M)])
         assert np.array_equal(Dv.cpu().numpy(), Dm[mix])
         del torch

@@ -1,9 +1,10 @@
-"""Host-side mirrors of the kernel-selection rules of the MLPG, UnitVarianceMLPG and DTW launchers, and a
-profiler helper that names the CUDA kernels a call launched.
+"""Host-side mirrors of the kernel-selection rules of the MLPG, UnitVarianceMLPG, DTW and GMM launchers, and
+a profiler helper that names the CUDA kernels a call launched.
 
 The mirrors restate, in Python, the size thresholds of the launchers (`pick_instance`, `as_geometry`,
 `tma_geometry` in csrc/nnk_mlpg*.cu*, `dtw_fused_smem` / `dtw_smem_bytes` / `dtw_fast_cells_bound` /
-`dtw_exact_chunk` in csrc/nnk_dtw.cu).  The tests of tests/test_kernel_variants_*_gpu.py pick their shapes
+`dtw_exact_chunk` in csrc/nnk_dtw.cu, `em_layout` / `estep_d` / `mstep_d` in csrc/nnk_gmm_em.cu and the
+launch sizes of csrc/nnk_gmm.cu).  The tests of tests/test_kernel_variants_*_gpu.py pick their shapes
 from them and then assert, with the profiler, that the kernel the mirror predicts is the one that ran: a
 later change to a geometry function makes those tests fail instead of silently moving their coverage."""
 import re
@@ -14,13 +15,19 @@ NNK_MAX_WIN = NNK_MAX_HALF = 4
 
 
 # ---- which kernels ran ---------------------------------------------------------------------------------------
-def profiled(fn, family=r"\b(mlpg|uv|dtw|fastdtw|trim_len)_\w*kernel\b", attempts=3):
+def profiled(fn, family=r"\b(mlpg|uv|dtw|fastdtw|trim_len)_\w*kernel\b", attempts=8):
     """Run ``fn()`` under torch.profiler (CUDA activity) and return ``(result, error, kernel_names)``.
 
     ``error`` is the exception ``fn`` raised (None if it returned).  CUPTI records the launches of the
     ctypes library as well as torch's own, but now and then a profile comes back without the records of
     a call; ``fn`` (every call here is repeatable) is then run again, at most ``attempts`` times, until the
-    profile holds a kernel of ``family``.  Fails (never skips) when no such name was collected."""
+    profile holds a kernel of ``family``.  Fails (never skips) when no such name was collected.
+
+    The losses come in bursts: on an H100 one call lost its kernel record in 3 of 20 consecutive profiles,
+    while 180 profiles of the same call in a fresh process lost none.  At that rate three attempts still
+    miss about once in 300 calls, and the suite makes hundreds; eight miss about once in 4 million.
+    Pass a ``family`` that names the kernel the caller asserts on, so that a profile that kept only the
+    call's other kernels is repeated too."""
     import torch
     from torch.autograd import DeviceType
     from torch.profiler import ProfilerActivity, profile
@@ -229,3 +236,73 @@ def fastdtw_levels(x, y, radius, kind):
             wmax = max(wmax, i - a + 1)
         out.append((ncells, wmax))
     return out
+
+
+# ---- GMM EM (csrc/nnk_gmm_em.cu) -------------------------------------------------------------------------------
+EM_MAX_D = EM_MAX_K = 128
+EM_ES_FT = 32          # E-step: frames per block (ES_FPW 8 x ES_WARPS 4)
+EM_ST_CHUNK = 1024     # statistics: frames per block
+EM_ST_SUB = EM_CV_SUB = 32
+K_NUM_SMS = 132
+EM_CV_TARGET_BLOCKS = 4 * K_NUM_SMS
+
+
+def em_estep_epl(D):
+    """EPL of the `em_estep_kernel<EPL, T>` that `estep_d` launches."""
+    assert 1 <= D <= EM_MAX_D
+    return min(4, (D + 31) // 32)
+
+
+def em_cov_ti(D):
+    """TI of the `em_cov_kernel<TI, T>` that `mstep_d` launches."""
+    assert 1 <= D <= EM_MAX_D
+    return min(8, (D + 15) // 16)
+
+
+def _round4(v):
+    return (v + 3) & ~3
+
+
+def em_layout(N, D, K):
+    """`em_layout`: tile / chunk counts and the workspace size `total` (in doubles)."""
+    n_tiles = (N + EM_ES_FT - 1) // EM_ES_FT
+    n_stat = (N + EM_ST_CHUNK - 1) // EM_ST_CHUNK
+    n_cov = (EM_CV_TARGET_BLOCKS + K - 1) // K
+    n_cov = max(1, min(n_cov, (N + 255) // 256))  # at least 256 frames per chunk
+    cov_chunk = ((N + n_cov - 1) // n_cov + EM_CV_SUB - 1) // EM_CV_SUB * EM_CV_SUB
+    n_cov = (N + cov_chunk - 1) // cov_chunk
+    # lse, stat, nk, cov, logw, logdet, muu
+    total = (_round4(n_tiles) + _round4(n_stat * K * (D + 1)) + _round4(K) + _round4(n_cov * K * D * D)
+             + _round4(K) + _round4(K) + _round4(K * D))
+    return dict(n_tiles=n_tiles, n_stat=n_stat, n_cov=n_cov, cov_chunk=cov_chunk, total=total)
+
+
+def em_estep_smem(D, K):
+    return 8 * (EM_ES_FT * D + EM_ES_FT * K + EM_ES_FT)
+
+
+def em_stats_smem(D, K):
+    return 8 * (K * (D + 1) + EM_ST_SUB * K + EM_ST_SUB * D)
+
+
+def em_cov_smem(D):
+    return 8 * (2 * EM_CV_SUB * 16 * em_cov_ti(D) + D)
+
+
+def em_factor_smem(D):
+    return 8 * (D * (D + 1) + D)
+
+
+# ---- GMM mapping (csrc/nnk_gmm.cu) -----------------------------------------------------------------------------
+GMM_FT = 16            # frames per block of gmm_logprob_kernel / gmm_posterior_kernel
+GMM_SELECT_FT = 4      # frames (one per warp) per block of gmm_select_kernel
+GMM_MAX_D = 96         # 32 lanes x GMM_EPL 3 outputs
+GMM_MAX_M = 65535      # grid.y of gmm_logprob_kernel
+
+
+def gmm_logprob_smem(D):
+    return 8 * (D * D + GMM_FT * D)
+
+
+def gmm_posterior_smem(D):
+    return 8 * (D * D + GMM_FT * D + 2 * GMM_FT)
