@@ -24,10 +24,21 @@
 #include "nnk_mlpg_tma.cuh"
 #include "nnk_mlpg_as.cuh"
 
-// assembler warps per chain group and TMA stages per assembler (A/B builds: -DNNK_AS_NA=2 -DNNK_AS_NSA=2)
+// assembler warps per chain group and TMA stages per assembler of the one-group kernel (A/B builds:
+// -DNNK_AS_NA=2 -DNNK_AS_NSA1=2)
 #ifndef NNK_AS_NA
 #define NNK_AS_NA 3
-#define NNK_AS_NSA 1
+#endif
+#ifndef NNK_AS_NSA1
+#define NNK_AS_NSA1 1
+#endif
+// chain groups per CTA of float32 forward solves (-DNNK_AS_G=1 keeps one group per CTA everywhere) and TMA
+// stages per assembler pair of the two-group kernel (-DNNK_AS_NSA=1 for A/B builds)
+#ifndef NNK_AS_G
+#define NNK_AS_G 2
+#endif
+#ifndef NNK_AS_NSA
+#define NNK_AS_NSA 2
 #endif
 // depth of the band-row (PB) ring in tiles; must be >= the producers' tile stride (see nnk_mlpg_as.cuh)
 #ifndef NNK_AS_ND
@@ -372,7 +383,7 @@ static int launch_mlpg(const nnk_mlpg_args_t& a, cudaStream_t st) {
   constexpr int ES = (int)sizeof(Tin);
   constexpr bool GRAD = (MODE == MODE_GRAD);
   constexpr bool GRAD_MODE = GRAD;
-  constexpr int TT = 4, NS = 4, TTB = 4, NA = NNK_AS_NA, NSA = NNK_AS_NSA, ND = NNK_AS_ND;
+  constexpr int TT = 4, NS = 4, TTB = 4, NA = NNK_AS_NA, NSA = NNK_AS_NSA1, ND = NNK_AS_ND;
   // backward-sweep scratch ring of the paired kernel: 64 frames in flight (32 when the variance rows ride along)
   constexpr int TTB_AS = 8, NSB_AS = GRAD_MODE ? 4 : 8;
   AsGeom as_geom;
@@ -381,6 +392,16 @@ static int launch_mlpg(const nnk_mlpg_args_t& a, cudaStream_t st) {
   const bool paired = (MODE == MODE_FWD || (GRAD && !a.go_f64)) && !force_single_warp() && (NT <= 5) &&
                       as_geometry<TT, NA, NSA, ND, TTB_AS, NSB_AS>(GRAD ? a.go_ld * 4 : a.in_ld * ES, a.var_ld * ES, GRAD, L,
                                                                    NT, as_geom, as_smem);
+  // float32 forward solves with two or more chain groups: one CTA per pair of groups (an odd last group runs
+  // with an empty second half), when that geometry fits two CTAs per SM.  Float64 rows and the gradient keep
+  // one group per CTA, and so do band depths S > 2: at the 128 registers of two 256-thread CTAs per SM the
+  // S = 4 assembler spills.
+  constexpr bool CAN_G2 = (NNK_AS_G >= 2) && (MODE == MODE_FWD) && (ES == 4) && (NT <= 3);
+  AsGeom as_geom2;
+  size_t as_smem2 = 0;
+  const bool grouped = CAN_G2 && paired && p.n_groups >= 2 &&
+                       as_geometry<TT, NA, NNK_AS_NSA, ND, TTB_AS, NSB_AS, 2>(a.in_ld * ES, a.var_ld * ES, false, L, NT,
+                                                                             as_geom2, as_smem2);
   const bool staged = !force_direct_loads() && (a.win.nw == NW) &&
                       (paired || (MODE == MODE_FWD && tma_geometry<TT, NS, TTB>(a.in_ld, a.var_ld, ES, NT, geom, smem_bytes)));
   for (int u0 = 0; u0 < a.n_utt; u0 += utt_per_launch) {
@@ -392,10 +413,24 @@ static int launch_mlpg(const nnk_mlpg_args_t& a, cudaStream_t st) {
       const bool varg = (a.var_ld == 0);
       const int grid = nu * p.n_groups;
       constexpr int AS_MODE = GRAD ? MODE_GRAD : MODE_FWD;  // MODE_SOLVE never gets here
-      if (paired) {
+      if (grouped) {
+        if constexpr (CAN_G2) {
+#define NNK_LAUNCH_AS2(STDV, VARGV)                                                                                  \
+  do {                                                                                                              \
+    auto kern = mlpg_fwd_as_kernel<Tin, NW, L, U, STDV, VARGV, AS_MODE, TT, NA, NNK_AS_NSA, ND, TTB_AS, NSB_AS, 2>; \
+    NNK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)as_smem2));        \
+    kern<<<nu * ((p.n_groups + 1) / 2), 2 * 32 * (NA + 1), as_smem2, st>>>(p, as_geom2);                            \
+  } while (0)
+          if (stdw && !varg) NNK_LAUNCH_AS2(CAN_STD, false);
+          else if (stdw && varg) NNK_LAUNCH_AS2(CAN_STD, true);
+          else if (!varg) NNK_LAUNCH_AS2(false, false);
+          else NNK_LAUNCH_AS2(false, true);
+#undef NNK_LAUNCH_AS2
+        }
+      } else if (paired) {
 #define NNK_LAUNCH_AS(STDV, VARGV)                                                                                   \
   do {                                                                                                              \
-    auto kern = mlpg_fwd_as_kernel<Tin, NW, L, U, STDV, VARGV, AS_MODE, TT, NA, NSA, ND, TTB_AS, NSB_AS>;                  \
+    auto kern = mlpg_fwd_as_kernel<Tin, NW, L, U, STDV, VARGV, AS_MODE, TT, NA, NSA, ND, TTB_AS, NSB_AS, 1>;               \
     NNK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)as_smem));         \
     kern<<<grid, 32 * (NA + 1), as_smem, st>>>(p, as_geom);                                                         \
   } while (0)
@@ -463,11 +498,11 @@ extern "C" size_t nnk_mlpg_workspace_bytes(int32_t n_utt, int32_t n_chain, int32
 }
 
 #ifdef NNK_AS_PROF
-// debug builds only: read and clear the phase counters of mlpg_fwd_as_kernel (synchronises)
-extern "C" int nnk_as_prof_read(unsigned long long* out16) {
+// debug builds only: read and clear the NNK_AS_PROF_SLOTS phase counters of mlpg_fwd_as_kernel (synchronises)
+extern "C" int nnk_as_prof_read(unsigned long long* out) {
   cudaDeviceSynchronize();
-  cudaMemcpyFromSymbol(out16, nnk::g_as_prof, sizeof(unsigned long long) * 16);
-  unsigned long long z[16] = {0};
+  cudaMemcpyFromSymbol(out, nnk::g_as_prof, sizeof(unsigned long long) * NNK_AS_PROF_SLOTS);
+  unsigned long long z[NNK_AS_PROF_SLOTS] = {0};
   cudaMemcpyToSymbol(nnk::g_as_prof, z, sizeof(z));
   return 0;
 }

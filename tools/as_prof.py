@@ -20,7 +20,6 @@ from nnmnkwii_b200 import _device as dev, _lib, paramgen as G  # noqa: E402
 
 if not hasattr(_lib.lib, "nnk_as_prof_read"):
     sys.exit("%s was built without -DNNK_AS_PROF" % _lib.LIB_PATH)
-NA = int(os.environ.get("NA", "3"))  # assembler warps per CTA of the build (NNK_AS_NA)
 device = torch.device("cuda", 0)
 wc = _lib.make_windows(bench.WINDOWS)
 
@@ -58,16 +57,15 @@ def t1000(mode, rhs, o, out_ld):
                  dtype_code=_lib.NNK_F32, go_f64=0, n_utt=B2, device=device, check=False)
 
 
-cases = (("configs[1]", cfg2, len(lens) * 2),
-         ("T1000 forward", lambda: t1000("fwd", None, y2, sd2), B2 * 2),
-         ("T1000 gradient", lambda: t1000("grad", go2, g2, 3 * sd2), B2 * 2))
-names = ["A wait pb_empty", "A wait input TMA", "A convert+assemble+publish", None,
-         "S wait pb_full", "S eliminate", "S wait scratch TMA", "S backward"]
-buf = (ctypes.c_ulonglong * 16)()
-print("%s, per-CTA average cycles (assemblers: per warp, %d warps; solver: one warp)" % (torch.cuda.get_device_name(0), NA))
-print("  %-28s" % "" + "".join("%16s" % c[0] for c in cases))
-cols, times = [], []
-for _, fn, n_cta in cases:
+cases = (("configs[1]", cfg2), ("T1000 forward", lambda: t1000("fwd", None, y2, sd2)),
+         ("T1000 gradient", lambda: t1000("grad", go2, g2, 3 * sd2)))
+A_PH = ["wait pb_empty", "wait input TMA", "convert+assemble+publish"]
+S_PH = ["wait pb_full", "eliminate", "wait scratch TMA", "backward"]
+SLOTS = 40  # NNK_AS_PROF_SLOTS: [role * 4 + phase], [32] CTAs, [33] G, [34] NA
+buf = (ctypes.c_ulonglong * SLOTS)()
+print("%s, per-CTA average cycles of each warp (assembler q.h: tile ownership q of chain group h of the CTA)"
+      % torch.cuda.get_device_name(0))
+for title, fn in cases:
     for _ in range(3):
         fn()
     _lib.lib.nnk_as_prof_read(buf)  # synchronises and clears the counters
@@ -76,9 +74,11 @@ for _, fn, n_cta in cases:
     fn()
     e1.record()
     _lib.lib.nnk_as_prof_read(buf)
-    times.append(e0.elapsed_time(e1))
-    cols.append([buf[i] / (n_cta * (NA if i < 4 else 1)) for i in range(8)])
-for i, nm in enumerate(names):
-    if nm:
-        print("  %-28s" % nm + "".join("%16.0f" % c[i] for c in cols))
-print("  %-28s" % "launch ms (instrumented)" + "".join("%16.3f" % t for t in times))
+    n_cta, G, na = int(buf[32]), int(buf[33]), int(buf[34])
+    print("%s: G = %d, NA = %d, %d CTAs, launch %.3f ms (instrumented)" % (title, G, na, n_cta, e0.elapsed_time(e1)))
+    for i, ph in enumerate(A_PH):
+        per = [buf[(h * na + q) * 4 + i] / n_cta for h in range(G) for q in range(na)]
+        print("  A %-26s" % ph + "".join("%10.0f" % x for x in per) + "   mean %.0f" % (sum(per) / len(per)))
+    for i, ph in enumerate(S_PH):
+        per = [buf[(G * na + h) * 4 + i] / n_cta for h in range(G)]
+        print("  S %-26s" % ph + "".join("%10.0f" % x for x in per))
