@@ -303,6 +303,22 @@ int nnk_gmm_em_estep(const nnk_gmm_em_args_t* args, void* stream);
 int nnk_gmm_em_mstep(const nnk_gmm_em_args_t* args, void* stream);
 int nnk_gmm_em_factor(const nnk_gmm_em_args_t* args, void* stream);
 
+/* ---- Merlin post-filter (postfilters/__init__.py:7-62) ------------------------------------------------
+ * Per frame c of a flat (N, D) batch (rows at stride ld, float32 or float64), weight w (D doubles on the
+ * device): out = w * c with out[0] += log(r0(c) / r0(w * c)) / 2, where r0 = c2acr(freqt(., order, -alpha),
+ * 0, fftlen) -- the reference's freqt / c2acr / mc2b / b2mc chain collapsed (mc2b and b2mc are exact
+ * inverses outside coefficient 0).  r0 runs on a float64 basis B = Cos F ((fftlen/2 + 1) x D) that
+ * nnk_postfilter_basis builds once per (alpha, D, order, fftlen) into `basis` (device, basis_elems =
+ * nnk_postfilter_basis_elems(D, fftlen) doubles, opaque order).  Arithmetic is float64, out has the dtype
+ * of mgc.  fftlen must be a power of two (SPTK's fftr), 0 <= order <= fftlen - 1 (c2acr's buffer);
+ * D > 128 or fftlen > 8192 is NNK_ERR_UNSUPPORTED.  nnk_postfilter_basis_elems returns 0 for such sizes. */
+int64_t nnk_postfilter_basis_elems(int32_t D, int32_t fftlen);
+int nnk_postfilter_basis(double alpha, int32_t D, int32_t order, int32_t fftlen, double* basis, int64_t basis_elems,
+                         void* stream);
+int nnk_postfilter_apply(const void* mgc, int32_t dtype, int64_t N, int32_t D, int64_t ld, const double* weight,
+                         int32_t fftlen, const double* basis, int64_t basis_elems, void* out, int64_t out_ld,
+                         void* stream);
+
 /* ---- sharded batches (SURVEY.md 8e; the reference has no multi-device path) ------------------------
  * Copies n_seg row segments (whole utterances) between two row-major device matrices:
  * dst[dst_row[s] + r, 0:cols] = src[src_row[s] + r, 0:cols] for r < len[s].  Used to bring the

@@ -128,6 +128,7 @@ EXPORTS = [
     "nnk_dtw_align", "nnk_dtw_workspace_bytes", "nnk_gather_rows", "nnk_trim_lengths", "nnk_delta_features",
     "nnk_metric_workspace_bytes", "nnk_frame_metric", "nnk_f0_metric", "nnk_segment_copy", "nnk_gmm_logprob", "nnk_gmm_map",
     "nnk_gmm_em_workspace_bytes", "nnk_gmm_em_estep", "nnk_gmm_em_mstep", "nnk_gmm_em_factor",
+    "nnk_postfilter_basis_elems", "nnk_postfilter_basis", "nnk_postfilter_apply",
     "nnk_peer_alloc", "nnk_peer_free", "nnk_peer_export", "nnk_peer_open", "nnk_peer_close", "nnk_peer_copy",
 ]
 
@@ -203,6 +204,12 @@ def _load():
     for name in ("nnk_gmm_em_estep", "nnk_gmm_em_mstep", "nnk_gmm_em_factor"):
         getattr(L, name).restype = ctypes.c_int
         getattr(L, name).argtypes = [ctypes.POINTER(NnkGmmEmArgs), vp]
+    L.nnk_postfilter_basis_elems.restype = i64
+    L.nnk_postfilter_basis_elems.argtypes = [i32, i32]
+    L.nnk_postfilter_basis.restype = ctypes.c_int
+    L.nnk_postfilter_basis.argtypes = [ctypes.c_double, i32, i32, i32, vp, i64, vp]
+    L.nnk_postfilter_apply.restype = ctypes.c_int
+    L.nnk_postfilter_apply.argtypes = [vp, i32, i64, i32, i64, vp, i32, vp, i64, vp, i64, vp]
     L.nnk_segment_copy.restype = ctypes.c_int
     L.nnk_segment_copy.argtypes = [vp, vp, i32, i64, i64, i64, vp, vp, vp, i32, i32, vp]
     return L
