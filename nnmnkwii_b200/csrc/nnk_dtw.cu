@@ -777,10 +777,7 @@ constexpr int DTW_NWARP = DTW_FR / 32;
 constexpr int DTW_CW = 128;    // columns per boundary ring
 constexpr int DTW_NBR = DTW_NWARP + 1;  // boundary rings (one per group in flight + the one being read)
 constexpr int DTW_POLL = 8;    // steps between progress checks / publications
-#ifndef NNK_DTW_TRIP
-#define NNK_DTW_TRIP 2
-#endif
-constexpr int DTW_TRIP = NNK_DTW_TRIP;  // columns per loop trip (cost evaluations in flight per lane)
+constexpr int DTW_TRIP = 2;    // columns per loop trip (cost evaluations in flight per lane)
 static_assert(DTW_POLL % DTW_TRIP == 0, "progress checks fall on trip boundaries");
 
 struct DtwFusedParams {
@@ -993,12 +990,6 @@ static const void* dtw_fused_fn(int nb8) {
     default: return (const void*)dtw_fused_kernel<T, 4>;
   }
 }
-static bool dtw_force_two_pass() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("NNK_DTW_TWO_PASS"); v = (e && e[0] == '1') ? 1 : 0; }  // A/B measurements only
-  return v == 1;
-}
-
 // pairs per chunk of the exact mode: 9 bytes per cell (float64 cost + back-pointer), <= ~2 GiB per chunk
 static int dtw_exact_chunk(int n_pairs, int max_tx, int max_ty) {
   const size_t per = (size_t)max_tx * (size_t)max_ty * 9;
@@ -1135,7 +1126,7 @@ extern "C" int nnk_dtw_align(const nnk_dtw_args_t* a, void* stream) {
     NNK_CUDA_CHECK(cudaFuncGetAttributes(&fa, a->dtype == NNK_F64 ? dtw_fused_fn<double>(a->D / 8) : dtw_fused_fn<float>(a->D / 8)));
     fused_dyn = (size_t)max_smem > fa.sharedSizeBytes ? (size_t)max_smem - fa.sharedSizeBytes : 0;
   }
-  if (full && !dtw_force_two_pass() && dtw_fused_ok(a->max_tx, a->max_ty, a->D, fused_dyn)) {
+  if (full && dtw_fused_ok(a->max_tx, a->max_ty, a->D, fused_dyn)) {
     DtwFusedParams f;
     f.X = a->X; f.Y = a->Y; f.x_pair_stride = a->x_pair_stride; f.y_pair_stride = a->y_pair_stride;
     f.x_ld = a->x_ld; f.y_ld = a->y_ld; f.D = a->D; f.len_x = a->len_x; f.len_y = a->len_y; f.order = a->order;

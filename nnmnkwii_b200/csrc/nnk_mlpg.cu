@@ -18,34 +18,21 @@
 // HBM.  L D L^T instead of the reference's L L^T: same pivots d[t] (so the same not-positive-
 // definite test, linalg.pyx:79), no sqrt on the loop-carried dependency chain, results agree to
 // rounding (1e-15 relative).
-#include <stdlib.h>
-
+//
+// Two kernels: mlpg_kernel below (one warp per work item, register-prefetched loads, every mode) and the
+// warp-specialised, TMA-staged mlpg_fwd_as_kernel of nnk_mlpg_as.cuh.  launch_mlpg takes the staged kernel
+// for forward solves and float32-grad_output gradients whose window set fills its template instance
+// (nw == NW), with NT <= 5 and rows narrow enough for as_geometry; everything else runs mlpg_kernel.
 #include "nnk_mlpg.cuh"
-#include "nnk_mlpg_tma.cuh"
 #include "nnk_mlpg_as.cuh"
 
-// assembler warps per chain group and TMA stages per assembler of the one-group kernel (A/B builds:
-// -DNNK_AS_NA=2 -DNNK_AS_NSA1=2)
-#ifndef NNK_AS_NA
-#define NNK_AS_NA 3
-#endif
-#ifndef NNK_AS_NSA1
-#define NNK_AS_NSA1 1
-#endif
-// chain groups per CTA of float32 forward solves (-DNNK_AS_G=1 keeps one group per CTA everywhere) and TMA
-// stages per assembler pair of the two-group kernel (-DNNK_AS_NSA=1 for A/B builds)
-#ifndef NNK_AS_G
-#define NNK_AS_G 2
-#endif
-#ifndef NNK_AS_NSA
-#define NNK_AS_NSA 2
-#endif
-// depth of the band-row (PB) ring in tiles; must be >= the producers' tile stride (see nnk_mlpg_as.cuh)
-#ifndef NNK_AS_ND
-#define NNK_AS_ND (NNK_AS_PAIRS ? 6 : 4)
-#endif
-
 namespace nnk {
+
+// staged kernel configuration, settled by the A/B measurements of DESIGN.md §3.1: 4-frame tiles, three
+// assembler warps per chain group with one TMA stage each (two per assembler pair when a CTA serves two chain
+// groups), a band-row ring of 6 tiles (>= the paired producers' tile stride 2 NA - 1, see nnk_mlpg_as.cuh), and
+// 8-frame backward tiles, 8 in flight (4 when the variance rows ride along in the gradient)
+constexpr int AS_TT = 4, AS_NA = 3, AS_NSA1 = 1, AS_NSA2 = 2, AS_ND = 6, AS_TTB = 8;
 
 __device__ __forceinline__ double load_go(const void* go, int is_f64, int64_t idx) {
   return is_f64 ? ld_stream(reinterpret_cast<const double*>(go) + idx)
@@ -341,30 +328,39 @@ static int pick_instance(const nnk_windows_t& w, int& inst) {
   return 2 * NNK_MAX_HALF;
 }
 
-// NNK_MLPG_DIRECT=1 selects the register-prefetch kernel for A/B measurements (both are CUDA paths)
-static bool force_direct_loads() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("NNK_MLPG_DIRECT"); v = (e && e[0] == '1') ? 1 : 0; }
-  return v == 1;
-}
-
-// NNK_MLPG_SINGLE=1 selects the single-warp TMA kernel instead of the assembler/solver pair
-static bool force_single_warp() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("NNK_MLPG_SINGLE"); v = (e && e[0] == '1') ? 1 : 0; }
-  return v == 1;
-}
-
 static bool is_std_windows(const nnk_windows_t& w) {
   if (w.nw != 3 || w.l[0] != 0 || w.u[0] != 0 || w.l[1] != 1 || w.u[1] != 1 || w.l[2] != 1 || w.u[2] != 1) return false;
   return w.coef[0][0] == 1.0 && w.coef[1][0] == -0.5 && w.coef[1][1] == 0.0 && w.coef[1][2] == 0.5 &&
          w.coef[2][0] == 1.0 && w.coef[2][1] == -2.0 && w.coef[2][2] == 1.0;
 }
 
+// one launch of the staged kernel with G chain groups per CTA; the standard window set (STD: closed-form band
+// rows) and global (D,) variances (VARG) are template parameters
+template <typename Tin, int NW, int L, int U, int MODE, int NSA, int G>
+static int launch_as(const MlpgParams<Tin, NW, L, U>& p, const AsGeom& g, size_t smem, int grid, bool stdw, bool varg,
+                     cudaStream_t st) {
+  constexpr bool CAN_STD = (NW == 3 && L == 1 && U == 1);
+  constexpr int NSB = (MODE == MODE_GRAD) ? 4 : 8;
+#define NNK_LAUNCH_AS(STDV, VARGV)                                                                                \
+  do {                                                                                                           \
+    auto kern = mlpg_fwd_as_kernel<Tin, NW, L, U, STDV, VARGV, MODE, AS_TT, AS_NA, NSA, AS_ND, AS_TTB, NSB, G>; \
+    NNK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));        \
+    kern<<<grid, 32 * G * (AS_NA + 1), smem, st>>>(p, g);                                                       \
+  } while (0)
+  if (stdw && !varg) NNK_LAUNCH_AS(CAN_STD, false);
+  else if (stdw && varg) NNK_LAUNCH_AS(CAN_STD, true);
+  else if (!varg) NNK_LAUNCH_AS(false, false);
+  else NNK_LAUNCH_AS(false, true);
+#undef NNK_LAUNCH_AS
+  return NNK_OK;
+}
+
 template <typename Tin, int NW, int L, int U, int MODE>
 static int launch_mlpg(const nnk_mlpg_args_t& a, cudaStream_t st) {
   constexpr int NT = L + U + 1;
   constexpr int PF = (L + U <= 2) ? 4 : 2;
+  constexpr int ES = (int)sizeof(Tin);
+  constexpr bool GRAD = (MODE == MODE_GRAD);
   MlpgParams<Tin, NW, L, U> p;
   if (!fill_wintab<NW, L, U>(a.win, p.win)) { set_error("window set does not fit kernel instance"); return NNK_ERR_UNSUPPORTED; }
   p.means = (const Tin*)a.means; p.vars = (const Tin*)a.vars; p.go = a.grad_out; p.go_f64 = a.go_f64; p.out = a.out;
@@ -376,81 +372,44 @@ static int launch_mlpg(const nnk_mlpg_args_t& a, cudaStream_t st) {
   size_t items_cap = per_item ? a.workspace_bytes / per_item : 0;
   int utt_per_launch = (int)(items_cap / (size_t)p.n_groups);
   if (utt_per_launch < 1) { set_error("workspace too small: need >= %zu bytes", per_item * p.n_groups); return NNK_ERR_WORKSPACE; }
-  // forward solves go through a staged kernel unless the rows are too wide for its rings: the warp-specialised
-  // kernel when as_geometry fits, else the single-warp TMA kernel when tma_geometry fits
-  TmaGeom geom;
-  size_t smem_bytes = 0;
-  constexpr int ES = (int)sizeof(Tin);
-  constexpr bool GRAD = (MODE == MODE_GRAD);
-  constexpr bool GRAD_MODE = GRAD;
-  constexpr int TT = 4, NS = 4, TTB = 4, NA = NNK_AS_NA, NSA = NNK_AS_NSA1, ND = NNK_AS_ND;
-  // backward-sweep scratch ring of the paired kernel: 64 frames in flight (32 when the variance rows ride along)
-  constexpr int TTB_AS = 8, NSB_AS = GRAD_MODE ? 4 : 8;
-  AsGeom as_geom;
-  size_t as_smem = 0;
-  // the gradient takes the staged path when grad_out is float32 (what autograd hands over)
-  const bool paired = (MODE == MODE_FWD || (GRAD && !a.go_f64)) && !force_single_warp() && (NT <= 5) &&
-                      as_geometry<TT, NA, NSA, ND, TTB_AS, NSB_AS>(GRAD ? a.go_ld * 4 : a.in_ld * ES, a.var_ld * ES, GRAD, L,
-                                                                   NT, as_geom, as_smem);
+  // The staged kernel serves forward solves and gradients with a float32 grad_out (what autograd hands over)
+  // when the window set fills the instance (nw == NW) and the rows fit as_geometry's rings.  It is compiled only
+  // for NT <= 5 and never for nnk_mlpg_solve; everything else runs mlpg_kernel.
+  constexpr bool CAN_AS = (MODE != MODE_SOLVE) && (NT <= 5);
   // float32 forward solves with two or more chain groups: one CTA per pair of groups (an odd last group runs
   // with an empty second half), when that geometry fits two CTAs per SM.  Float64 rows and the gradient keep
   // one group per CTA, and so do band depths S > 2: at the 128 registers of two 256-thread CTAs per SM the
   // S = 4 assembler spills.
-  constexpr bool CAN_G2 = (NNK_AS_G >= 2) && (MODE == MODE_FWD) && (ES == 4) && (NT <= 3);
-  AsGeom as_geom2;
-  size_t as_smem2 = 0;
-  const bool grouped = CAN_G2 && paired && p.n_groups >= 2 &&
-                       as_geometry<TT, NA, NNK_AS_NSA, ND, TTB_AS, NSB_AS, 2>(a.in_ld * ES, a.var_ld * ES, false, L, NT,
-                                                                             as_geom2, as_smem2);
-  const bool staged = !force_direct_loads() && (a.win.nw == NW) &&
-                      (paired || (MODE == MODE_FWD && tma_geometry<TT, NS, TTB>(a.in_ld, a.var_ld, ES, NT, geom, smem_bytes)));
+  constexpr bool CAN_G2 = CAN_AS && (MODE == MODE_FWD) && (ES == 4) && (NT <= 3);
+  constexpr int NSB = GRAD ? 4 : 8;
+  AsGeom geom, geom2;
+  size_t smem = 0, smem2 = 0;
+  bool staged = false, grouped = false;
+  if constexpr (CAN_AS) {
+    staged = (a.win.nw == NW) && !(GRAD && a.go_f64) &&
+             as_geometry<AS_TT, AS_NA, AS_NSA1, AS_ND, AS_TTB, NSB>(GRAD ? a.go_ld * 4 : a.in_ld * ES, a.var_ld * ES, GRAD,
+                                                                    L, NT, geom, smem);
+    if constexpr (CAN_G2)
+      grouped = staged && p.n_groups >= 2 &&
+                as_geometry<AS_TT, AS_NA, AS_NSA2, AS_ND, AS_TTB, NSB, 2>(a.in_ld * ES, a.var_ld * ES, false, L, NT, geom2,
+                                                                          smem2);
+  }
+  const bool stdw = (NW == 3 && L == 1 && U == 1) && is_std_windows(a.win);
+  const bool varg = (a.var_ld == 0);
   for (int u0 = 0; u0 < a.n_utt; u0 += utt_per_launch) {
     const int nu = (a.n_utt - u0 < utt_per_launch) ? a.n_utt - u0 : utt_per_launch;
     p.urank0 = u0;
-    if (staged) {
-      constexpr bool CAN_STD = (NW == 3 && L == 1 && U == 1);
-      const bool stdw = CAN_STD && is_std_windows(a.win);
-      const bool varg = (a.var_ld == 0);
-      const int grid = nu * p.n_groups;
-      constexpr int AS_MODE = GRAD ? MODE_GRAD : MODE_FWD;  // MODE_SOLVE never gets here
-      if (grouped) {
-        if constexpr (CAN_G2) {
-#define NNK_LAUNCH_AS2(STDV, VARGV)                                                                                  \
-  do {                                                                                                              \
-    auto kern = mlpg_fwd_as_kernel<Tin, NW, L, U, STDV, VARGV, AS_MODE, TT, NA, NNK_AS_NSA, ND, TTB_AS, NSB_AS, 2>; \
-    NNK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)as_smem2));        \
-    kern<<<nu * ((p.n_groups + 1) / 2), 2 * 32 * (NA + 1), as_smem2, st>>>(p, as_geom2);                            \
-  } while (0)
-          if (stdw && !varg) NNK_LAUNCH_AS2(CAN_STD, false);
-          else if (stdw && varg) NNK_LAUNCH_AS2(CAN_STD, true);
-          else if (!varg) NNK_LAUNCH_AS2(false, false);
-          else NNK_LAUNCH_AS2(false, true);
-#undef NNK_LAUNCH_AS2
-        }
-      } else if (paired) {
-#define NNK_LAUNCH_AS(STDV, VARGV)                                                                                   \
-  do {                                                                                                              \
-    auto kern = mlpg_fwd_as_kernel<Tin, NW, L, U, STDV, VARGV, AS_MODE, TT, NA, NSA, ND, TTB_AS, NSB_AS, 1>;               \
-    NNK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)as_smem));         \
-    kern<<<grid, 32 * (NA + 1), as_smem, st>>>(p, as_geom);                                                         \
-  } while (0)
-        if (stdw && !varg) NNK_LAUNCH_AS(CAN_STD, false);
-        else if (stdw && varg) NNK_LAUNCH_AS(CAN_STD, true);
-        else if (!varg) NNK_LAUNCH_AS(false, false);
-        else NNK_LAUNCH_AS(false, true);
-#undef NNK_LAUNCH_AS
-      } else {
-#define NNK_LAUNCH_TMA(STDV, VARGV) \
-  mlpg_fwd_tma_kernel<Tin, NW, L, U, STDV, VARGV, TT, NS, TTB><<<grid, 32, smem_bytes, st>>>(p, geom)
-        if (stdw && !varg) NNK_LAUNCH_TMA(CAN_STD, false);
-        else if (stdw && varg) NNK_LAUNCH_TMA(CAN_STD, true);
-        else if (!varg) NNK_LAUNCH_TMA(false, false);
-        else NNK_LAUNCH_TMA(false, true);
-#undef NNK_LAUNCH_TMA
-      }
-    }
-    else
+    if (!staged) {
       mlpg_kernel<Tin, NW, L, U, MODE, PF><<<nu * p.n_groups, 32, 0, st>>>(p);
+    } else if constexpr (CAN_AS) {
+      int r;
+      if constexpr (CAN_G2)
+        r = grouped ? launch_as<Tin, NW, L, U, MODE, AS_NSA2, 2>(p, geom2, smem2, nu * ((p.n_groups + 1) / 2), stdw, varg, st)
+                    : launch_as<Tin, NW, L, U, MODE, AS_NSA1, 1>(p, geom, smem, nu * p.n_groups, stdw, varg, st);
+      else
+        r = launch_as<Tin, NW, L, U, MODE, AS_NSA1, 1>(p, geom, smem, nu * p.n_groups, stdw, varg, st);
+      if (r != NNK_OK) return r;
+    }
     count_launch();
     NNK_CUDA_CHECK(cudaGetLastError());
   }

@@ -1,4 +1,4 @@
-// nnk_mlpg.cuh -- declarations shared by the MLPG kernels (nnk_mlpg.cu, nnk_mlpg_tma.cuh).
+// nnk_mlpg.cuh -- declarations shared by the MLPG kernels (nnk_mlpg.cu, nnk_mlpg_as.cuh).
 #pragma once
 #include "nnk_common.cuh"
 

@@ -3,10 +3,10 @@
 The suite's other MLPG tests run the kernels the benchmark workloads use.  Here each case names the kernel
 it expects (`variant_mirror.mlpg_kernel_for`, a restatement of the launcher's thresholds) and the profiler
 confirms that it ran:
-  * template instance 3 (NW = 4, L = U = 4): four windows -> `mlpg_fwd_tma_kernel` forward; three windows
-    with a half-width-3 window, and two windows of half-width 2 in instance 2, take `mlpg_kernel` because
-    nw < NW;
-  * both sides of the row-width limits of the staged kernels, forward and gradient;
+  * template instance 3 (NW = 4, L = U = 4): NT = 9 is beyond the staged kernel, so four windows take
+    `mlpg_kernel`; three windows with a half-width-3 window, and two windows of half-width 2 in instance 2,
+    take `mlpg_kernel` because nw < NW;
+  * both sides of the row-width limit of the staged kernel, forward and gradient;
   * a 513-bin spectral envelope with standard windows (D = 1539), which only `mlpg_kernel` takes;
   * a batch split into several launches ("waves") when its factor scratch exceeds the workspace cap;
   * the not-positive-definite report of every kernel."""
@@ -48,7 +48,7 @@ def _data(rng, T, D, dt, var_global=False):
 
 def _assert_ran(names, kernel):
     """`kernel` ran, and no other MLPG kernel did."""
-    mlpg = M.launched(names, r"\bmlpg_(fwd_as_|fwd_tma_)?kernel<")
+    mlpg = M.launched(names, r"\bmlpg_(fwd_as_)?kernel<")
     assert mlpg and all(kernel + "<" in n for n in mlpg), (kernel, mlpg)
 
 
@@ -71,7 +71,7 @@ def _grad(ws, m, v, kernel, rng):
 
 
 @pytest.mark.parametrize("name,ws,fwd_kernel,grad_kernel", [
-    ("nw4", WIN_NW4, M.TMA, M.DIRECT),
+    ("nw4", WIN_NW4, M.DIRECT, M.DIRECT),
     ("nw3_halfwidth3", WIN_NW3_HW3, M.DIRECT, M.DIRECT),
     ("nw2_halfwidth2", WIN_NW2_HW2, M.DIRECT, M.DIRECT),
 ])
@@ -109,21 +109,9 @@ def test_row_width_limit_of_the_staged_kernels(wi, dt, mode):
             _grad(ws, m, v, kernel, rng)
 
 
-@pytest.mark.parametrize("dt", [np.float32, np.float64], ids=["f32", "f64"])
-def test_row_width_limit_of_the_single_warp_kernel(dt):
-    """Four windows (instance 3): `mlpg_fwd_tma_kernel` up to its 40 KB ring, `mlpg_kernel` beyond."""
-    es = np.dtype(dt).itemsize
-    lim = M.staged_limit("fwd", WIN_NW4, es)
-    rng = np.random.default_rng(lim)
-    for D, kernel in ((lim - 1, M.TMA), (lim, M.TMA), (lim + 1, M.DIRECT)):
-        assert M.mlpg_kernel_for("fwd", WIN_NW4, D, es) == kernel, (D, lim)
-        m, v = _data(rng, 29, D, dt)
-        _fwd(WIN_NW4, m, v, kernel)
-
-
 def test_wide_spectral_envelope():
     """513-bin WORLD spectral envelope with static / delta / delta-delta windows: D = 1539 is wider than
-    either staged kernel's ring, so forward and gradient run `mlpg_kernel`."""
+    the staged kernel's rings, so forward and gradient run `mlpg_kernel`."""
     rng = np.random.default_rng(513)
     sd, T = 513, 600
     D = 3 * sd
@@ -215,12 +203,12 @@ def test_wave_split_reports_the_first_failure_in_reference_order(monkeypatch):
 # ---- not positive definite ----------------------------------------------------------------------------------
 @pytest.mark.parametrize("mode,ws,sd,kernel", [
     ("fwd", STD, 6, M.AS),
-    ("fwd", WIN_NW4, 5, M.TMA),
+    ("fwd", WIN_NW4, 5, M.DIRECT),
     ("fwd", WIN_NW3_HW3, 5, M.DIRECT),
     ("fwd", STD, 200, M.DIRECT),
     ("grad", STD, 6, M.AS),
     ("grad", WIN_NW4, 5, M.DIRECT),
-], ids=["fwd-as", "fwd-tma", "fwd-direct-narrow-set", "fwd-direct-wide-rows", "grad-as", "grad-direct"])
+], ids=["fwd-as", "fwd-direct-instance3", "fwd-direct-narrow-set", "fwd-direct-wide-rows", "grad-as", "grad-direct"])
 def test_not_positive_definite_through_every_kernel(mode, ws, sd, kernel):
     G = _G()
     rng = np.random.default_rng(sd)

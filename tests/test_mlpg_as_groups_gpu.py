@@ -21,7 +21,7 @@ STD = windows_set()[2]
 # three windows of half-width 1 that are not the standard static / delta / delta-delta set
 ODD3 = [(0, 0, np.array([1.0])), (1, 1, np.array([-1.0, 0.0, 1.0])), (0, 1, np.array([-1.0, 1.0]))]
 SKEW3 = [(0, 0, np.array([1.0])), (1, 0, np.array([-1.0, 1.0])), (1, 1, np.array([0.25, -0.5, 0.25]))]
-AS_FAMILY = r"\bmlpg_(fwd_as_|fwd_tma_)?kernel<"
+AS_FAMILY = r"\bmlpg_(fwd_as_)?kernel<"
 
 
 def _G():
@@ -46,18 +46,9 @@ def _run(fn, want_g):
     return out
 
 
-def _g2_fits(row_bytes):
-    """`as_geometry<TT=4, NA=3, NSA=2, ND=6, TTB=8, NSB=8, G=2>` of csrc/nnk_mlpg_as.cuh (float32 forward, S = 2)."""
-    sb_in = (6 * row_bytes + 32 + 15) // 16 * 16
-    ring = (2 * 2 * sb_in + 127) // 128 * 128
-    pbb, bwd = 2 * 6 * 4 * 4 * 256, 2 * 8 * 8 * 3 * 32 * 8
-    if 3 * ring + pbb < bwd:
-        ring = ((bwd - pbb) // 3 + 127) // 128 * 128
-    return 512 + 3 * ring + pbb <= 113 * 1024
-
-
 def _want_g(n_chain, D):
-    return 2 if n_chain > 32 and _g2_fits(4 * D) else 1
+    """G of a float32 standard-window forward solve with per-frame variances, D columns in both arrays."""
+    return 2 if n_chain > 32 and M.as_geometry_fits(4 * D, 4 * D, False, 1, 3, G=2, NSA=2) else 1
 
 
 def _single(rng, T, sd, dt=np.float32, var_global=False, nw=3):

@@ -90,7 +90,7 @@ def outcomes(NA, ND, pairs, runs=200, biases=(0.02, 1.0, 4.0, 16.0)):
 
 
 def test_shipped_configuration_is_safe():
-    assert outcomes(NA=3, ND=4, pairs=False) == {"ok"}      # stride 3 <= 4 (production)
+    assert outcomes(NA=3, ND=4, pairs=False) == {"ok"}      # stride 3 <= 4 (unpaired tiles)
     assert outcomes(NA=2, ND=4, pairs=False) == {"ok"}
     assert outcomes(NA=4, ND=4, pairs=False) == {"ok"}      # stride == ND is still covered
 
@@ -104,7 +104,7 @@ def test_paired_tiles_with_ring_depth_4_corrupt_or_hang():
 
 
 def test_paired_tiles_with_ring_depth_6_are_safe():
-    assert outcomes(NA=3, ND=6, pairs=True) == {"ok"}       # the -DNNK_AS_PAIRS=1 build (NNK_AS_ND = 6)
+    assert outcomes(NA=3, ND=6, pairs=True) == {"ok"}       # the shipped kernel (paired tiles, ND = 6)
     assert outcomes(NA=3, ND=5, pairs=True) == {"ok"}       # stride 5 <= 5
 
 

@@ -1,8 +1,8 @@
 """Host-side mirrors of the kernel-selection rules of the MLPG, UnitVarianceMLPG, DTW and GMM launchers, and
 a profiler helper that names the CUDA kernels a call launched.
 
-The mirrors restate, in Python, the size thresholds of the launchers (`pick_instance`, `as_geometry`,
-`tma_geometry` in csrc/nnk_mlpg*.cu*, `dtw_fused_smem` / `dtw_smem_bytes` / `dtw_fast_cells_bound` /
+The mirrors restate, in Python, the size thresholds of the launchers (`pick_instance`, `as_geometry`
+in csrc/nnk_mlpg*.cu*, `dtw_fused_smem` / `dtw_smem_bytes` / `dtw_fast_cells_bound` /
 `dtw_exact_chunk` in csrc/nnk_dtw.cu, `em_layout` / `estep_d` / `mstep_d` in csrc/nnk_gmm_em.cu and the
 launch sizes of csrc/nnk_gmm.cu).  The tests of tests/test_kernel_variants_*_gpu.py pick their shapes
 from them and then assert, with the profiler, that the kernel the mirror predicts is the one that ran: a
@@ -73,50 +73,43 @@ def _r16(n):
     return (n + 32 + 15) // 16 * 16
 
 
-def as_geometry_fits(row_bytes_m, row_bytes_v, grad, half_l, nt):
-    """`as_geometry<TT=4, NA=3, NSA=1, ND=6, TTB=8, NSB=grad ? 4 : 8>` of csrc/nnk_mlpg_as.cuh."""
-    TT, NA, NSA, ND, TTB = 4, 3, 1, 6, 8
+def as_geometry_fits(row_bytes_m, row_bytes_v, grad, half_l, nt, G=1, NSA=1):
+    """`as_geometry<TT=4, NA=3, NSA, ND=6, TTB=8, NSB=grad ? 4 : 8, G>` of csrc/nnk_mlpg_as.cuh.  The launcher
+    asks for NSA = 1 at G = 1 and NSA = 2 at G = 2."""
+    TT, NA, ND, TTB = 4, 3, 6, 8
     NSB = 4 if grad else 8
     ld = max(row_bytes_m, row_bytes_v)
     sb_in = _r16((TT + nt - 1) * ld)
     sb_ws = TTB * nt * 32 * 8
     sb_var = _r16((TTB + half_l) * row_bytes_v) if grad else 0
     ring_a = (NSA * 2 * sb_in + 127) // 128 * 128
-    pbb = ND * TT * (nt + 1) * 32 * 8
-    bwd = NSB * (sb_ws + sb_var)
+    pbb = G * ND * TT * (nt + 1) * 32 * 8
+    bwd = G * NSB * (sb_ws + sb_var)
     if NA * ring_a + pbb < bwd:
         ring_a = ((bwd - pbb) // NA + 127) // 128 * 128
-    return 512 + NA * ring_a + pbb <= 100 * 1024
+    return 512 + NA * ring_a + pbb <= (100 if G == 1 else 113) * 1024
 
 
-def tma_geometry_fits(in_ld, var_ld, es, nt):
-    """`tma_geometry<TT=4, NS=4, TTB=4>` of csrc/nnk_mlpg_tma.cuh."""
-    TT, NS, TTB = 4, 4, 4
-    ld = max(in_ld, var_ld)
-    sb_in = _r16(TT * ld * es)
-    sb_ws = TTB * nt * 32 * 8
-    return 128 + max(NS * 2 * sb_in, NS * sb_ws) <= 40 * 1024
-
-
-AS, TMA, DIRECT = "mlpg_fwd_as_kernel", "mlpg_fwd_tma_kernel", "mlpg_kernel"
+AS, DIRECT = "mlpg_fwd_as_kernel", "mlpg_kernel"
 
 
 def mlpg_kernel_for(mode, windows, D, es, var_global=False, go_ld=None, go_f64=False):
     """Name of the kernel `launch_mlpg` runs for a single-stream call: mode "fwd" (in_ld = D) or "grad"
-    (go_ld = columns of grad_output, static_dim for paramgen.mlpg_grad)."""
+    (go_ld = columns of grad_output, static_dim for paramgen.mlpg_grad).
+
+    The staged kernel runs when the window set fills its instance (nw == NW), NT <= 5, the call is a forward
+    solve or has a float32 grad_output, and `as_geometry` fits; everything else runs `mlpg_kernel`."""
     NW, L, U = pick_instance(windows)
     nt = L + U + 1
     var_ld = 0 if var_global else D
     if mode == "fwd":
-        paired = nt <= 5 and as_geometry_fits(D * es, var_ld * es, False, L, nt)
-        staged = len(windows) == NW and (paired or tma_geometry_fits(D, var_ld, es, nt))
+        row_bytes_m = D * es
     else:
-        go_ld = D // len(windows) if go_ld is None else go_ld
-        paired = (not go_f64) and nt <= 5 and as_geometry_fits(go_ld * 4, var_ld * es, True, L, nt)
-        staged = len(windows) == NW and paired
-    if not staged:
-        return DIRECT
-    return AS if paired else TMA
+        if go_f64:
+            return DIRECT
+        row_bytes_m = 4 * (D // len(windows) if go_ld is None else go_ld)
+    staged = len(windows) == NW and nt <= 5 and as_geometry_fits(row_bytes_m, var_ld * es, mode == "grad", L, nt)
+    return AS if staged else DIRECT
 
 
 def staged_limit(mode, windows, es, var_global=False):
