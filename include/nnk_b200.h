@@ -303,6 +303,64 @@ int nnk_gmm_em_estep(const nnk_gmm_em_args_t* args, void* stream);
 int nnk_gmm_em_mstep(const nnk_gmm_em_args_t* args, void* stream);
 int nnk_gmm_em_factor(const nnk_gmm_em_args_t* args, void* stream);
 
+/* ---- k-means initialisation of the GMM fit (sklearn.cluster.KMeans(n_init=1) / kmeans_plusplus) -----------
+ * N frames of D features (D <= 128), K clusters (K <= 128, N >= K); X is float32 (widened on load) or float64,
+ * every other array float64 on the device.  With centre != 0 (KMeans.fit) every kernel reads x - mean(X) and the
+ * centres are kept in those centred coordinates; with centre == 0 (kmeans_plusplus) the raw rows.
+ *   nnk_kmeans_prepare      : mean (D) = column means (zeros when centre == 0); status[NNK_KM_VAR_MEAN] =
+ *                             mean(var(X, axis=0)) (centre != 0), the scale of KMeans' tolerance;
+ *   nnk_kmeans_seed         : k-means++ with 2 + int(log K) local trials: centers (K, D) and indices (K).  The
+ *                             random draws come from the caller: `first` (the first centre) and rand
+ *                             ((K - 1) x trials uniforms in [0, 1)), so a host RandomState is consumed as
+ *                             scikit-learn consumes it;
+ *   nnk_kmeans_lloyd        : update != 0: one Lloyd iteration from centers -- labels (N), cluster sums (K, D),
+ *                             weights (K), status[NNK_KM_CHANGED] labels that changed, status[NNK_KM_EMPTY]
+ *                             empty clusters; without empty clusters centers becomes the averages and
+ *                             status[NNK_KM_SHIFT] = sum of squared centre shifts.  With empty clusters centers
+ *                             is left alone: the caller relocates them (nnk_kmeans_relocate_dist, its own fix of
+ *                             sums / weights) and calls nnk_kmeans_average.  update == 0: labels only;
+ *   nnk_kmeans_relocate_dist: dist (N) = squared distance of every row to centers[label];
+ *   nnk_kmeans_average      : centers = sums / weights (an empty cluster copies the heaviest one), status shift;
+ *   nnk_kmeans_inertia      : status[NNK_KM_INERTIA] = sum of squared distances to centers[label],
+ *                             status[NNK_KM_DISTINCT] = distinct labels, out_centers = centers + mean.
+ * labels must hold -1 (or the previous labels) before the first Lloyd iteration.  Every reduction runs in a fixed
+ * order: identical inputs give bit-identical outputs.  Sizes outside the limits are NNK_ERR_UNSUPPORTED. */
+#define NNK_KM_CHANGED 0
+#define NNK_KM_EMPTY 1
+#define NNK_KM_SHIFT 2
+#define NNK_KM_INERTIA 3
+#define NNK_KM_DISTINCT 4
+#define NNK_KM_VAR_MEAN 5
+#define NNK_KM_STATUS_LEN 8
+typedef struct nnk_kmeans_args {
+  const void* X;              /* device (N, x_ld) frames                                               */
+  int64_t N, x_ld;
+  int32_t dtype;              /* NNK_F32 / NNK_F64 of X                                                */
+  int32_t D, K;
+  int32_t centre;             /* 1 = KMeans (centred rows), 0 = kmeans_plusplus (raw rows)             */
+  int32_t update;             /* nnk_kmeans_lloyd: 1 = assign and update, 0 = assign only              */
+  int64_t first;              /* nnk_kmeans_seed: index of the first centre                            */
+  const double* rand;         /* device (K - 1, trials): nnk_kmeans_seed's uniform draws               */
+  double* centers;            /* device (K, D)                                                         */
+  double* sums;               /* device (K, D) cluster sums                                            */
+  double* weights;            /* device (K) cluster weights                                            */
+  int32_t* labels;            /* device (N)                                                            */
+  int64_t* indices;           /* device (K) k-means++ seeds                                            */
+  double* mean;               /* device (D)                                                            */
+  double* dist;               /* device (N) nnk_kmeans_relocate_dist output                            */
+  double* out_centers;        /* device (K, D) nnk_kmeans_inertia output                               */
+  double* status;             /* device (NNK_KM_STATUS_LEN)                                            */
+  void* workspace;
+  size_t workspace_bytes;     /* >= nnk_kmeans_workspace_bytes(N, D, K); 0 = unsupported sizes          */
+} nnk_kmeans_args_t;
+size_t nnk_kmeans_workspace_bytes(int64_t N, int32_t D, int32_t K);
+int nnk_kmeans_prepare(const nnk_kmeans_args_t* args, void* stream);
+int nnk_kmeans_seed(const nnk_kmeans_args_t* args, void* stream);
+int nnk_kmeans_lloyd(const nnk_kmeans_args_t* args, void* stream);
+int nnk_kmeans_relocate_dist(const nnk_kmeans_args_t* args, void* stream);
+int nnk_kmeans_average(const nnk_kmeans_args_t* args, void* stream);
+int nnk_kmeans_inertia(const nnk_kmeans_args_t* args, void* stream);
+
 /* ---- Merlin post-filter (postfilters/__init__.py:7-62) ------------------------------------------------
  * Per frame c of a flat (N, D) batch (rows at stride ld, float32 or float64), weight w (D doubles on the
  * device): out = w * c with out[0] += log(r0(c) / r0(w * c)) / 2, where r0 = c2acr(freqt(., order, -alpha),

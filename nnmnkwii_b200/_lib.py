@@ -89,6 +89,36 @@ class NnkGmmEmArgs(ctypes.Structure):
     ]
 
 
+NNK_KM_CHANGED, NNK_KM_EMPTY, NNK_KM_SHIFT, NNK_KM_INERTIA, NNK_KM_DISTINCT, NNK_KM_VAR_MEAN = 0, 1, 2, 3, 4, 5
+NNK_KM_STATUS_LEN = 8
+
+
+class NnkKmeansArgs(ctypes.Structure):
+    _fields_ = [
+        ("X", ctypes.c_void_p),
+        ("N", ctypes.c_int64),
+        ("x_ld", ctypes.c_int64),
+        ("dtype", ctypes.c_int32),
+        ("D", ctypes.c_int32),
+        ("K", ctypes.c_int32),
+        ("centre", ctypes.c_int32),
+        ("update", ctypes.c_int32),
+        ("first", ctypes.c_int64),
+        ("rand", ctypes.c_void_p),
+        ("centers", ctypes.c_void_p),
+        ("sums", ctypes.c_void_p),
+        ("weights", ctypes.c_void_p),
+        ("labels", ctypes.c_void_p),
+        ("indices", ctypes.c_void_p),
+        ("mean", ctypes.c_void_p),
+        ("dist", ctypes.c_void_p),
+        ("out_centers", ctypes.c_void_p),
+        ("status", ctypes.c_void_p),
+        ("workspace", ctypes.c_void_p),
+        ("workspace_bytes", ctypes.c_size_t),
+    ]
+
+
 class NnkDtwArgs(ctypes.Structure):
     _fields_ = [
         ("X", ctypes.c_void_p),
@@ -128,6 +158,8 @@ EXPORTS = [
     "nnk_dtw_align", "nnk_dtw_workspace_bytes", "nnk_gather_rows", "nnk_trim_lengths", "nnk_delta_features",
     "nnk_metric_workspace_bytes", "nnk_frame_metric", "nnk_f0_metric", "nnk_segment_copy", "nnk_gmm_logprob", "nnk_gmm_map",
     "nnk_gmm_em_workspace_bytes", "nnk_gmm_em_estep", "nnk_gmm_em_mstep", "nnk_gmm_em_factor",
+    "nnk_kmeans_workspace_bytes", "nnk_kmeans_prepare", "nnk_kmeans_seed", "nnk_kmeans_lloyd", "nnk_kmeans_relocate_dist",
+    "nnk_kmeans_average", "nnk_kmeans_inertia",
     "nnk_postfilter_basis_elems", "nnk_postfilter_basis", "nnk_postfilter_apply",
     "nnk_peer_alloc", "nnk_peer_free", "nnk_peer_export", "nnk_peer_open", "nnk_peer_close", "nnk_peer_copy",
 ]
@@ -204,6 +236,12 @@ def _load():
     for name in ("nnk_gmm_em_estep", "nnk_gmm_em_mstep", "nnk_gmm_em_factor"):
         getattr(L, name).restype = ctypes.c_int
         getattr(L, name).argtypes = [ctypes.POINTER(NnkGmmEmArgs), vp]
+    L.nnk_kmeans_workspace_bytes.restype = ctypes.c_size_t
+    L.nnk_kmeans_workspace_bytes.argtypes = [i64, i32, i32]
+    for name in ("nnk_kmeans_prepare", "nnk_kmeans_seed", "nnk_kmeans_lloyd", "nnk_kmeans_relocate_dist",
+                 "nnk_kmeans_average", "nnk_kmeans_inertia"):
+        getattr(L, name).restype = ctypes.c_int
+        getattr(L, name).argtypes = [ctypes.POINTER(NnkKmeansArgs), vp]
     L.nnk_postfilter_basis_elems.restype = i64
     L.nnk_postfilter_basis_elems.argtypes = [i32, i32]
     L.nnk_postfilter_basis.restype = ctypes.c_int

@@ -294,6 +294,194 @@ def _host_f64(t):
     return t.detach().cpu().numpy().astype(np.float64, copy=True)
 
 
+_KM_MAX_FEATURES = 128
+_KM_MAX_CLUSTERS = 128
+
+
+def _check_kmeans_sizes(Xd, K):
+    """The limits of csrc/nnk_kmeans.cu, raised before anything is launched."""
+    import torch
+    N, D = Xd.shape
+    if not 1 <= D <= _KM_MAX_FEATURES:
+        raise ValueError("k-means on the GPU supports 1 to %d features (got %d)" % (_KM_MAX_FEATURES, D))
+    if not 1 <= K <= _KM_MAX_CLUSTERS:
+        raise ValueError("k-means on the GPU supports 1 to %d clusters (got %d)" % (_KM_MAX_CLUSTERS, K))
+    if N < K:
+        raise ValueError("n_samples=%d should be >= n_clusters=%d." % (N, K))
+    if Xd.dtype not in (torch.float32, torch.float64) or Xd.stride(1) != 1 or Xd.stride(0) < D:
+        raise ValueError("k-means on the GPU reads float32 / float64 rows with unit column stride")
+
+
+def _kmeans_plusplus_draws(N, K, random_state):
+    """The RandomState calls of sklearn's ``_kmeans_plusplus`` (unit sample weights), in its order: the first
+    centre, then ``n_local_trials`` uniforms per later centre.  Returns (first, (K - 1, trials) array)."""
+    trials = 2 + int(np.log(K))
+    sample_weight = np.ones(N, dtype=np.float64)
+    first = int(random_state.choice(N, p=sample_weight / sample_weight.sum()))
+    u = np.empty((K - 1, trials), dtype=np.float64)
+    for c in range(1, K):
+        u[c - 1] = random_state.uniform(size=trials)
+    return first, u
+
+
+class _KMeansState(object):
+    """Device buffers of one k-means run over the frames ``X`` (csrc/nnk_kmeans.cu) and the filled
+    ``nnk_kmeans_args_t``.  ``centre``: KMeans reads the rows minus their mean, kmeans_plusplus the raw rows."""
+
+    def __init__(self, X, K, centre):
+        import torch
+
+        from .. import _device as dev
+        from .. import _lib
+        _check_kmeans_sizes(X, K)
+        self.X, self.K = X, K
+        N, D = X.shape
+        f64 = dict(dtype=torch.float64, device=X.device)
+        self.labels = torch.full((N,), -1, dtype=torch.int32, device=X.device)
+        self.centers = torch.zeros((K, D), **f64)
+        self.sums = torch.zeros((K, D), **f64)
+        self.weights = torch.zeros(K, **f64)
+        self.indices = torch.zeros(K, dtype=torch.int64, device=X.device)
+        self.mean = torch.zeros(D, **f64)
+        self.out_centers = torch.zeros((K, D), **f64)
+        self.status = torch.zeros(_lib.NNK_KM_STATUS_LEN, **f64)
+        self.dist = None
+        self.rand = None
+        self.ws = dev.workspace(X.device, _lib.lib.nnk_kmeans_workspace_bytes(N, D, K))
+        a = _lib.NnkKmeansArgs()
+        a.X, a.N, a.x_ld, a.dtype, a.D, a.K = X.data_ptr(), N, X.stride(0), dev.torch_dtype_code(X.dtype), D, K
+        a.centre = int(bool(centre))
+        for name in ("centers", "sums", "weights", "labels", "indices", "mean", "out_centers", "status"):
+            setattr(a, name, getattr(self, name).data_ptr())
+        a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws.numel()
+        self.args = a
+        self.stream = dev.current_stream_ptr(X.device)
+
+    def _call(self, name):
+        from .. import _lib
+        _lib.check(getattr(_lib.lib, name)(ctypes.byref(self.args), self.stream), name)
+
+    def read_status(self):
+        """Synchronises: the small status record of the last call."""
+        return self.status.cpu().numpy()
+
+    def prepare(self):
+        self._call("nnk_kmeans_prepare")
+
+    def seed(self, first, u):
+        import torch
+        self.rand = torch.from_numpy(np.ascontiguousarray(u, dtype=np.float64)).to(self.X.device)
+        self.args.first = int(first)
+        self.args.rand = self.rand.data_ptr() if self.rand.numel() else None
+        self._call("nnk_kmeans_seed")
+
+    def lloyd(self, update):
+        self.args.update = int(bool(update))
+        self._call("nnk_kmeans_lloyd")
+
+    def relocate_empty_clusters(self):
+        """sklearn's ``_relocate_empty_clusters_dense`` on the sums and weights of the last Lloyd step.  The
+        distances come from the device; the choice of samples is numpy's own ``argpartition``, because the
+        order of its introselect among the farthest samples is not something a kernel can restate.  Only the
+        chosen rows are downloaded.  Rare: k-means++ seeds seldom leave a cluster empty."""
+        import torch
+        if self.dist is None:
+            self.dist = torch.empty(self.X.shape[0], dtype=torch.float64, device=self.X.device)
+            self.args.dist = self.dist.data_ptr()
+        self._call("nnk_kmeans_relocate_dist")
+        distances = self.dist.cpu().numpy()
+        weights = self.weights.cpu().numpy()
+        empty = np.where(np.equal(weights, 0))[0]
+        n_empty = empty.shape[0]
+        far = np.argpartition(distances, -n_empty)[:-n_empty - 1:-1]
+        if np.max(distances) == 0:
+            return
+        sums = self.sums.cpu().numpy()
+        far_t = torch.from_numpy(far.astype(np.int64)).to(self.X.device)
+        rows = self.X[far_t].to(torch.float64).cpu().numpy() - self.mean.cpu().numpy()
+        labels = self.labels[far_t].cpu().numpy()
+        for idx in range(n_empty):
+            new, old, weight = empty[idx], labels[idx], 1.0
+            sums[old] -= rows[idx] * weight
+            sums[new] = rows[idx] * weight
+            weights[new] = weight
+            weights[old] -= weight
+        self.sums.copy_(torch.from_numpy(sums))
+        self.weights.copy_(torch.from_numpy(weights))
+
+    def average(self):
+        self._call("nnk_kmeans_average")
+
+    def inertia(self):
+        self._call("nnk_kmeans_inertia")
+
+
+def _device_kmeans_plusplus(Xd, K, random_state):
+    """sklearn's public ``kmeans_plusplus(X, K, random_state=...)`` on the raw rows of the device frames ``Xd``
+    (no centring, as that function does not centre): returns (centers (K, D) float64, indices (K,) int64),
+    both CUDA tensors.  ``random_state`` is consumed exactly as scikit-learn consumes it."""
+    from sklearn.utils import check_random_state
+    _check_kmeans_sizes(Xd, K)
+    first, u = _kmeans_plusplus_draws(Xd.shape[0], K, check_random_state(random_state))
+    st = _KMeansState(Xd, K, centre=False)
+    st.prepare()
+    st.seed(first, u)
+    return st.centers, st.indices
+
+
+def _device_kmeans(Xd, K, random_state=None, init=None, max_iter=300, tol=1e-4):
+    """sklearn's ``KMeans(n_clusters=K, n_init=1, init=init or "k-means++", max_iter, tol, random_state).fit``
+    (Lloyd) on the device frames ``Xd``.  Returns (labels (N,) int64 CUDA tensor, centers (K, D) float64 CUDA
+    tensor, inertia, n_iter).  One small status record is read back per iteration."""
+    import warnings
+
+    import torch
+    from sklearn.exceptions import ConvergenceWarning
+    from sklearn.utils import check_random_state
+
+    from .. import _lib
+    _check_kmeans_sizes(Xd, K)
+    if int(max_iter) < 1:
+        raise ValueError("max_iter must be >= 1 (got %r)" % (max_iter,))
+    if init is not None:
+        init = np.array(init, dtype=np.float64, copy=True)
+        if init.shape != (K, Xd.shape[1]):
+            raise ValueError("init should be of shape %s, got %s" % ((K, Xd.shape[1]), init.shape))
+    st = _KMeansState(Xd, K, centre=True)
+    st.prepare()
+    if init is None:
+        first, u = _kmeans_plusplus_draws(Xd.shape[0], K, check_random_state(random_state))
+        st.seed(first, u)
+        s = st.read_status()
+    else:
+        s = st.read_status()
+        init -= st.mean.cpu().numpy()
+        st.centers.copy_(torch.from_numpy(init))
+    tol_abs = 0.0 if tol == 0 else float(s[_lib.NNK_KM_VAR_MEAN]) * tol
+    strict = False
+    for i in range(int(max_iter)):
+        st.lloyd(True)
+        s = st.read_status()
+        if s[_lib.NNK_KM_EMPTY] > 0:
+            st.relocate_empty_clusters()
+            st.average()
+            s = st.read_status()
+        if s[_lib.NNK_KM_CHANGED] == 0:
+            strict = True
+            break
+        if s[_lib.NNK_KM_SHIFT] <= tol_abs:
+            break
+    if not strict:
+        st.lloyd(False)  # labels that match the final centres
+    st.inertia()
+    s = st.read_status()
+    distinct = int(s[_lib.NNK_KM_DISTINCT])
+    if distinct < K:
+        warnings.warn("Number of distinct clusters ({}) found smaller than n_clusters ({}). Possibly due to "
+                      "duplicate points in X.".format(distinct, K), ConvergenceWarning, stacklevel=2)
+    return st.labels.to(torch.int64), st.out_centers, float(s[_lib.NNK_KM_INERTIA]), i + 1
+
+
 class GaussianMixture(_SkGaussianMixture):
     """``sklearn.mixture.GaussianMixture`` whose EM runs on the GPU (csrc/nnk_gmm_em.cu).
 
@@ -310,13 +498,30 @@ class GaussianMixture(_SkGaussianMixture):
     computed from them on the device.  Only ``covariance_type="full"`` is supported, with at most 128
     features and 128 components.
 
+    ``init_device`` (additive, default False): with ``init_params`` "kmeans" or "k-means++" the k-means
+    initialisation runs on the GPU as well (csrc/nnk_kmeans.cu): scikit-learn's ``KMeans(n_init=1)`` /
+    ``kmeans_plusplus`` restated step for step, consuming ``random_state`` the same way, in float64 on the
+    frames widened to float64.  Only its labels (or seeds) cross into EM, so on the same labels the fit is
+    bit-identical to ``init_device=False``.  "random" and "random_from_data" ignore it.
+
     ``X`` may be a NumPy array or a torch CUDA tensor, float32 or float64; a CUDA tensor is copied to
-    the host only when a host initialiser ("kmeans", "k-means++") needs it, and ``fit_predict`` then
-    returns the labels as a CUDA tensor.  The arithmetic is always float64.  Note that scikit-learn 1.9
+    the host only when a host initialiser ("kmeans", "k-means++" with ``init_device=False``) needs it, and
+    ``fit_predict`` then returns the labels as a CUDA tensor.  The arithmetic is always float64.  Note that scikit-learn 1.9
     itself fits float32 data in float32, so on float32 input the two differ; this class matches
     scikit-learn run on the same data widened to float64 (to about 1e-10 relative: the summation order
     of the reductions differs in the last bits).
     """
+
+    _parameter_constraints = {**_SkGaussianMixture._parameter_constraints, "init_device": ["boolean"]}
+
+    def __init__(self, n_components=1, *, covariance_type="full", tol=1e-3, reg_covar=1e-6, max_iter=100, n_init=1,
+                 init_params="kmeans", weights_init=None, means_init=None, precisions_init=None, random_state=None,
+                 warm_start=False, verbose=0, verbose_interval=10, init_device=False):
+        super().__init__(n_components=n_components, covariance_type=covariance_type, tol=tol, reg_covar=reg_covar,
+                         max_iter=max_iter, n_init=n_init, init_params=init_params, weights_init=weights_init,
+                         means_init=means_init, precisions_init=precisions_init, random_state=random_state,
+                         warm_start=warm_start, verbose=verbose, verbose_interval=verbose_interval)
+        self.init_device = init_device
 
     def _check_sizes(self, D):
         if self.covariance_type != "full":
@@ -350,13 +555,29 @@ class GaussianMixture(_SkGaussianMixture):
             resp[indices, np.arange(K)] = 1
         return resp
 
+    def _device_initial_resp(self, st, random_state):
+        """``_initial_resp`` for "kmeans" / "k-means++" with the k-means on the device: the one-hot
+        responsibilities are scattered into ``st.resp`` without a host copy of the frames."""
+        import torch
+        K = self.n_components
+        st.resp.zero_()
+        if self.init_params == "kmeans":
+            labels, _, _, _ = _device_kmeans(st.X, K, random_state=random_state)
+            st.resp.scatter_(1, labels[:, None], 1.0)
+        else:
+            _, indices = _device_kmeans_plusplus(st.X, K, random_state)
+            st.resp[indices, torch.arange(K, device=st.resp.device)] = 1.0
+
     def _device_initialize(self, st, n_samples, host_X, random_state):
         """sklearn's ``GaussianMixture._initialize_parameters`` + ``_initialize``; returns whether the
         device covariances are valid (they are not when ``precisions_init`` is given)."""
         from sklearn.mixture._gaussian_mixture import _compute_precision_cholesky_from_precisions
         from sklearn.utils._array_api import get_namespace
         compute_resp = self.weights_init is None or self.means_init is None or self.precisions_init is None
-        if compute_resp:
+        if compute_resp and self.init_device and self.init_params in ("kmeans", "k-means++"):
+            self._device_initial_resp(st, random_state)
+            st.mstep(0 if self.weights_init is None else 2)
+        elif compute_resp:
             st.put("resp", self._initial_resp(n_samples, host_X, random_state))
             st.mstep(0 if self.weights_init is None else 2)
         if self.weights_init is not None:

@@ -208,13 +208,16 @@ class IterativeDTWAligner(object):
     as in the reference) or ``"device"`` (:class:`nnmnkwii_b200.baseline.gmm.GaussianMixture`, EM on the
     GPU in float64, same ``n_components``, ``max_iter`` and ``random_state``).  The two are not
     bit-identical: scikit-learn fits float32 frames in float32, and even on float64 frames the
-    summation order differs in the last bits.
+    summation order differs in the last bits.  ``gmm_init_device=True`` (with ``gmm="device"`` only) runs
+    that fit's k-means initialisation on the GPU too (``GaussianMixture(init_device=True)``).
     """
 
     def __init__(self, n_iter=3, dist=_default_dist, radius=1, max_iter_gmm=100, n_components_gmm=16, verbose=0,
-                 random_state=None, gmm="sklearn"):
+                 random_state=None, gmm="sklearn", gmm_init_device=False):
         if gmm not in ("sklearn", "device"):
             raise ValueError("gmm must be 'sklearn' or 'device' (got %r)" % (gmm,))
+        if gmm_init_device and gmm != "device":
+            raise ValueError("gmm_init_device=True needs gmm='device' (got gmm=%r)" % (gmm,))
         self.n_iter = n_iter
         self.dist = dist
         self.radius = radius
@@ -223,6 +226,7 @@ class IterativeDTWAligner(object):
         self.verbose = verbose
         self.random_state = random_state  # additive: the reference leaves the GMM unseeded
         self.gmm = gmm
+        self.gmm_init_device = gmm_init_device
 
     def transform(self, XY):
         import torch
@@ -265,8 +269,9 @@ class IterativeDTWAligner(object):
                 lx, ly = res.len_x.cpu().numpy(), res.len_y.cpu().numpy()
                 for idx in range(len(d)):
                     print("{}, distance: {}".format(idx, d[idx] / (lx[idx] + ly[idx])))
+            init_kw = {"init_device": True} if self.gmm_init_device else {}
             gmm = GaussianMixture(n_components=self.n_components_gmm, covariance_type="full", max_iter=self.max_iter_gmm,
-                                  random_state=self.random_state)
+                                  random_state=self.random_state, **init_kw)
             XYj = np.concatenate((X_aligned, Y_aligned), axis=-1).reshape(-1, X.shape[-1] * 2)
             gmm.fit(XYj)
             paramgen = MLPG(gmm, windows=[(0, 0, np.array([1.0]))])  # no delta (alignment.py:179-180)
