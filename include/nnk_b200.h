@@ -377,6 +377,29 @@ int nnk_postfilter_apply(const void* mgc, int32_t dtype, int64_t N, int32_t D, i
                          int32_t fftlen, const double* basis, int64_t basis_elems, void* out, int64_t out_ld,
                          void* stream);
 
+/* ---- corpus normalisation (preprocessing/generic.py:496-828) -----------------------------------------
+ * nnk_frame_stats folds the rows of n_utt utterances into a running per-column state (device, float64,
+ * 1 + 4*D doubles, in and out): [count, mean[D], m2[D], min[D], max[D]], m2 = sum of squared deviations
+ * (= var * count).  Utterance u is rows utt_off[u] .. of a row-major float32 / float64 matrix (row stride
+ * ld elements, int64 offsets on the device); it has min(utt_off[u+1] - utt_off[u], lengths[u], max_rows)
+ * valid rows (lengths: int32 on the device, NULL = no limit, negative = 0); no other row is read.  The
+ * incoming state is merged first (Chan's pairwise formula), so chunks stream through one state.  min / max
+ * start from the state's min / max (+inf / -inf for a fresh state).  A NaN propagates into its column's
+ * mean, m2, min and max.  Deterministic: fixed tiles, fixed-order fold of per-block partials.
+ * workspace >= nnk_frame_stats_workspace_bytes(n_utt, max_rows, D), any contents (reset on the stream).
+ *
+ * nnk_column_affine: per-column affine map of a contiguous (n_rows, D) matrix in the dtype `dtype`
+ * (x may be float32 while dtype is float64; a, b are D-vectors in `dtype` on the device):
+ *   form 0: out = (x - a[c]) / b[c]   (scale, inv_minmax_scale)
+ *   form 1: out = x * b[c] + a[c]     (inv_scale, minmax_scale)
+ * IEEE round-to-nearest for every operation and no contraction: bit-identical to the NumPy expression. */
+int64_t nnk_frame_stats_workspace_bytes(int32_t n_utt, int32_t max_rows, int32_t D);
+int nnk_frame_stats(const void* X, int32_t dtype, int32_t D, int64_t ld, const int64_t* utt_off,
+                    const int32_t* lengths, int32_t n_utt, int32_t max_rows, double* state, void* workspace,
+                    int64_t workspace_bytes, void* stream);
+int nnk_column_affine(const void* x, int32_t x_dtype, int32_t dtype, int64_t n_rows, int32_t D, const void* a,
+                      const void* b, int32_t form, void* out, void* stream);
+
 /* ---- sharded batches (SURVEY.md 8e; the reference has no multi-device path) ------------------------
  * Copies n_seg row segments (whole utterances) between two row-major device matrices:
  * dst[dst_row[s] + r, 0:cols] = src[src_row[s] + r, 0:cols] for r < len[s].  Used to bring the

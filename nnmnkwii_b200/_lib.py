@@ -161,6 +161,7 @@ EXPORTS = [
     "nnk_kmeans_workspace_bytes", "nnk_kmeans_prepare", "nnk_kmeans_seed", "nnk_kmeans_lloyd", "nnk_kmeans_relocate_dist",
     "nnk_kmeans_average", "nnk_kmeans_inertia",
     "nnk_postfilter_basis_elems", "nnk_postfilter_basis", "nnk_postfilter_apply",
+    "nnk_frame_stats_workspace_bytes", "nnk_frame_stats", "nnk_column_affine",
     "nnk_peer_alloc", "nnk_peer_free", "nnk_peer_export", "nnk_peer_open", "nnk_peer_close", "nnk_peer_copy",
 ]
 
@@ -248,6 +249,12 @@ def _load():
     L.nnk_postfilter_basis.argtypes = [ctypes.c_double, i32, i32, i32, vp, i64, vp]
     L.nnk_postfilter_apply.restype = ctypes.c_int
     L.nnk_postfilter_apply.argtypes = [vp, i32, i64, i32, i64, vp, i32, vp, i64, vp, i64, vp]
+    L.nnk_frame_stats_workspace_bytes.restype = i64
+    L.nnk_frame_stats_workspace_bytes.argtypes = [i32, i32, i32]
+    L.nnk_frame_stats.restype = ctypes.c_int
+    L.nnk_frame_stats.argtypes = [vp, i32, i32, i64, vp, vp, i32, i32, vp, vp, i64, vp]
+    L.nnk_column_affine.restype = ctypes.c_int
+    L.nnk_column_affine.argtypes = [vp, i32, i32, i64, i32, vp, vp, i32, vp, vp]
     L.nnk_segment_copy.restype = ctypes.c_int
     L.nnk_segment_copy.argtypes = [vp, vp, i32, i64, i64, i64, vp, vp, vp, i32, i32, vp]
     return L

@@ -1,5 +1,6 @@
 """Pre-processing pieces on the DTW hot path (drop-in for the names the aligners need from
-``nnmnkwii.preprocessing``)."""
+``nnmnkwii.preprocessing``) and corpus normalisation (``normalize``: meanvar / meanstd / minmax and the
+scale family)."""
 import numpy as np
 
 
@@ -64,4 +65,8 @@ def delta_features(x, windows, lengths=None):
     return res if res.dtype == x.dtype else res.astype(x.dtype)
 
 
-__all__ = ["trim_zeros_frames", "delta_features"]
+from .normalize import (inv_minmax_scale, inv_scale, meanstd, meanvar, minmax, minmax_scale,  # noqa: E402
+                        minmax_scale_params, remove_zeros_frames, scale)
+
+__all__ = ["trim_zeros_frames", "delta_features", "meanvar", "meanstd", "minmax", "scale", "inv_scale",
+           "minmax_scale_params", "minmax_scale", "inv_minmax_scale", "remove_zeros_frames"]
