@@ -1,0 +1,74 @@
+"""The constants that tests/variant_mirror.py restates, read out of the CUDA sources (no GPU needed).
+
+The metric, statistics, affine and segment-copy variant tests pick their shapes from the mirror; if one of
+these constants is retuned in a .cu file without the mirror, this test fails instead of the GPU tests
+quietly covering other instances than they say."""
+import os
+import re
+
+import pytest
+
+import variant_mirror as M
+
+CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "nnmnkwii_b200", "csrc")
+
+
+def _source(name):
+    with open(os.path.join(CSRC, name)) as f:
+        return f.read()
+
+
+def _constexpr(src, name):
+    m = re.findall(r"constexpr\s+(?:int|int64_t)\s+%s\s*=\s*(\d+)\s*;" % name, src)
+    assert len(m) == 1, (name, m)
+    return int(m[0])
+
+
+def _function(src, signature):
+    """Body of the function whose definition starts with `signature` (up to the next top-level brace)."""
+    i = src.index(signature)
+    j = src.index("{", i)
+    depth = 0
+    for k in range(j, len(src)):
+        depth += {"{": 1, "}": -1}.get(src[k], 0)
+        if depth == 0:
+            return src[j:k + 1]
+    raise AssertionError("unterminated body of " + signature)
+
+
+def test_number_of_sms():
+    assert _constexpr(_source("nnk_common.cuh"), "kNumSMs") == M.K_NUM_SMS
+
+
+@pytest.mark.parametrize("name", ["MT_TILE_ELEMS", "MT_TBLOCK", "MT_MIN_TILE_FRAMES", "MT_BLOCK", "MT_UNROLL"])
+def test_metric_constants(name):
+    assert _constexpr(_source("nnk_metrics.cu"), name) == getattr(M, name)
+
+
+def test_metric_dispatch_rule():
+    src = _function(_source("nnk_metrics.cu"), "static void dispatch_frame(")
+    assert "p.D < 128 && p.frame_stride == p.D" in src
+    assert "MT_TILE_ELEMS * 4 / (int)sizeof(T) / p.D" in src
+    assert "while (G < 32 && G < p.D) G <<= 1;" in src
+    # the smallest tile (float64, widest tiled row) is the one the partial workspace is sized for
+    assert min(M.metric_kernel_for(D, D, 8)[1] for D in range(1, 128)) == M.MT_MIN_TILE_FRAMES
+
+
+@pytest.mark.parametrize("name", ["ST_BLOCK", "ST_ROWS_PER_THREAD", "ST_THREADS_PER_SM", "AF_BLOCK", "AF_UNROLL"])
+def test_stats_constants(name):
+    assert _constexpr(_source("nnk_stats.cu"), name) == getattr(M, name)
+
+
+def test_stats_and_affine_geometry():
+    src = _source("nnk_stats.cu")
+    shape = _function(src, "static StatsShape stats_shape(")
+    assert "if (bps > 8) bps = 8;" in shape
+    assert "s.tile_rows = ST_ROWS_PER_THREAD * s.RS;" in shape
+    affine = _function(src, "static void launch_affine(")
+    assert re.findall(r"kNumSMs \* (\d+)", affine) == [str(M.AF_BLOCKS_PER_SM)] * 2
+
+
+def test_segment_copy_constants():
+    src = _function(_source("nnk_shard.cu"), 'extern "C" int nnk_segment_copy(')
+    assert re.findall(r"p\.rows_per_block = (\d+);", src) == [str(M.SEG_ROWS_PER_BLOCK)]
+    assert M.segment_copy_vec(4, 4, 4, 4, 0, 0) and not M.segment_copy_vec(4, 4, 4, 4, 4, 0)

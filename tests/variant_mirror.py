@@ -1,12 +1,15 @@
-"""Host-side mirrors of the kernel-selection rules of the MLPG, UnitVarianceMLPG, DTW and GMM launchers, and
-a profiler helper that names the CUDA kernels a call launched.
+"""Host-side mirrors of the kernel-selection rules of the MLPG, UnitVarianceMLPG, DTW, GMM, metric, statistics,
+affine and segment-copy launchers, and a profiler helper that names the CUDA kernels a call launched.
 
 The mirrors restate, in Python, the size thresholds of the launchers (`pick_instance`, `as_geometry`
 in csrc/nnk_mlpg*.cu*, `dtw_fused_smem` / `dtw_smem_bytes` / `dtw_fast_cells_bound` /
-`dtw_exact_chunk` in csrc/nnk_dtw.cu, `em_layout` / `estep_d` / `mstep_d` in csrc/nnk_gmm_em.cu and the
-launch sizes of csrc/nnk_gmm.cu).  The tests of tests/test_kernel_variants_*_gpu.py pick their shapes
-from them and then assert, with the profiler, that the kernel the mirror predicts is the one that ran: a
-later change to a geometry function makes those tests fail instead of silently moving their coverage."""
+`dtw_exact_chunk` in csrc/nnk_dtw.cu, `em_layout` / `estep_d` / `mstep_d` in csrc/nnk_gmm_em.cu, the
+launch sizes of csrc/nnk_gmm.cu, `dispatch_frame` in csrc/nnk_metrics.cu, `stats_shape` and
+`launch_affine` in csrc/nnk_stats.cu and the vector test of `nnk_segment_copy` in csrc/nnk_shard.cu).
+The tests of tests/test_kernel_variants_*_gpu.py and tests/test_variants_*_gpu.py pick their shapes from them and then assert, with the
+profiler, that the kernel the mirror predicts is the one that ran: a later change to a geometry function
+makes those tests fail instead of silently moving their coverage.  tests/test_variant_mirror_constants_cpu.py
+reads the constants restated here out of the CUDA sources, so a retuned constant fails there first."""
 import re
 
 import numpy as np
@@ -299,3 +302,108 @@ def gmm_logprob_smem(D):
 
 def gmm_posterior_smem(D):
     return 8 * (D * D + GMM_FT * D + 2 * GMM_FT)
+
+
+# ---- kernel names in a child process -----------------------------------------------------------------------------
+_CHILD_SCRIPT = r"""
+import json, sys
+sys.path[:0] = sys.argv[1:3]
+import importlib
+import variant_mirror as M
+mod = importlib.import_module(sys.argv[3])
+launch = getattr(mod, sys.argv[4])
+out = []
+for case, family in json.loads(sys.argv[5]):
+    _, err, names = M.profiled(lambda: launch(*case), family)
+    out.append([sorted(set(M.launched(names, family))), repr(err)])
+print(json.dumps(out))
+"""
+
+
+def profiled_in_child(module, launcher, cases):
+    """``[(kernel names of family, repr(error))]`` of ``module.launcher(*case)`` for each ``(case, family)`` of
+    ``cases``, each call profiled by `profiled` in a child Python process.  Profiling many calls in the pytest
+    process has made torch.profiler lose the records of later modules' calls on an H100; a child process
+    keeps the profiler state of those modules clean."""
+    import json
+    import os
+    import subprocess
+    import sys
+    here = os.path.dirname(os.path.abspath(__file__))
+    root = os.path.dirname(here)
+    res = subprocess.run([sys.executable, "-c", _CHILD_SCRIPT, here, root, module, launcher, json.dumps(cases)],
+                         capture_output=True, text=True, timeout=900, cwd=root)
+    assert res.returncode == 0, res.stderr[-3000:]
+    return json.loads(res.stdout.strip().splitlines()[-1])
+
+
+def _itemsize(dtype):
+    """Bytes of a NumPy / torch float dtype (or an int that already is one)."""
+    if isinstance(dtype, int):
+        return dtype
+    size = getattr(dtype, "itemsize", None)  # torch.dtype
+    return size if isinstance(size, int) else np.dtype(dtype).itemsize
+
+
+# ---- metrics (csrc/nnk_metrics.cu) -------------------------------------------------------------------------------
+MT_BLOCK = 256          # threads of frame_metric_kernel / f0_metric_kernel
+MT_UNROLL = 4           # frames in flight per lane group
+MT_TILE_ELEMS = 11776   # float32 elements of one frame_metric_tile_kernel tile
+MT_TBLOCK = 128         # threads (and most frames) of a tile
+MT_MIN_TILE_FRAMES = 46  # the smallest tile (float64, D = 127): sizes the partial workspace
+
+
+def metric_kernel_for(D, frame_stride, dtype):
+    """`dispatch_frame`: ``("tile", F)`` for `frame_metric_tile_kernel<T>` with F frames per tile, or
+    ``("frame", G)`` for `frame_metric_kernel<T, G>` with G lanes per frame."""
+    if D < 128 and frame_stride == D:
+        return "tile", min(MT_TILE_ELEMS * 4 // _itemsize(dtype) // D, MT_TBLOCK)
+    G = 1
+    while G < 32 and G < D:
+        G <<= 1
+    return "frame", G
+
+
+# ---- corpus statistics and the per-column affine map (csrc/nnk_stats.cu) ----------------------------------------
+ST_BLOCK = 256             # threads per block at most (CW * RS)
+ST_ROWS_PER_THREAD = 64    # rows a thread reads per tile
+ST_THREADS_PER_SM = 816    # resident threads per SM the grid is sized for
+AF_BLOCK = 256
+AF_UNROLL = 4
+AF_BLOCKS_PER_SM = 16      # the grid of column_affine_kernel is capped at K_NUM_SMS * 16 blocks
+
+
+def stats_shape(n_utt, max_rows, D):
+    """`stats_shape`: column strips, strip width CW, row slices RS, rows per tile, tiles and the grid."""
+    nstrips = max(1, (D + ST_BLOCK - 1) // ST_BLOCK)
+    w = (D + nstrips - 1) // nstrips
+    CW = max(32, (w + 31) // 32 * 32)
+    RS = ST_BLOCK // CW
+    tile_rows = ST_ROWS_PER_THREAD * RS
+    tiles_per_utt = (max_rows + tile_rows - 1) // tile_rows
+    n_tiles = n_utt * tiles_per_utt
+    bps = min(8, ST_THREADS_PER_SM // (CW * RS))
+    grid = max(1, min(K_NUM_SMS * bps // nstrips, n_tiles))
+    return dict(nstrips=nstrips, CW=CW, RS=RS, tile_rows=tile_rows, tiles_per_utt=tiles_per_utt, n_tiles=n_tiles,
+                grid=grid)
+
+
+def affine_passes(n, D):
+    """``(passes, step_c, stride_c)`` of `column_affine_kernel` over n = rows * D elements: the grid-stride
+    passes of the first thread (the most any thread makes), the column step between its unrolled elements and
+    the column step between its passes."""
+    per_block = AF_BLOCK * AF_UNROLL
+    grid = min((n + per_block - 1) // per_block, K_NUM_SMS * AF_BLOCKS_PER_SM)
+    stride = grid * per_block
+    return (n + stride - 1) // stride, AF_BLOCK % D, stride % D
+
+
+# ---- row-segment copy (csrc/nnk_shard.cu) ------------------------------------------------------------------------
+SEG_ROWS_PER_BLOCK = 64
+
+
+def segment_copy_vec(cols, es, src_ld, dst_ld, src_ptr, dst_ptr):
+    """True when `nnk_segment_copy` runs `segment_copy_kernel<uint4>` (16-byte words), False for
+    `segment_copy_kernel<uint32_t>`."""
+    row, sp, dp = cols * es, src_ld * es, dst_ld * es
+    return row % 16 == 0 and sp % 16 == 0 and dp % 16 == 0 and src_ptr % 16 == 0 and dst_ptr % 16 == 0
