@@ -39,6 +39,8 @@ extern "C" {
 
 #define NNK_F32 0
 #define NNK_F64 1
+#define NNK_I32 2 /* integer element types: inputs of nnk_mulaw's inverse quantiser only       */
+#define NNK_I64 3
 
 #define NNK_MAX_WIN 4  /* windows per stream (static, delta, delta-delta, +1)                  */
 #define NNK_MAX_HALF 4 /* max(l, u) of any window                                              */
@@ -399,6 +401,25 @@ int nnk_frame_stats(const void* X, int32_t dtype, int32_t D, int64_t ld, const i
                     int64_t workspace_bytes, void* stream);
 int nnk_column_affine(const void* x, int32_t x_dtype, int32_t dtype, int64_t n_rows, int32_t D, const void* a,
                       const void* b, int32_t form, void* out, void* stream);
+
+/* ---- waveform and F0 preprocessing (csrc/nnk_wave.cu; DESIGN.md 3.13) -------------------------------
+ * nnk_f0_interp: preprocessing.interp1d on B padded rows of T_max frames (row-major, contiguous); row b
+ * is interpolated over [0, lengths[b]) (lengths NULL: T_max), later frames are copied.  kind 0 linear,
+ * 1 slinear, 2 zero, 3 nearest, 4 nearest-up, 5 previous, 6 next.  Bit-identical to scipy.
+ * nnk_preemphasis: pre-emphasis (inverse 0) or its inverse (inverse 1) along rows of T_max samples,
+ * row b over [0, lengths[b]); bit-identical to scipy.signal.lfilter in the input dtype.  The inverse
+ * needs the workspace and a 2-word device counter (chunks rerun, samples rewritten by the repair walk).
+ * nnk_mulaw: mode 0 mulaw, 1 inv_mulaw, 2 mulaw_quantize (int64 out), 3 inv_mulaw_quantize; variant
+ * 0 = float32 NumPy chain (float64 result), 1 = float32 chain, 2 = float64 chain.                    */
+int64_t nnk_f0_interp_workspace_bytes(int32_t B, int32_t T_max);
+int nnk_f0_interp(const void* x, void* out, int32_t dtype, int32_t B, int32_t T_max, const int32_t* lengths,
+                  int32_t kind, void* workspace, int64_t workspace_bytes, void* stream);
+int64_t nnk_preemphasis_workspace_bytes(int32_t dtype, int64_t rows, int64_t T_max, double coef, int32_t inverse);
+int nnk_preemphasis(const void* x, void* out, int32_t dtype, int64_t rows, int64_t T_max, const int32_t* lengths,
+                    double coef, int32_t inverse, void* workspace, int64_t workspace_bytes,
+                    unsigned long long* counters, void* stream);
+int nnk_mulaw(const void* x, int32_t in_type, void* out, int32_t mode, int32_t variant, int64_t n, double mu,
+              void* stream);
 
 /* ---- sharded batches (SURVEY.md 8e; the reference has no multi-device path) ------------------------
  * Copies n_seg row segments (whole utterances) between two row-major device matrices:

@@ -13,6 +13,7 @@ LIB_PATH = os.environ.get("NNK_LIB_PATH") or os.path.join(_HERE, "libnnk_b200.so
 
 NNK_OK, NNK_ERR_ARG, NNK_ERR_UNSUPPORTED, NNK_ERR_CUDA, NNK_ERR_WORKSPACE, NNK_ERR_NOT_PD = 0, -1, -2, -3, -4, -5
 NNK_F32, NNK_F64 = 0, 1
+NNK_I32, NNK_I64 = 2, 3
 NNK_MAX_WIN, NNK_MAX_HALF = 4, 4
 NNK_MAX_TAPS = 2 * NNK_MAX_HALF + 1
 ABI_VERSION = 2
@@ -162,6 +163,7 @@ EXPORTS = [
     "nnk_kmeans_average", "nnk_kmeans_inertia",
     "nnk_postfilter_basis_elems", "nnk_postfilter_basis", "nnk_postfilter_apply",
     "nnk_frame_stats_workspace_bytes", "nnk_frame_stats", "nnk_column_affine",
+    "nnk_f0_interp_workspace_bytes", "nnk_f0_interp", "nnk_preemphasis_workspace_bytes", "nnk_preemphasis", "nnk_mulaw",
     "nnk_peer_alloc", "nnk_peer_free", "nnk_peer_export", "nnk_peer_open", "nnk_peer_close", "nnk_peer_copy",
 ]
 
@@ -255,6 +257,16 @@ def _load():
     L.nnk_frame_stats.argtypes = [vp, i32, i32, i64, vp, vp, i32, i32, vp, vp, i64, vp]
     L.nnk_column_affine.restype = ctypes.c_int
     L.nnk_column_affine.argtypes = [vp, i32, i32, i64, i32, vp, vp, i32, vp, vp]
+    L.nnk_f0_interp_workspace_bytes.restype = i64
+    L.nnk_f0_interp_workspace_bytes.argtypes = [i32, i32]
+    L.nnk_f0_interp.restype = ctypes.c_int
+    L.nnk_f0_interp.argtypes = [vp, vp, i32, i32, i32, vp, i32, vp, i64, vp]
+    L.nnk_preemphasis_workspace_bytes.restype = i64
+    L.nnk_preemphasis_workspace_bytes.argtypes = [i32, i64, i64, ctypes.c_double, i32]
+    L.nnk_preemphasis.restype = ctypes.c_int
+    L.nnk_preemphasis.argtypes = [vp, vp, i32, i64, i64, vp, ctypes.c_double, i32, vp, i64, vp, vp]
+    L.nnk_mulaw.restype = ctypes.c_int
+    L.nnk_mulaw.argtypes = [vp, i32, vp, i32, i32, i64, ctypes.c_double, vp]
     L.nnk_segment_copy.restype = ctypes.c_int
     L.nnk_segment_copy.argtypes = [vp, vp, i32, i64, i64, i64, vp, vp, vp, i32, i32, vp]
     return L

@@ -1,6 +1,7 @@
 """Pre-processing pieces on the DTW hot path (drop-in for the names the aligners need from
-``nnmnkwii.preprocessing``) and corpus normalisation (``normalize``: meanvar / meanstd / minmax and the
-scale family)."""
+``nnmnkwii.preprocessing``), corpus normalisation (``normalize``: meanvar / meanstd / minmax and the
+scale family), F0 interpolation (``f0``), pre-emphasis and mu-law (``waveform``) and the frame-length
+helpers."""
 import numpy as np
 
 
@@ -17,6 +18,53 @@ def trim_zeros_frames(x, eps=1e-7, trim="b"):
     first = live[0] if "f" in trim else 0
     last = live[-1] + 1 if "b" in trim else len(x)
     return x if (first == 0 and last == len(x)) else x[first:last]
+
+
+def _pad_end(x, n, kwargs):
+    return np.pad(x, (0, n) if x.ndim == 1 else [(0, n), (0, 0)], **kwargs)
+
+
+def adjust_frame_length(x, pad=True, divisible_by=1, **kwargs):
+    """Pad (``pad=True``) or trim the end of a ``(T,)`` or ``(T, D)`` array so that its length is divisible
+    by ``divisible_by`` (nnmnkwii/preprocessing/generic.py:359-414).  ``kwargs`` go to :func:`numpy.pad`
+    (default ``mode="constant"``).  Host-side, NumPy only, the reference's semantics."""
+    kwargs.setdefault("mode", "constant")
+    assert x.ndim == 2 or x.ndim == 1
+    Tx = x.shape[0]
+    T = Tx
+    if divisible_by > 1 and Tx % divisible_by:
+        T = Tx + divisible_by - Tx % divisible_by if pad else Tx - Tx % divisible_by
+    if T > Tx:
+        return _pad_end(x, T - Tx, kwargs)
+    return x[:T] if T < Tx else x
+
+
+def adjust_frame_lengths(x, y, pad=True, ensure_even=False, divisible_by=1, **kwargs):
+    """Give two ``(T, D)`` (or ``(T,)``) arrays the same length, divisible by ``divisible_by``, by padding
+    both to the longer (``pad=True``) or trimming both to the shorter (nnmnkwii/preprocessing/generic.py:
+    417-493).  ``ensure_even`` (deprecated) means ``divisible_by=2``.  Host-side, NumPy only."""
+    assert x.ndim in [1, 2] and y.ndim in [1, 2]
+    kwargs.setdefault("mode", "constant")
+    Tx, Ty = x.shape[0], y.shape[0]
+    if x.ndim == 2:
+        assert x.shape[-1] == y.shape[-1]
+    if ensure_even:
+        divisible_by = 2
+    if pad:
+        T = max(Tx, Ty)
+        if divisible_by > 1 and T % divisible_by:
+            T += divisible_by - T % divisible_by
+    else:
+        T = min(Tx, Ty)
+        if divisible_by > 1:
+            T -= T % divisible_by
+    x = _pad_end(x, T - Tx, kwargs) if Tx < T else x[:T] if Tx > T else x
+    y = _pad_end(y, T - Ty, kwargs) if Ty < T else y[:T] if Ty > T else y
+    return x, y
+
+
+adjast_frame_length = adjust_frame_length  # deprecated spellings, kept by the reference
+adjast_frame_lengths = adjust_frame_lengths
 
 
 def delta_features(x, windows, lengths=None):
@@ -67,6 +115,11 @@ def delta_features(x, windows, lengths=None):
 
 from .normalize import (inv_minmax_scale, inv_scale, meanstd, meanvar, minmax, minmax_scale,  # noqa: E402
                         minmax_scale_params, remove_zeros_frames, scale)
+from .f0 import interp1d  # noqa: E402
+from .waveform import (inv_mulaw, inv_mulaw_quantize, inv_preemphasis, mulaw, mulaw_quantize,  # noqa: E402
+                       preemphasis)
 
 __all__ = ["trim_zeros_frames", "delta_features", "meanvar", "meanstd", "minmax", "scale", "inv_scale",
-           "minmax_scale_params", "minmax_scale", "inv_minmax_scale", "remove_zeros_frames"]
+           "minmax_scale_params", "minmax_scale", "inv_minmax_scale", "remove_zeros_frames", "interp1d",
+           "preemphasis", "inv_preemphasis", "mulaw", "inv_mulaw", "mulaw_quantize", "inv_mulaw_quantize",
+           "adjust_frame_length", "adjust_frame_lengths", "adjast_frame_length", "adjast_frame_lengths"]
