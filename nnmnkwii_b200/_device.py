@@ -8,7 +8,7 @@ import torch
 from . import _lib
 from ._lib import CHAIN_DTYPE, NnkMlpgArgs, NnkStatus, lib
 
-_chain_cache = {}
+_const_cache = {}
 
 WORKSPACE_CAP_BYTES = 2 << 30  # the launcher splits a batch into waves if it needs more
 
@@ -18,6 +18,65 @@ def require_cuda():
         raise RuntimeError(
             "nnmnkwii_b200 needs a CUDA device (H100, sm_90a): there is no CPU fallback. "
             "torch.cuda.is_available() is False.")
+
+
+# ---- the array boundary: caller's NumPy arrays / tensors <-> device tensors -----------------------------
+def is_tensor(x):
+    return type(x).__module__.startswith("torch")
+
+
+def np_dtype(x):
+    """NumPy dtype of an array or tensor."""
+    return np.dtype(str(x.dtype).replace("torch.", "")) if is_tensor(x) else np.asarray(x).dtype
+
+
+def cuda_device(x=None):
+    """The CUDA device of tensor ``x`` if it is on one, otherwise the current device."""
+    if is_tensor(x) and x.is_cuda:
+        return x.device
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+def to_device(x, device=None):
+    """``x`` as a device tensor of its own dtype, not copied where it can be avoided: a tensor is detached (a
+    CUDA tensor stays on its device, a CPU tensor goes to ``device`` or the current device); an array is
+    made contiguous and uploaded."""
+    if is_tensor(x):
+        return x.detach() if x.is_cuda else x.detach().to(device or cuda_device())
+    return torch.from_numpy(np.ascontiguousarray(x)).to(device or cuda_device())
+
+
+def like_input(out, x):
+    """Device result ``out`` in the form of input ``x``: CUDA tensor, CPU tensor or NumPy array."""
+    if is_tensor(x):
+        return out if x.is_cuda else out.cpu()
+    return out.cpu().numpy()
+
+
+def check_lengths(lengths, n_items):
+    if lengths is None:
+        return None
+    if is_tensor(lengths):
+        lengths = lengths.detach().cpu().numpy()
+    lens = np.asarray(lengths)
+    if lens.ndim != 1 or (lens.size and not np.issubdtype(lens.dtype, np.integer)):
+        raise ValueError("lengths must be a 1-D sequence of integers")
+    lens = lens.astype(np.int64)
+    if n_items is None:
+        raise ValueError("lengths needs a sized dataset (len(dataset))")
+    if len(lens) != n_items:
+        raise ValueError("lengths has %d entries for %d items" % (len(lens), n_items))
+    if lens.size and int(lens.min()) < 0:
+        raise ValueError("lengths must be >= 0")
+    return lens
+
+
+def lengths_on(lens, device, T=None):
+    """Host lengths as an int32 device tensor, clipped to ``T`` when given; None stays None."""
+    if lens is None:
+        return None
+    lens = np.asarray(lens)
+    return torch.as_tensor((lens if T is None else np.minimum(lens, T)).astype(np.int32), device=device)
 
 
 def current_stream_ptr(device):
@@ -43,21 +102,27 @@ def simple_chains(static_dim):
     return ch
 
 
-def chains_on_device(chains_np, device):
-    key = (chains_np.tobytes(), str(device))
-    t = _chain_cache.get(key)
+def constant_on_device(a, device):
+    """Device copy of a small host constant (chain table, filter weights), kept in a bounded cache."""
+    key = (a.tobytes(), a.dtype.str, a.shape, str(device))
+    t = _const_cache.get(key)
     if t is None:
-        t = torch.from_numpy(chains_np.view(np.int32).reshape(-1, 4).copy()).to(device)
-        if len(_chain_cache) > 64:
-            _chain_cache.clear()
-        _chain_cache[key] = t
+        t = torch.from_numpy(a.copy()).to(device)
+        if len(_const_cache) >= 64:
+            _const_cache.clear()
+        _const_cache[key] = t
     return t
 
 
+def chains_on_device(chains_np, device):
+    return constant_on_device(chains_np.view(np.int32).reshape(-1, 4), device)
+
+
 def torch_dtype_code(dt):
-    if dt == torch.float32:
+    """C-ABI dtype code of a torch or NumPy dtype."""
+    if dt in (torch.float32, np.float32):
         return _lib.NNK_F32
-    if dt == torch.float64:
+    if dt in (torch.float64, np.float64):
         return _lib.NNK_F64
     raise TypeError("CUDA kernels support float32 / float64, got %s" % dt)
 
@@ -143,7 +208,6 @@ def run_mlpg(mode, *, means, variances, rhs, out, offsets, lengths, order, chain
     need = lib.nnk_mlpg_workspace_bytes(n_utt, n_chain, max_T, ctypes.byref(windows_c))
     if need == 0 and n_utt and n_chain and max_T:
         raise NotImplementedError("window set not supported by the CUDA kernels")
-    groups = (n_chain + 31) // 32
     per_utt = need // max(1, n_utt)
     nbytes = max(per_utt, min(need, max(WORKSPACE_CAP_BYTES, per_utt)))
     ws = workspace(device, max(nbytes, 256))
@@ -154,7 +218,6 @@ def run_mlpg(mode, *, means, variances, rhs, out, offsets, lengths, order, chain
     a.status_word = status.data_ptr()
     fn = {"fwd": lib.nnk_mlpg_fwd, "grad": lib.nnk_mlpg_grad, "solve": lib.nnk_mlpg_solve}[mode]
     _lib.check(fn(ctypes.byref(a), current_stream_ptr(device)), "nnk_mlpg_" + mode)
-    del groups
     if check == "deferred":
         _defer_check(status, device)
     elif check:

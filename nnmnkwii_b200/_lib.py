@@ -151,21 +151,69 @@ class NnkDtwArgs(ctypes.Structure):
 
 CHAIN_DTYPE = np.dtype([("in_col", np.int32), ("win_stride", np.int32), ("out_col", np.int32), ("flags", np.int32)])
 
-# every symbol include/nnk_b200.h declares (tests check the library exports all of them)
-EXPORTS = [
-    "nnk_abi_version", "nnk_last_error", "nnk_launch_count", "nnk_status_decode",
-    "nnk_mlpg_fwd", "nnk_mlpg_grad", "nnk_mlpg_solve", "nnk_mlpg_workspace_bytes", "nnk_mlpg_host", "nnk_mlpg_batch_host",
-    "nnk_uv_band_profile", "nnk_uv_band_extract", "nnk_uv_apply", "nnk_uv_apply_toeplitz", "nnk_uv_apply_factored",
-    "nnk_dtw_align", "nnk_dtw_workspace_bytes", "nnk_gather_rows", "nnk_trim_lengths", "nnk_delta_features",
-    "nnk_metric_workspace_bytes", "nnk_frame_metric", "nnk_f0_metric", "nnk_segment_copy", "nnk_gmm_logprob", "nnk_gmm_map",
-    "nnk_gmm_em_workspace_bytes", "nnk_gmm_em_estep", "nnk_gmm_em_mstep", "nnk_gmm_em_factor",
-    "nnk_kmeans_workspace_bytes", "nnk_kmeans_prepare", "nnk_kmeans_seed", "nnk_kmeans_lloyd", "nnk_kmeans_relocate_dist",
-    "nnk_kmeans_average", "nnk_kmeans_inertia",
-    "nnk_postfilter_basis_elems", "nnk_postfilter_basis", "nnk_postfilter_apply",
-    "nnk_frame_stats_workspace_bytes", "nnk_frame_stats", "nnk_column_affine",
-    "nnk_f0_interp_workspace_bytes", "nnk_f0_interp", "nnk_preemphasis_workspace_bytes", "nnk_preemphasis", "nnk_mulaw",
-    "nnk_peer_alloc", "nnk_peer_free", "nnk_peer_export", "nnk_peer_open", "nnk_peer_close", "nnk_peer_copy",
-]
+P, vp, i32, i64, f64 = ctypes.POINTER, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_double
+size_t = ctypes.c_size_t
+_MLPG, _GMM_EM, _KMEANS = [P(NnkMlpgArgs), vp], [P(NnkGmmEmArgs), vp], [P(NnkKmeansArgs), vp]
+
+# name -> (restype, argtypes) of every function include/nnk_b200.h declares (tests check both against it)
+SIGNATURES = {
+    "nnk_abi_version": (ctypes.c_int, []),
+    "nnk_last_error": (ctypes.c_char_p, []),
+    "nnk_launch_count": (i64, []),
+    "nnk_status_decode": (None, [ctypes.c_uint64, P(NnkStatus)]),
+    "nnk_mlpg_fwd": (ctypes.c_int, _MLPG),
+    "nnk_mlpg_grad": (ctypes.c_int, _MLPG),
+    "nnk_mlpg_solve": (ctypes.c_int, _MLPG),
+    "nnk_mlpg_workspace_bytes": (size_t, [i32, i32, i32, P(NnkWindows)]),
+    "nnk_mlpg_host": (ctypes.c_int, [vp, vp, i32, i32, i64, i64, P(NnkWindows), vp, P(i32)]),
+    "nnk_mlpg_batch_host": (ctypes.c_int, [vp, vp, i32, i32, i64, i64, i64, vp, i32, vp, i32, P(NnkWindows), vp,
+                                           P(NnkStatus)]),
+    "nnk_uv_band_profile": (ctypes.c_int, [vp, i32, i32, i32, vp, vp]),
+    "nnk_uv_band_extract": (ctypes.c_int, [vp, i32, i32, i32, i32, vp, vp, vp]),
+    "nnk_uv_apply": (ctypes.c_int, [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp]),
+    "nnk_uv_apply_toeplitz": (ctypes.c_int, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp]),
+    "nnk_uv_apply_factored": (ctypes.c_int, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp]),
+    "nnk_dtw_align": (ctypes.c_int, [P(NnkDtwArgs), vp]),
+    "nnk_dtw_workspace_bytes": (size_t, [i32, i32, i32, i32, i32]),
+    "nnk_gather_rows": (ctypes.c_int, [vp, i32, i64, i32, vp, i32, vp, vp, i64, i32, i32, i32, vp]),
+    "nnk_trim_lengths": (ctypes.c_int, [vp, i32, i64, i32, i32, i32, f64, i32, vp, vp]),
+    "nnk_delta_features": (ctypes.c_int, [vp, i32, i32, i64, vp, vp, i32, i32, P(NnkWindows), vp, i64, vp]),
+    "nnk_metric_workspace_bytes": (i64, [i32, i32]),
+    "nnk_frame_metric": (ctypes.c_int, [vp, vp, i32, i32, i32, i32, i64, i64, vp, i32, vp, vp, vp, i64, vp]),
+    "nnk_f0_metric": (ctypes.c_int, [vp, vp, vp, vp, i32, i32, i32, i64, i64, vp, i32, vp, vp, vp, i64, vp]),
+    "nnk_segment_copy": (ctypes.c_int, [vp, vp, i32, i64, i64, i64, vp, vp, vp, i32, i32, vp]),
+    "nnk_gmm_logprob": (ctypes.c_int, [P(NnkGmm), vp, i64, i32, vp, vp]),
+    "nnk_gmm_map": (ctypes.c_int, [P(NnkGmm), vp, i64, i32, vp, i32, vp, vp, vp, vp]),
+    "nnk_gmm_em_workspace_bytes": (size_t, [i64, i32, i32]),
+    "nnk_gmm_em_estep": (ctypes.c_int, _GMM_EM),
+    "nnk_gmm_em_mstep": (ctypes.c_int, _GMM_EM),
+    "nnk_gmm_em_factor": (ctypes.c_int, _GMM_EM),
+    "nnk_kmeans_workspace_bytes": (size_t, [i64, i32, i32]),
+    "nnk_kmeans_prepare": (ctypes.c_int, _KMEANS),
+    "nnk_kmeans_seed": (ctypes.c_int, _KMEANS),
+    "nnk_kmeans_lloyd": (ctypes.c_int, _KMEANS),
+    "nnk_kmeans_relocate_dist": (ctypes.c_int, _KMEANS),
+    "nnk_kmeans_average": (ctypes.c_int, _KMEANS),
+    "nnk_kmeans_inertia": (ctypes.c_int, _KMEANS),
+    "nnk_postfilter_basis_elems": (i64, [i32, i32]),
+    "nnk_postfilter_basis": (ctypes.c_int, [f64, i32, i32, i32, vp, i64, vp]),
+    "nnk_postfilter_apply": (ctypes.c_int, [vp, i32, i64, i32, i64, vp, i32, vp, i64, vp, i64, vp]),
+    "nnk_frame_stats_workspace_bytes": (i64, [i32, i32, i32]),
+    "nnk_frame_stats": (ctypes.c_int, [vp, i32, i32, i64, vp, vp, i32, i32, vp, vp, i64, vp]),
+    "nnk_column_affine": (ctypes.c_int, [vp, i32, i32, i64, i32, vp, vp, i32, vp, vp]),
+    "nnk_f0_interp_workspace_bytes": (i64, [i32, i32]),
+    "nnk_f0_interp": (ctypes.c_int, [vp, vp, i32, i32, i32, vp, i32, vp, i64, vp]),
+    "nnk_preemphasis_workspace_bytes": (i64, [i32, i64, i64, f64, i32]),
+    "nnk_preemphasis": (ctypes.c_int, [vp, vp, i32, i64, i64, vp, f64, i32, vp, i64, vp, vp]),
+    "nnk_mulaw": (ctypes.c_int, [vp, i32, vp, i32, i32, i64, f64, vp]),
+    "nnk_peer_alloc": (ctypes.c_int, [size_t, P(vp)]),
+    "nnk_peer_free": (ctypes.c_int, [vp]),
+    "nnk_peer_export": (ctypes.c_int, [vp, vp]),
+    "nnk_peer_open": (ctypes.c_int, [vp, P(vp)]),
+    "nnk_peer_close": (ctypes.c_int, [vp]),
+    "nnk_peer_copy": (ctypes.c_int, [vp, vp, size_t, vp]),
+}
+EXPORTS = list(SIGNATURES)
 
 
 class NnkError(RuntimeError):
@@ -181,94 +229,9 @@ def _load():
     L.nnk_abi_version.restype = ctypes.c_int
     if L.nnk_abi_version() != ABI_VERSION:
         raise ImportError("libnnk_b200.so ABI %d != binding ABI %d: rebuild" % (L.nnk_abi_version(), ABI_VERSION))
-    vp, i32, i64 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64
-    L.nnk_last_error.restype = ctypes.c_char_p
-    L.nnk_launch_count.restype = ctypes.c_int64
-    L.nnk_status_decode.restype = None
-    L.nnk_status_decode.argtypes = [ctypes.c_uint64, ctypes.POINTER(NnkStatus)]
-    L.nnk_mlpg_fwd.restype = ctypes.c_int
-    L.nnk_mlpg_fwd.argtypes = [ctypes.POINTER(NnkMlpgArgs), vp]
-    L.nnk_mlpg_grad.restype = ctypes.c_int
-    L.nnk_mlpg_grad.argtypes = [ctypes.POINTER(NnkMlpgArgs), vp]
-    L.nnk_mlpg_solve.restype = ctypes.c_int
-    L.nnk_mlpg_solve.argtypes = [ctypes.POINTER(NnkMlpgArgs), vp]
-    L.nnk_mlpg_workspace_bytes.restype = ctypes.c_size_t
-    L.nnk_mlpg_workspace_bytes.argtypes = [i32, i32, i32, ctypes.POINTER(NnkWindows)]
-    L.nnk_mlpg_host.restype = ctypes.c_int
-    L.nnk_mlpg_host.argtypes = [vp, vp, i32, i32, i64, i64, ctypes.POINTER(NnkWindows), vp, ctypes.POINTER(i32)]
-    L.nnk_mlpg_batch_host.restype = ctypes.c_int
-    L.nnk_mlpg_batch_host.argtypes = [vp, vp, i32, i32, i64, i64, i64, vp, i32, vp, i32,
-                                      ctypes.POINTER(NnkWindows), vp, ctypes.POINTER(NnkStatus)]
-    L.nnk_uv_band_profile.restype = ctypes.c_int
-    L.nnk_uv_band_profile.argtypes = [vp, i32, i32, i32, vp, vp]
-    L.nnk_uv_band_extract.restype = ctypes.c_int
-    L.nnk_uv_band_extract.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp]
-    L.nnk_uv_apply.restype = ctypes.c_int
-    L.nnk_uv_apply.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp]
-    L.nnk_uv_apply_toeplitz.restype = ctypes.c_int
-    L.nnk_uv_apply_toeplitz.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp]
-    L.nnk_uv_apply_factored.restype = ctypes.c_int
-    L.nnk_uv_apply_factored.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp]
-    L.nnk_dtw_align.restype = ctypes.c_int
-    L.nnk_dtw_align.argtypes = [ctypes.POINTER(NnkDtwArgs), vp]
-    L.nnk_dtw_workspace_bytes.restype = ctypes.c_size_t
-    L.nnk_dtw_workspace_bytes.argtypes = [i32, i32, i32, i32, i32]
-    L.nnk_gather_rows.restype = ctypes.c_int
-    L.nnk_gather_rows.argtypes = [vp, i32, i64, i32, vp, i32, vp, vp, i64, i32, i32, i32, vp]
-    L.nnk_trim_lengths.restype = ctypes.c_int
-    L.nnk_trim_lengths.argtypes = [vp, i32, i64, i32, i32, i32, ctypes.c_double, i32, vp, vp]
-    L.nnk_delta_features.restype = ctypes.c_int
-    L.nnk_delta_features.argtypes = [vp, i32, i32, i64, vp, vp, i32, i32, ctypes.POINTER(NnkWindows), vp, i64, vp]
-    L.nnk_metric_workspace_bytes.restype = i64
-    L.nnk_metric_workspace_bytes.argtypes = [i32, i32]
-    L.nnk_frame_metric.restype = ctypes.c_int
-    L.nnk_frame_metric.argtypes = [vp, vp, i32, i32, i32, i32, i64, i64, vp, i32, vp, vp, vp, i64, vp]
-    L.nnk_f0_metric.restype = ctypes.c_int
-    L.nnk_f0_metric.argtypes = [vp, vp, vp, vp, i32, i32, i32, i64, i64, vp, i32, vp, vp, vp, i64, vp]
-    for name, args in (("nnk_peer_alloc", [ctypes.c_size_t, ctypes.POINTER(vp)]), ("nnk_peer_free", [vp]),
-                       ("nnk_peer_export", [vp, vp]), ("nnk_peer_open", [vp, ctypes.POINTER(vp)]), ("nnk_peer_close", [vp]),
-                       ("nnk_peer_copy", [vp, vp, ctypes.c_size_t, vp])):
-        getattr(L, name).restype = ctypes.c_int
-        getattr(L, name).argtypes = args
-    L.nnk_gmm_logprob.restype = ctypes.c_int
-    L.nnk_gmm_logprob.argtypes = [ctypes.POINTER(NnkGmm), vp, i64, i32, vp, vp]
-    L.nnk_gmm_map.restype = ctypes.c_int
-    L.nnk_gmm_map.argtypes = [ctypes.POINTER(NnkGmm), vp, i64, i32, vp, i32, vp, vp, vp, vp]
-    L.nnk_gmm_em_workspace_bytes.restype = ctypes.c_size_t
-    L.nnk_gmm_em_workspace_bytes.argtypes = [i64, i32, i32]
-    for name in ("nnk_gmm_em_estep", "nnk_gmm_em_mstep", "nnk_gmm_em_factor"):
-        getattr(L, name).restype = ctypes.c_int
-        getattr(L, name).argtypes = [ctypes.POINTER(NnkGmmEmArgs), vp]
-    L.nnk_kmeans_workspace_bytes.restype = ctypes.c_size_t
-    L.nnk_kmeans_workspace_bytes.argtypes = [i64, i32, i32]
-    for name in ("nnk_kmeans_prepare", "nnk_kmeans_seed", "nnk_kmeans_lloyd", "nnk_kmeans_relocate_dist",
-                 "nnk_kmeans_average", "nnk_kmeans_inertia"):
-        getattr(L, name).restype = ctypes.c_int
-        getattr(L, name).argtypes = [ctypes.POINTER(NnkKmeansArgs), vp]
-    L.nnk_postfilter_basis_elems.restype = i64
-    L.nnk_postfilter_basis_elems.argtypes = [i32, i32]
-    L.nnk_postfilter_basis.restype = ctypes.c_int
-    L.nnk_postfilter_basis.argtypes = [ctypes.c_double, i32, i32, i32, vp, i64, vp]
-    L.nnk_postfilter_apply.restype = ctypes.c_int
-    L.nnk_postfilter_apply.argtypes = [vp, i32, i64, i32, i64, vp, i32, vp, i64, vp, i64, vp]
-    L.nnk_frame_stats_workspace_bytes.restype = i64
-    L.nnk_frame_stats_workspace_bytes.argtypes = [i32, i32, i32]
-    L.nnk_frame_stats.restype = ctypes.c_int
-    L.nnk_frame_stats.argtypes = [vp, i32, i32, i64, vp, vp, i32, i32, vp, vp, i64, vp]
-    L.nnk_column_affine.restype = ctypes.c_int
-    L.nnk_column_affine.argtypes = [vp, i32, i32, i64, i32, vp, vp, i32, vp, vp]
-    L.nnk_f0_interp_workspace_bytes.restype = i64
-    L.nnk_f0_interp_workspace_bytes.argtypes = [i32, i32]
-    L.nnk_f0_interp.restype = ctypes.c_int
-    L.nnk_f0_interp.argtypes = [vp, vp, i32, i32, i32, vp, i32, vp, i64, vp]
-    L.nnk_preemphasis_workspace_bytes.restype = i64
-    L.nnk_preemphasis_workspace_bytes.argtypes = [i32, i64, i64, ctypes.c_double, i32]
-    L.nnk_preemphasis.restype = ctypes.c_int
-    L.nnk_preemphasis.argtypes = [vp, vp, i32, i64, i64, vp, ctypes.c_double, i32, vp, i64, vp, vp]
-    L.nnk_mulaw.restype = ctypes.c_int
-    L.nnk_mulaw.argtypes = [vp, i32, vp, i32, i32, i64, ctypes.c_double, vp]
-    L.nnk_segment_copy.restype = ctypes.c_int
-    L.nnk_segment_copy.argtypes = [vp, vp, i32, i64, i64, i64, vp, vp, vp, i32, i32, vp]
+    for name, (restype, argtypes) in SIGNATURES.items():
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
     return L
 
 

@@ -13,14 +13,8 @@ import numpy as np
 import torch
 from torch.autograd import Function
 
+from . import _device as dev
 from . import paramgen as G
-
-
-def _cuda_device(t):
-    from . import _device as dev
-
-    dev.require_cuda()
-    return t.device if t.is_cuda else torch.device("cuda", torch.cuda.current_device())
 
 
 def _global_variance(variances):
@@ -45,7 +39,8 @@ class MLPG(Function):
         variances = _global_variance(variances)  # (D,) or a stride-0 expansion of it -> 1-D (16*sd B/frame path)
         ctx.save_for_backward(means, variances)
         assert variances.dim() == 1 or means.size() == variances.size()
-        device = _cuda_device(means)
+        dev.require_cuda()
+        device = dev.cuda_device(means)
         m = means.detach().to(device)
         v = variances.detach().to(device)
         # CUDA inputs: non-blocking status check (surfaces at the next call); CPU inputs (the reference's
@@ -57,7 +52,8 @@ class MLPG(Function):
     @staticmethod
     def backward(ctx, grad_output):
         means, variances = ctx.saved_tensors
-        device = _cuda_device(means)
+        dev.require_cuda()
+        device = dev.cuda_device(means)
         g = G.mlpg_grad(means.detach().to(device), variances.detach().to(device), ctx.windows,
                         grad_output.detach().to(device), check=ctx.check)
         return g.to(means.device), None, None
@@ -75,7 +71,8 @@ class MLPGBatch(Function):
         ctx.windows = windows
         ctx.lengths = [int(n) for n in (lengths.tolist() if torch.is_tensor(lengths) else lengths)]
         ctx.save_for_backward(means, variances)
-        device = _cuda_device(means)
+        dev.require_cuda()
+        device = dev.cuda_device(means)
         ctx.check = "deferred" if means.is_cuda else True
         y = G.mlpg_batch(means.detach().to(device), variances.detach().to(device), windows, lengths=ctx.lengths,
                          check=ctx.check)
@@ -84,7 +81,8 @@ class MLPGBatch(Function):
     @staticmethod
     def backward(ctx, grad_output):
         means, variances = ctx.saved_tensors
-        device = _cuda_device(means)
+        dev.require_cuda()
+        device = dev.cuda_device(means)
         g = G.mlpg_grad_batch(variances.detach().to(device), ctx.windows, grad_output.detach().to(device), ctx.lengths,
                               check=ctx.check)
         return g.to(means.device), None, None, None
@@ -113,7 +111,8 @@ class UnitVarianceMLPG(Function):
             B, T_, D = means.shape
             means3 = means
         reshaped = not (T == T_)  # mlpg.py:123: input already (T*nw, static_dim)?
-        device = _cuda_device(means)
+        dev.require_cuda()
+        device = dev.cuda_device(means)
         band = uv.band_of(R, device)
         out = uv.apply_forward(band, means3.detach().to(device), reshaped).to(means.device)
         ctx.reshaped = reshaped
@@ -134,7 +133,8 @@ class UnitVarianceMLPG(Function):
             grad_output = grad_output.reshape(B, T, -1)
         else:
             B, T_, D = means.shape
-        device = _cuda_device(means)
+        dev.require_cuda()
+        device = dev.cuda_device(means)
         band = uv.band_of(R, device)
         grad = uv.apply_backward(band, grad_output.detach().to(device), ctx.reshaped, D).to(means.device)
         if dim == 2:

@@ -72,7 +72,7 @@ class MLPGBase(object):
 
         from .. import _device as dev
         dev.require_cuda()
-        device = torch.device("cuda", torch.cuda.current_device())
+        device = dev.cuda_device()
         if self._dev is not None and self._dev["device"] == device:
             return self._dev
 
@@ -287,7 +287,7 @@ def _as_frames(X):
     if isinstance(X, torch.Tensor):
         X = X.numpy()
     Xh = check_array(X, dtype=[np.float64, np.float32], ensure_min_samples=2, estimator="GaussianMixture")
-    return torch.from_numpy(np.ascontiguousarray(Xh)).to(torch.device("cuda", torch.cuda.current_device())), Xh
+    return dev.to_device(Xh), Xh
 
 
 def _host_f64(t):

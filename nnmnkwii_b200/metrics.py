@@ -19,17 +19,6 @@ _logdb_const = 10.0 / np.log(10.0) * np.sqrt(2.0)  # metrics/__init__.py:5
 _ws_cache = {}
 
 
-def _dev(x, device=None):
-    import torch
-    if isinstance(x, torch.Tensor):
-        t = x.detach()
-    else:
-        t = torch.from_numpy(np.ascontiguousarray(np.asarray(x)))
-    if not t.is_cuda:
-        t = t.to(device if device is not None else torch.device("cuda", torch.cuda.current_device()))
-    return t
-
-
 def _prepare(arrays):
     """Move to one device, promote to a common float dtype, make contiguous."""
     import torch
@@ -41,7 +30,7 @@ def _prepare(arrays):
         if isinstance(a, torch.Tensor) and a.is_cuda:
             device = a.device
             break
-    ts = [_dev(a, device) for a in arrays]
+    ts = [dev.to_device(a, device) for a in arrays]
     dt = torch.float32 if all(t.dtype == torch.float32 for t in ts) else torch.float64
     return [t.to(dt).contiguous() for t in ts], ts[0].device, dt
 

@@ -32,10 +32,6 @@ __all__ = [
 ]
 
 
-def _is_torch(x):
-    return type(x).__module__.startswith("torch")
-
-
 def build_win_mats(windows, T):
     """Builds a window matrix of a given size for each window in a collection (_mlpg.py:13-50).
 
@@ -67,7 +63,8 @@ def reshape_means(means, static_dim):
     T, D = means.shape
     if D == static_dim:
         return means
-    if _is_torch(means):
+    from ._device import is_tensor
+    if is_tensor(means):
         return means.reshape(T, -1, static_dim).transpose(0, 1).reshape(-1, static_dim)
     return means.reshape(T, -1, static_dim).transpose(1, 0, 2).reshape(-1, static_dim)
 
@@ -122,12 +119,23 @@ def _offsets_from(lengths=None, offsets=None, n_rows=None):
     return np.ascontiguousarray(off)
 
 
-def _np_dtype_code(dt):
-    if dt == np.float32:
-        return _lib.NNK_F32
-    if dt == np.float64:
-        return _lib.NNK_F64
-    return None
+def _utterance_table(lengths, offsets, n_rows, padded=None):
+    """Host table of the utterances of a batch: ``(offsets, lengths, order, max_T, n_utt)`` with ``order``
+    longest first.  ``padded=(B, Tmax)``: utterance b has ``lengths[b] <= Tmax`` frames from row
+    ``b * Tmax``; otherwise ``lengths`` / ``offsets`` (default: one utterance) cover the ``n_rows`` rows
+    back to back.  The kernels index rows, ``order`` and lengths from this table: it is checked here."""
+    from ._device import is_tensor
+    lengths, offsets = (a.cpu().numpy() if is_tensor(a) else a for a in (lengths, offsets))
+    if padded:
+        B, Tmax = padded
+        lens = np.asarray(lengths, dtype=np.int64)
+        assert len(lens) == B and lens.max(initial=0) <= Tmax
+        off = np.arange(B + 1, dtype=np.int64) * Tmax
+    else:
+        off = _offsets_from(lengths, offsets, n_rows)
+        assert off[0] == 0 and off[-1] == n_rows
+        lens = np.diff(off)
+    return off, lens, np.argsort(-lens, kind="stable").astype(np.int32), int(lens.max(initial=0)), len(lens)
 
 
 def mlpg_batch(means, variances, windows, lengths=None, offsets=None, layout=None, check=True, out=None):
@@ -146,6 +154,7 @@ def mlpg_batch(means, variances, windows, lengths=None, offsets=None, layout=Non
     Returns:
         ``(sum_T, D_out)`` (or ``(B, Tmax, D_out)``) array / tensor of the input dtype.
     """
+    from ._device import is_tensor, torch_dtype_code
     padded = means.ndim == 3
     D = means.shape[-1]
     if layout is None:
@@ -154,12 +163,11 @@ def mlpg_batch(means, variances, windows, lengths=None, offsets=None, layout=Non
     if padded:
         assert lengths is not None, "padded (B, Tmax, D) input needs lengths"
         B, Tmax = means.shape[0], means.shape[1]
-    if _is_torch(means):
+    if is_tensor(means):
         return _mlpg_batch_device(means, variances, windows, lengths, offsets, layout, padded, check)
 
     dtype = means.dtype
-    code = _np_dtype_code(dtype)
-    work_dtype = dtype if (code is not None and np.asarray(variances).dtype == dtype) else np.float64
+    work_dtype = dtype if (dtype in (np.float32, np.float64) and np.asarray(variances).dtype == dtype) else np.float64
     m = np.ascontiguousarray(means, dtype=work_dtype)
     v = np.ascontiguousarray(variances, dtype=work_dtype)
     var1d = v.ndim == 1
@@ -170,8 +178,7 @@ def mlpg_batch(means, variances, windows, lengths=None, offsets=None, layout=Non
     wc = _lib.make_windows(windows)
     if padded:
         # zero-padded batch: run on the flat view, one "utterance" per row block
-        lens = np.asarray(lengths, dtype=np.int64)
-        assert len(lens) == B and lens.max(initial=0) <= Tmax
+        lens = _utterance_table(lengths, None, None, (B, Tmax))[1]
         keep = np.concatenate([np.arange(b * Tmax, b * Tmax + lens[b]) for b in range(B)]) if B else np.zeros(0, np.int64)
         flat_m = m.reshape(B * Tmax, D)[keep]
         flat_v = v if var1d else v.reshape(B * Tmax, D)[keep]
@@ -180,8 +187,7 @@ def mlpg_batch(means, variances, windows, lengths=None, offsets=None, layout=Non
         out[keep] = y
         return out.reshape(B, Tmax, layout.D_out)
     n_rows = m.shape[0]
-    off = _offsets_from(lengths, offsets, n_rows)
-    assert off[0] == 0 and off[-1] == n_rows
+    off = _utterance_table(lengths, offsets, n_rows)[0]
     if out is not None and (out.shape != (n_rows, layout.D_out) or out.dtype != work_dtype or not out.flags.c_contiguous):
         raise ValueError("out must be a C-contiguous (%d, %d) array of dtype %s" % (n_rows, layout.D_out, work_dtype))
     if out is None:
@@ -189,7 +195,7 @@ def mlpg_batch(means, variances, windows, lengths=None, offsets=None, layout=Non
     st = _lib.NnkStatus()
     chains = np.ascontiguousarray(layout.chains)
     rc = _lib.lib.nnk_mlpg_batch_host(
-        m.ctypes.data, v.ctypes.data, int(var1d), _np_dtype_code(np.dtype(work_dtype)), n_rows, D, layout.D_out,
+        m.ctypes.data, v.ctypes.data, int(var1d), torch_dtype_code(work_dtype), n_rows, D, layout.D_out,
         off.ctypes.data, len(off) - 1, chains.ctypes.data, layout.n_chain, ctypes.byref(wc), out.ctypes.data,
         ctypes.byref(st))
     _lib.check(rc, "nnk_mlpg_batch_host")
@@ -203,6 +209,8 @@ def _mlpg_batch_device(means, variances, windows, lengths, offsets, layout, padd
 
     dev.require_cuda()
     assert means.is_cuda, "torch inputs must be CUDA tensors (no CPU fallback)"
+    n_rows = means.shape[0] * means.shape[1] if padded else means.shape[0]
+    off, lens, order, max_T, n_utt = _utterance_table(lengths, offsets, n_rows, means.shape[:2] if padded else None)
     device = means.device
     dtype = means.dtype
     if dtype not in (torch.float32, torch.float64) or variances.dtype != dtype:
@@ -217,30 +225,11 @@ def _mlpg_batch_device(means, variances, windows, lengths, offsets, layout, padd
         v = v.expand_as(m).contiguous() if v.shape != m.shape else v.contiguous()
     else:
         v = v.contiguous()
-    if padded:
-        B, Tmax = m.shape[0], m.shape[1]
-        lens_np = np.asarray(lengths.cpu() if _is_torch(lengths) else lengths, dtype=np.int64)
-        off_np = np.arange(B + 1, dtype=np.int64) * Tmax
-        n_rows = B * Tmax
-        lens_t = torch.from_numpy(lens_np.astype(np.int32)).to(device)
-        max_T = int(lens_np.max(initial=0))
-    else:
-        n_rows = m.shape[0]
-        if _is_torch(offsets):
-            offsets = offsets.cpu().numpy()
-        if _is_torch(lengths):
-            lengths = lengths.cpu().numpy()
-        off_np = _offsets_from(lengths, offsets, n_rows)
-        lens_np = np.diff(off_np)
-        lens_t = None
-        max_T = int(lens_np.max(initial=0))
-    n_utt = len(off_np) - 1
     out = torch.zeros((n_rows, layout.D_out), dtype=work, device=device)
     if n_utt and max_T and layout.n_chain:
-        order = np.argsort(-lens_np, kind="stable").astype(np.int32)
         dev.run_mlpg(
             "fwd", means=m, variances=v, rhs=None, out=out,
-            offsets=torch.from_numpy(off_np).to(device), lengths=lens_t,
+            offsets=torch.from_numpy(off).to(device), lengths=dev.lengths_on(lens, device) if padded else None,
             order=torch.from_numpy(order).to(device), chains=dev.chains_on_device(layout.chains, device),
             n_chain=layout.n_chain, max_T=max_T, windows_c=_lib.make_windows(windows),
             in_ld=D, var_ld=0 if var1d else D, go_ld=0, out_ld=layout.D_out,
@@ -266,7 +255,8 @@ def mlpg(mean_frames, variance_frames, windows):
     Returns:
         Generated static features ``(T, D // len(windows))`` in the dtype of ``mean_frames``.
     """
-    if _is_torch(mean_frames):
+    from ._device import is_tensor, torch_dtype_code
+    if is_tensor(mean_frames):
         T, D = mean_frames.shape
         if variance_frames.dim() == 1 and variance_frames.shape[0] == D:
             pass
@@ -280,15 +270,14 @@ def mlpg(mean_frames, variance_frames, windows):
     var1d = variance_frames.ndim == 1 and variance_frames.shape[0] == D
     if not var1d:
         assert mean_frames.shape == variance_frames.shape
-    code = _np_dtype_code(dtype)
-    work_dtype = dtype if (code is not None and variance_frames.dtype == dtype) else np.float64
+    work_dtype = dtype if (dtype in (np.float32, np.float64) and variance_frames.dtype == dtype) else np.float64
     m = np.ascontiguousarray(mean_frames, dtype=work_dtype)
     v = np.ascontiguousarray(variance_frames, dtype=work_dtype)
     wc = _lib.make_windows(windows)
     static_dim = D // len(windows)
     y = np.zeros((T, static_dim), dtype=work_dtype)
     bad = ctypes.c_int32(0)
-    rc = _lib.lib.nnk_mlpg_host(m.ctypes.data, v.ctypes.data, int(var1d), _np_dtype_code(np.dtype(work_dtype)),
+    rc = _lib.lib.nnk_mlpg_host(m.ctypes.data, v.ctypes.data, int(var1d), torch_dtype_code(work_dtype),
                                 T, D, ctypes.byref(wc), y.ctypes.data, ctypes.byref(bad))
     _lib.check(rc, "nnk_mlpg_host")
     return y if y.dtype == dtype else y.astype(dtype)
@@ -307,22 +296,16 @@ def mlpg_grad(mean_frames, variance_frames, windows, grad_output, check=True):
     from . import _device as dev
 
     dev.require_cuda()
-    is_t = _is_torch(mean_frames)
-    device = mean_frames.device if is_t and mean_frames.is_cuda else torch.device("cuda", torch.cuda.current_device())
-
-    def to_dev(x, dt=None):
-        t = x if _is_torch(x) else torch.from_numpy(np.ascontiguousarray(x))
-        return t.to(device=device, dtype=dt) if dt is not None else t.to(device)
-
+    device = dev.cuda_device(mean_frames)
     T, D = mean_frames.shape
-    v = to_dev(variance_frames)
+    v = dev.to_device(variance_frames, device).to(device)
     if v.dtype not in (torch.float32, torch.float64):
         v = v.to(torch.float64)
     if v.dim() == 2 and v.shape[0] > 1 and v.stride(0) == 0:
         v = v[0]  # v.expand(T, D) of a global variance (tests/test_autograd.py:191): keep it 1-D
     var1d = v.dim() == 1
     v = v.contiguous()
-    go = to_dev(grad_output)
+    go = dev.to_device(grad_output, device).to(device)
     if go.dtype not in (torch.float32, torch.float64):
         go = go.to(torch.float32)
     go = go.contiguous()
@@ -338,9 +321,7 @@ def mlpg_grad(mean_frames, variance_frames, windows, grad_output, check=True):
             windows_c=_lib.make_windows(windows), in_ld=D, var_ld=0 if var1d else D, go_ld=go.shape[1], out_ld=D,
             dtype_code=dev.torch_dtype_code(v.dtype), go_f64=int(go.dtype == torch.float64), n_utt=1,
             device=device, check=check)
-    if is_t:
-        return out
-    return out.cpu().numpy()
+    return out if dev.is_tensor(mean_frames) else out.cpu().numpy()
 
 
 def mlpg_grad_batch(variances, windows, grad_output, lengths, layout=None, check=True):
@@ -364,10 +345,9 @@ def mlpg_grad_batch(variances, windows, grad_output, lengths, layout=None, check
     from . import _device as dev
 
     dev.require_cuda()
-    assert _is_torch(grad_output) and grad_output.is_cuda, "device tensors only (no CPU fallback)"
+    assert dev.is_tensor(grad_output) and grad_output.is_cuda, "device tensors only (no CPU fallback)"
     device = grad_output.device
     padded = grad_output.dim() == 3
-    lens_np = np.asarray(lengths.cpu() if _is_torch(lengths) else lengths, dtype=np.int64)
     go = grad_output.detach()
     if go.dtype not in (torch.float32, torch.float64):
         go = go.to(torch.float32)
@@ -380,22 +360,11 @@ def mlpg_grad_batch(variances, windows, grad_output, lengths, layout=None, check
     if layout is None:
         layout = StreamLayout.single(D, len(windows))
     assert layout.D_in == D and go.shape[-1] == layout.D_out
-    if padded:
-        B, Tmax = go.shape[0], go.shape[1]
-        off_np = np.arange(B + 1, dtype=np.int64) * Tmax
-        lens_t = torch.from_numpy(lens_np.astype(np.int32)).to(device)
-        n_rows = B * Tmax
-        if not var1d:
-            v = v.expand(B, Tmax, D)
-    else:
-        off_np = _offsets_from(lens_np, None, go.shape[0])
-        lens_t = None
-        n_rows = go.shape[0]
-        if not var1d:
-            v = v.expand(n_rows, D)
+    n_rows = go.shape[0] * go.shape[1] if padded else go.shape[0]
+    off, lens, order, max_T, n_utt = _utterance_table(lengths, None, n_rows, go.shape[:2] if padded else None)
+    if not var1d:
+        v = v.expand(*go.shape[:-1], D)
     v = v.contiguous()  # materialises stride-0 expanded variances
-    max_T = int(lens_np.max(initial=0))
-    n_utt = len(lens_np)
     out = torch.zeros((n_rows, D), dtype=torch.float32, device=device)
     if n_utt and max_T and layout.n_chain:
         # the gradient kernel indexes grad_output by chain: chain c reads column c, so route the
@@ -406,8 +375,8 @@ def mlpg_grad_batch(variances, windows, grad_output, lengths, layout=None, check
             go2 = go2.index_select(1, out_cols).contiguous()
         dev.run_mlpg(
             "grad", means=None, variances=v, rhs=go2, out=out,
-            offsets=torch.from_numpy(off_np).to(device), lengths=lens_t,
-            order=torch.from_numpy(np.argsort(-lens_np, kind="stable").astype(np.int32)).to(device),
+            offsets=torch.from_numpy(off).to(device), lengths=dev.lengths_on(lens, device) if padded else None,
+            order=torch.from_numpy(order).to(device),
             chains=dev.chains_on_device(layout.chains, device), n_chain=layout.n_chain, max_T=max_T,
             windows_c=_lib.make_windows(windows), in_ld=D, var_ld=0 if var1d else D, go_ld=layout.n_chain, out_ld=D,
             dtype_code=dev.torch_dtype_code(v.dtype), go_f64=int(go2.dtype == torch.float64), n_utt=n_utt,
@@ -428,7 +397,7 @@ def unit_variance_mlpg_matrix(windows, T):
     from . import _device as dev
 
     dev.require_cuda()
-    device = torch.device("cuda", torch.cuda.current_device())
+    device = dev.cuda_device()
     nw = len(windows)
     win_mats = build_win_mats(windows, T)
     max_win_width = int(np.max([max(w.l, w.u) for w in win_mats]))

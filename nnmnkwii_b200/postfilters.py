@@ -4,7 +4,6 @@ import numpy as np
 __all__ = ["merlin_post_filter"]
 
 _basis_cache = {}
-_weight_cache = {}
 
 
 def _basis(device, alpha, D, order, fftlen):
@@ -31,18 +30,6 @@ def _basis(device, alpha, D, order, fftlen):
             _basis_cache.clear()
         _basis_cache[key] = b
     return b
-
-
-def _weight_on_device(weight, device):
-    import torch
-    key = (str(device), weight.tobytes())
-    w = _weight_cache.get(key)
-    if w is None:
-        w = torch.from_numpy(weight.copy()).to(device)
-        if len(_weight_cache) >= 32:
-            _weight_cache.clear()
-        _weight_cache[key] = w
-    return w
 
 
 def merlin_post_filter(mgc, alpha, minimum_phase_order=511, fftlen=1024, coef=1.4, weight=None):
@@ -86,13 +73,12 @@ def merlin_post_filter(mgc, alpha, minimum_phase_order=511, fftlen=1024, coef=1.
         raise ValueError("merlin_post_filter: minimum_phase_order must be >= 0, got %d" % order)
     if order + 1 > fftlen:
         raise ValueError("merlin_post_filter: minimum_phase_order + 1 (%d) exceeds fftlen (%d)" % (order + 1, fftlen))
-    if type(weight).__module__.startswith("torch"):
+    if dev.is_tensor(weight):
         weight = weight.detach().cpu().numpy()
     weight = np.ascontiguousarray(weight, dtype=np.float64).ravel()
     dev.require_cuda()
 
-    is_t = type(mgc).__module__.startswith("torch")
-    if is_t:
+    if dev.is_tensor(mgc):
         if not mgc.is_cuda:
             raise ValueError("merlin_post_filter: a torch tensor must be on a CUDA device")
         x = mgc if mgc.dtype in (torch.float32, torch.float64) else mgc.to(torch.float64)
@@ -105,8 +91,8 @@ def merlin_post_filter(mgc, alpha, minimum_phase_order=511, fftlen=1024, coef=1.
     out = torch.empty((T, D), dtype=x.dtype, device=device)
     if T and D:
         basis = _basis(device, alpha, D, order, fftlen)
-        w = _weight_on_device(weight, device)
+        w = dev.constant_on_device(weight, device)
         _lib.check(_lib.lib.nnk_postfilter_apply(x.data_ptr(), dev.torch_dtype_code(x.dtype), T, D, max(x.stride(0), D),
                                                  w.data_ptr(), fftlen, basis.data_ptr(), basis.numel(), out.data_ptr(), D,
                                                  dev.current_stream_ptr(device)), "nnk_postfilter_apply")
-    return out if is_t else out.cpu().numpy()
+    return dev.like_input(out, mgc)

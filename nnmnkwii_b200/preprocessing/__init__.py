@@ -70,9 +70,10 @@ adjast_frame_lengths = adjust_frame_lengths
 def delta_features(x, windows, lengths=None):
     """Compute delta features and combine them (nnmnkwii/preprocessing/generic.py:229-288).
 
-    ``x`` is ``(T, D)`` static features (NumPy array or torch CUDA tensor); ``windows`` is a list of
+    ``x`` is ``(T, D)`` static features (NumPy array or torch tensor); ``windows`` is a list of
     ``(l, u, coeff)`` triples (only ``coeff`` is used, as in the reference) or of plain coefficient
-    arrays.  Returns ``(T, D * len(windows))`` in the dtype of ``x``.  Additive: with ``lengths`` the
+    arrays.  Returns ``(T, D * len(windows))`` in the dtype and form of ``x`` (a CPU tensor is computed on
+    the GPU and comes back as a CPU tensor).  Additive: with ``lengths`` the
     rows of ``x`` are several utterances back to back and the deltas do not cross their boundaries.
     Runs on the GPU (C ABI ``nnk_delta_features``, csrc/nnk_delta.cu).
     """
@@ -87,19 +88,14 @@ def delta_features(x, windows, lengths=None):
     assert len(windows) > 0
     coefs = [np.asarray(w[2] if isinstance(w, tuple) else w, dtype=np.float64).ravel() for w in windows]
     T, D = x.shape
-    is_t = type(x).__module__.startswith("torch")
     lens = np.asarray([T] if lengths is None else lengths, dtype=np.int64)
     assert int(lens.sum()) == T
     for c in coefs:
         if len(lens) and int(lens.min()) < len(c):
             raise ValueError("delta window longer than the utterance (np.correlate 'same' would change the length)")
     wc = _lib.make_windows([((len(c) - 1) // 2, len(c) - 1 - (len(c) - 1) // 2, c) for c in coefs])
-    if is_t:
-        xd = x if x.dtype in (torch.float32, torch.float64) else x.to(torch.float64)
-    else:
-        xn = np.ascontiguousarray(x)
-        xd = torch.from_numpy(xn if xn.dtype in (np.float32, np.float64) else xn.astype(np.float64)).cuda()
-    xd = xd.contiguous()
+    xd = dev.to_device(x)
+    xd = (xd if xd.dtype in (torch.float32, torch.float64) else xd.to(torch.float64)).contiguous()
     device = xd.device
     out = torch.empty((T, D * len(coefs)), dtype=xd.dtype, device=device)
     off = torch.from_numpy(np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)).to(device)
@@ -107,10 +103,10 @@ def delta_features(x, windows, lengths=None):
         _lib.check(_lib.lib.nnk_delta_features(xd.data_ptr(), dev.torch_dtype_code(xd.dtype), D, D, off.data_ptr(), None, len(lens),
                                                int(lens.max()), ctypes.byref(wc), out.data_ptr(), D * len(coefs),
                                                dev.current_stream_ptr(device)), "nnk_delta_features")
-    if is_t:
-        return out if out.dtype == x.dtype else out.to(x.dtype)
-    res = out.cpu().numpy()
-    return res if res.dtype == x.dtype else res.astype(x.dtype)
+    res = dev.like_input(out, x)
+    if res.dtype == x.dtype:
+        return res
+    return res.to(x.dtype) if dev.is_tensor(x) else res.astype(x.dtype)
 
 
 from .normalize import (inv_minmax_scale, inv_scale, meanstd, meanvar, minmax, minmax_scale,  # noqa: E402

@@ -133,18 +133,16 @@ def _gather(src, path, path_len, out_rows):
 
 
 def _to_device(A):
-    import torch
-
     from .. import _device as dev
 
     dev.require_cuda()
-    if type(A).__module__.startswith("torch"):
+    if dev.is_tensor(A):
         assert A.is_cuda, "torch inputs must be CUDA tensors"
         return A, True
     A = np.asarray(A)
     if A.dtype not in (np.float32, np.float64):
         A = A.astype(np.float64)
-    return torch.from_numpy(np.ascontiguousarray(A)).cuda(), False
+    return dev.to_device(A), False
 
 
 class DTWAligner(object):

@@ -14,8 +14,6 @@ Deliberate differences from the reference:
 """
 import numpy as np
 
-from .normalize import _check_lengths, _is_tensor
-
 KINDS = {"linear": 0, "slinear": 1, "zero": 2, "nearest": 3, "nearest-up": 4, "previous": 5, "next": 6}
 _SPLINE = ("zero", "slinear", "quadratic", "cubic")
 
@@ -40,7 +38,7 @@ def _launch(xt, B, T, lens, code):
     from .._lib import check, lib
     out = torch.empty_like(xt)
     ws = dev.workspace(xt.device, int(lib.nnk_f0_interp_workspace_bytes(B, T)))
-    lt = None if lens is None else torch.as_tensor(np.minimum(lens, T).astype(np.int32), device=xt.device)
+    lt = dev.lengths_on(lens, xt.device, T)
     check(lib.nnk_f0_interp(xt.data_ptr(), out.data_ptr(), dev.torch_dtype_code(xt.dtype), B, T,
                             lt.data_ptr() if lt is not None else None, code, ws.data_ptr(), ws.numel(),
                             dev.current_stream_ptr(xt.device)), "nnk_f0_interp")
@@ -65,9 +63,8 @@ def interp1d(f0, kind="slinear", lengths=None):
     """
     from .. import _device as dev
     code, spline = _kind_code(kind)
-    is_t = _is_tensor(f0)
     shape = tuple(int(s) for s in f0.shape)
-    dt = np.dtype(str(f0.dtype).replace("torch.", "")) if is_t else np.asarray(f0).dtype
+    dt = dev.np_dtype(f0)
     if dt not in (np.float32, np.float64):
         raise TypeError("interp1d: f0 must be float32 or float64, got %s" % dt)
     if lengths is None:
@@ -78,20 +75,15 @@ def interp1d(f0, kind="slinear", lengths=None):
         if len(shape) not in (2, 3) or (len(shape) == 3 and shape[2] != 1):
             raise ValueError("interp1d: with lengths, f0 must be (B, Tmax) or (B, Tmax, 1), got %s" % (shape,))
         B, T = shape[0], shape[1]
-        lens = _check_lengths(lengths, B)
+        lens = dev.check_lengths(lengths, B)
     dev.require_cuda()
-    import torch
-    if is_t:
-        device = f0.device if f0.is_cuda else torch.device("cuda", torch.cuda.current_device())
-        xt = f0.detach().to(device).contiguous()
-    else:
-        xt = torch.from_numpy(np.ascontiguousarray(f0)).cuda()
+    xt = dev.to_device(f0).contiguous()
     if lengths is None and spline and T == 1 and code == KINDS["slinear"] and bool((xt > 0).any()):
         raise ValueError("x and y arrays must have at least 2 entries")
     out = _launch(xt, B, T, lens, code) if B and T else xt.clone()
-    if is_t:
-        return out if f0.is_cuda else out.cpu()
-    res = out.cpu().numpy()
+    res = dev.like_input(out, f0)
+    if dev.is_tensor(f0):
+        return res
     if lengths is None and not (res.reshape(-1) > 0).any():
         return f0  # nothing to do: the reference returns its input object
     if lengths is None:

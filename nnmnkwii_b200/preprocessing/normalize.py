@@ -47,14 +47,11 @@ def _handle_zeros_in_scale(scale, copy=True):
             scale = scale.copy()
         scale[scale == 0.0] = 1.0
         return scale
-    if _is_tensor(scale):
+    from .._device import is_tensor
+    if is_tensor(scale):
         import torch
         return torch.where(scale == 0.0, torch.ones_like(scale), scale)
     return scale
-
-
-def _is_tensor(x):
-    return type(x).__module__.startswith("torch")
 
 
 def remove_zeros_frames(x, eps=1e-7):
@@ -66,24 +63,6 @@ def remove_zeros_frames(x, eps=1e-7):
 
 
 # ---- statistics ----------------------------------------------------------------------------------------
-def _check_lengths(lengths, n_items):
-    if lengths is None:
-        return None
-    if _is_tensor(lengths):
-        lengths = lengths.detach().cpu().numpy()
-    lens = np.asarray(lengths)
-    if lens.ndim != 1 or (lens.size and not np.issubdtype(lens.dtype, np.integer)):
-        raise ValueError("lengths must be a 1-D sequence of integers")
-    lens = lens.astype(np.int64)
-    if n_items is None:
-        raise ValueError("lengths needs a sized dataset (len(dataset))")
-    if len(lens) != n_items:
-        raise ValueError("lengths has %d entries for %d items" % (len(lens), n_items))
-    if lens.size and int(lens.min()) < 0:
-        raise ValueError("lengths must be >= 0")
-    return lens
-
-
 def _compute_dtype(dt):
     return np.float32 if np.dtype(dt) == np.float32 else np.float64
 
@@ -119,7 +98,9 @@ class _State:
 
 def _vec_f64(v, D, device):
     import torch
-    if _is_tensor(v):
+
+    from .._device import is_tensor
+    if is_tensor(v):
         t = v.detach().to(device=device, dtype=torch.float64)
     else:
         t = torch.as_tensor(np.asarray(v, dtype=np.float64), device=device)
@@ -141,6 +122,8 @@ def _pinned_buffer(nbytes):
 def _stats_tensor(x, lens, mean_, var_, count):
     """Form (c): a 3-D CUDA tensor, read in place with one launch."""
     import torch
+
+    from .. import _device as dev
     B, T, D = (int(s) for s in x.shape)
     if x.dtype not in (torch.float32, torch.float64):
         x = x.to(torch.float64)
@@ -152,17 +135,16 @@ def _stats_tensor(x, lens, mean_, var_, count):
     st = _State(D, x.device, mean_, var_, count)
     if frames:
         off = torch.arange(B + 1, dtype=torch.int64, device=x.device) * T  # padded batch: utterance b at row b * T
-        l = None
-        if lens is not None:
-            l = torch.as_tensor(np.minimum(lens, T).astype(np.int32), device=x.device)
-        st.fold(x, ld, off, l, B, T)
+        st.fold(x, ld, off, dev.lengths_on(lens, x.device, T), B, T)
     return st, frames
 
 
 def _stats_host(dataset, lens, mean_, var_, count):
     """Forms (a) and (b): pack utterances into page-locked staging, one launch per full buffer."""
     import torch
-    device = torch.device("cuda", torch.cuda.current_device())
+
+    from .. import _device as dev
+    device = dev.cuda_device()
     stream = torch.cuda.current_stream(device)
     st = None
     dtype = None
@@ -189,7 +171,7 @@ def _stats_host(dataset, lens, mean_, var_, count):
             events[slot].synchronize()  # the other half's copy has finished: it can be refilled
 
     for idx, x in enumerate(dataset):
-        if _is_tensor(x):
+        if dev.is_tensor(x):
             x = x.detach().cpu().numpy()
         x = np.asarray(x)
         if x.ndim != 2:
@@ -230,7 +212,7 @@ def _run_stats(dataset, lengths, mean_=0.0, var_=0.0, count=0, allow_empty=False
     """-> (state, frames, result dtype or None for CUDA results).  Argument errors come before any launch."""
     from .. import _device as dev
     T = None
-    if isinstance(dataset, np.ndarray) or _is_tensor(dataset):
+    if isinstance(dataset, np.ndarray) or dev.is_tensor(dataset):
         if len(dataset.shape) != 3:
             raise ValueError("an array dataset must be (B, T, D), got %d-D" % len(dataset.shape))
         T = int(dataset.shape[1])
@@ -241,13 +223,13 @@ def _run_stats(dataset, lengths, mean_=0.0, var_=0.0, count=0, allow_empty=False
         n_items = len(dataset)
     except TypeError:
         pass
-    lens = _check_lengths(lengths, n_items)
+    lens = dev.check_lengths(lengths, n_items)
     if n_items == 0:
         raise ValueError("dataset is empty")
     if not allow_empty and (T == 0 or (lens is not None and int(lens.sum()) == 0)):
         raise ValueError("no frames: every length is 0")
     dev.require_cuda()
-    if _is_tensor(dataset) and dataset.is_cuda:
+    if dev.is_tensor(dataset) and dataset.is_cuda:
         st, frames = _stats_tensor(dataset, lens, mean_, var_, count)
         return st, frames, None
     return _stats_host(dataset, lens, mean_, var_, count)
@@ -292,8 +274,9 @@ def meanvar(dataset, lengths=None, mean_=0.0, var_=0.0, last_sample_count=0, ret
 
 def meanstd(dataset, lengths=None, mean_=0.0, var_=0.0, last_sample_count=0, return_last_sample_count=False):
     """Mean and standard deviation (zero -> 1) of every column (preprocessing/generic.py:552-602)."""
+    from .._device import is_tensor
     m, v, n = _meanvar(dataset, lengths, mean_, var_, last_sample_count)
-    if _is_tensor(v):
+    if is_tensor(v):
         import torch
         s = _handle_zeros_in_scale(torch.sqrt(v))
     else:
@@ -314,15 +297,6 @@ def minmax(dataset, lengths=None):
 
 
 # ---- per-column affine maps ----------------------------------------------------------------------------
-def _param_dtype(p):
-    if np.isscalar(p) and not isinstance(p, np.generic):
-        return p  # a Python scalar: weak, as in NumPy's own promotion
-    if _is_tensor(p):
-        import torch
-        return np.dtype(str(p.dtype).replace("torch.", ""))
-    return np.asarray(p).dtype
-
-
 def _affine(x, a, b, form):
     """form 0: (x - a) / b, form 1: x * b + a, per column of the last axis, on the GPU."""
     import torch
@@ -330,27 +304,22 @@ def _affine(x, a, b, form):
     from .. import _device as dev
     from .._lib import check, lib
     dev.require_cuda()
-    is_t = _is_tensor(x)
-    xdt = np.dtype(str(x.dtype).replace("torch.", "")) if is_t else np.asarray(x).dtype
     if len(x.shape) == 0:
         raise ValueError("x must have at least one dimension")
     D = int(x.shape[-1])
-    cdt = np.result_type(xdt, _param_dtype(a), _param_dtype(b))
+    params = [p if np.isscalar(p) and not isinstance(p, np.generic) else dev.np_dtype(p) for p in (a, b)]
+    cdt = np.result_type(dev.np_dtype(x), *params)  # a Python scalar parameter stays weak, as in NumPy's promotion
     if cdt not in (np.float32, np.float64):
         raise TypeError("scaling computes in float32 or float64, numpy.result_type gives %s" % cdt)
     tcdt = torch.float32 if cdt == np.float32 else torch.float64
-    if is_t:
-        device = x.device if x.is_cuda else torch.device("cuda", torch.cuda.current_device())
-        xt = x.detach().to(device)
-    else:
-        device = torch.device("cuda", torch.cuda.current_device())
-        xt = torch.from_numpy(np.ascontiguousarray(x)).to(device)
+    xt = dev.to_device(x)
+    device = xt.device
     if xt.dtype not in (torch.float32, torch.float64) or (xt.dtype == torch.float64 and tcdt == torch.float32):
         xt = xt.to(tcdt)
     xt = xt.contiguous()
 
     def vec(p):
-        if _is_tensor(p):
+        if dev.is_tensor(p):
             t = p.detach().to(device=device, dtype=tcdt)
         else:
             t = torch.as_tensor(np.asarray(p, dtype=cdt), device=device)
@@ -364,9 +333,7 @@ def _affine(x, a, b, form):
         check(lib.nnk_column_affine(xt.data_ptr(), dev.torch_dtype_code(xt.dtype), dev.torch_dtype_code(tcdt), rows, D,
                                     av.data_ptr(), bv.data_ptr(), form, out.data_ptr(), dev.current_stream_ptr(device)),
               "nnk_column_affine")
-    if is_t:
-        return out if x.is_cuda else out.cpu()
-    return out.cpu().numpy()
+    return dev.like_input(out, x)
 
 
 def scale(x, data_mean, data_std):

@@ -18,28 +18,14 @@ import numbers
 
 import numpy as np
 
-from .normalize import _check_lengths, _is_tensor
-
 _last_counters = None
-
-
-def _np_dtype(x):
-    return np.dtype(str(x.dtype).replace("torch.", "")) if _is_tensor(x) else np.asarray(x).dtype
-
-
-def _to_device(x):
-    import torch
-    if _is_tensor(x):
-        device = x.device if x.is_cuda else torch.device("cuda", torch.cuda.current_device())
-        return x.detach().to(device).contiguous()
-    return torch.from_numpy(np.ascontiguousarray(x)).cuda()
 
 
 def _filter(x, coef, lengths, inverse):
     global _last_counters
     from .. import _device as dev
     from .._lib import check, lib
-    dt = _np_dtype(x)
+    dt = dev.np_dtype(x)
     if dt not in (np.float32, np.float64):
         # what scipy.signal.lfilter raises for the reference's coefficient arrays of this dtype
         if inverse:
@@ -52,16 +38,16 @@ def _filter(x, coef, lengths, inverse):
     if lengths is not None:
         if len(shape) != 2:
             raise ValueError("lengths requires a 2-D (B, T) x, got %d-D" % len(shape))
-        lens = _check_lengths(lengths, shape[0])
+        lens = dev.check_lengths(lengths, shape[0])
     coef = float(coef)
     dev.require_cuda()
     import torch
-    xt = _to_device(x)
+    xt = dev.to_device(x).contiguous()
     T = shape[-1]
     rows = xt.numel() // T if T else 0
     out = torch.empty_like(xt)
     if rows and T:
-        lt = None if lens is None else torch.as_tensor(np.minimum(lens, T).astype(np.int32), device=xt.device)
+        lt = dev.lengths_on(lens, xt.device, T)
         code = dev.torch_dtype_code(xt.dtype)
         ws = dev.workspace(xt.device, int(lib.nnk_preemphasis_workspace_bytes(code, rows, T, coef, int(inverse))))
         counters = torch.empty(2, dtype=torch.int64, device=xt.device)
@@ -71,9 +57,7 @@ def _filter(x, coef, lengths, inverse):
               "nnk_preemphasis")
         if inverse:
             _last_counters = counters
-    if _is_tensor(x):
-        return out if x.is_cuda else out.cpu()
-    return out.cpu().numpy()
+    return dev.like_input(out, x)
 
 
 def _repair_counters():
@@ -113,13 +97,13 @@ def _mulaw_call(x, mu, mode):
     from .. import _device as dev
     from .._lib import NNK_F32, NNK_F64, check, lib
     mu = float(mu) if not isinstance(mu, numbers.Integral) else int(mu)
-    is_t = _is_tensor(x)
+    is_t = dev.is_tensor(x)
     scalar = not is_t and np.isscalar(x)
     if not is_t and not scalar and not isinstance(x, np.ndarray):
         raise TypeError("expected a NumPy array, a scalar or a torch tensor, got %s" % type(x).__name__)
     if scalar and not isinstance(x, (numbers.Number, np.generic)):
         raise TypeError("expected a numeric scalar, got %s" % type(x).__name__)
-    dt = _np_dtype(x) if not scalar else None
+    dt = dev.np_dtype(x) if not scalar else None
     if mode == 3:
         if is_t:
             if x.dtype == torch.bool or x.is_complex():
@@ -154,15 +138,13 @@ def _mulaw_call(x, mu, mode):
         else:
             out_np = np.float64 if variant in (0, 2) else np.float32
     dev.require_cuda()
-    xt = _to_device(src)
+    xt = dev.to_device(src).contiguous()
     code = {torch.float32: NNK_F32, torch.float64: NNK_F64, torch.int32: 2, torch.int64: 3}[xt.dtype]
     out = torch.empty(xt.shape, dtype=getattr(torch, np.dtype(out_np).name), device=xt.device)
     if xt.numel():
         check(lib.nnk_mulaw(xt.data_ptr(), code, out.data_ptr(), mode, variant, xt.numel(), float(mu),
                             dev.current_stream_ptr(xt.device)), "nnk_mulaw")
-    if is_t:
-        return out if x.is_cuda else out.cpu()
-    res = out.cpu().numpy()
+    res = dev.like_input(out, x)
     if scalar:
         v = res[0]
         return int(v) if mode == 2 else v

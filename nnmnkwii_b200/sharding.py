@@ -427,7 +427,9 @@ def mlpg_batch_sharded(means, variances, windows, lengths, layout=None, group=No
         layout = G.StreamLayout.single(means.shape[1], len(windows))
     plan = ShardPlan(lengths, world, n_buckets)
     if device is None:
-        device = _default_device()
+        from . import _device as dev
+        dev.require_cuda()
+        device = dev.cuda_device()
     dtype = torch.float32 if means.dtype == np.float32 and np.asarray(variances).dtype == np.float32 else torch.float64
     np_dt = np.float32 if dtype == torch.float32 else np.float64
     if transport is None:
@@ -448,13 +450,6 @@ def mlpg_batch_sharded(means, variances, windows, lengths, layout=None, group=No
         batch.result = None
         return out
     return res.to_utterance_order() if utterance_order else res
-
-
-def _default_device():
-    import torch
-    from . import _device as dev
-    dev.require_cuda()
-    return torch.device("cuda", torch.cuda.current_device())
 
 
 _ = ctypes

@@ -24,6 +24,38 @@ def test_library_exports_every_declared_symbol():
     assert _lib.lib.nnk_abi_version() == int(re.search(r"#define NNK_ABI_VERSION (\d+)", _header()).group(1))
 
 
+def _c_kind(c_type):
+    """'ptr', 'i4', 'i8', 'f8' or None (void) of a C type."""
+    if "*" in c_type:
+        return "ptr"
+    return {"void": None, "int": "i4", "int32_t": "i4", "int64_t": "i8", "uint64_t": "i8", "size_t": "i8",
+            "double": "f8"}[c_type.strip()]
+
+
+def _ctypes_kind(t):
+    if t is None:
+        return None
+    if issubclass(t, (ctypes._Pointer, ctypes.c_void_p, ctypes.c_char_p)):
+        return "ptr"
+    if t is ctypes.c_double:
+        return "f8"
+    return "i%d" % ctypes.sizeof(t)
+
+
+def test_signature_table_matches_header_prototypes():
+    """Every binding has the header's arity and, per argument and result, the same kind: an int32_t bound
+    as an int64_t (or back) would silently truncate or misread the argument."""
+    from nnmnkwii_b200 import _lib
+    h = re.sub(r"/\*.*?\*/|//[^\n]*", "", _header(), flags=re.S)
+    protos = re.findall(r"([A-Za-z_][\w ]*\**)\s*\b(nnk_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", h)
+    assert sorted(name for _, name, _ in protos) == sorted(_lib.SIGNATURES)
+    for ret, name, params in protos:
+        restype, argtypes = _lib.SIGNATURES[name]
+        params = [] if params.strip() in ("", "void") else params.split(",")
+        assert _ctypes_kind(restype) == _c_kind(ret), name
+        assert [_ctypes_kind(t) for t in argtypes] == [_c_kind(p.rsplit(None, 1)[0]) for p in params], name
+
+
 def test_struct_layouts_match_header():
     from nnmnkwii_b200 import _lib
     h = _header()

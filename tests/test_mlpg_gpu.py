@@ -400,3 +400,35 @@ def test_deferred_check_surfaces_not_positive_definite():
     with pytest.raises(np.linalg.LinAlgError):
         dev.poll_errors(block=True)
     dev.poll_errors(block=True)  # the record is consumed
+
+
+def test_batch_tables_are_checked_before_any_launch_on_every_path():
+    """Padded lengths of the wrong size or above Tmax, and flat lengths that do not cover the rows, raise
+    AssertionError for CUDA inputs of mlpg_batch / mlpg_grad_batch exactly as for NumPy mlpg_batch."""
+    import torch
+
+    from nnmnkwii_b200 import _lib
+    from nnmnkwii_b200 import paramgen as G
+    ws = windows_set()[2]
+    rng = np.random.default_rng(11)
+    m = rng.standard_normal((3, 20, 3 * 4)).astype(np.float32)
+    v = np.ones_like(m)
+    go = torch.ones((3, 20, 4), device="cuda")
+    bad_padded = ([20, 20], [20, 20, 20, 20], [5, 21, 5])
+    bad_flat = ([20, 20, 19], [20, 20, 20, 1])
+    n0 = _lib.launch_count()
+    for lens in bad_padded:
+        for call in (lambda: G.mlpg_batch(m, v, ws, lengths=lens),
+                     lambda: G.mlpg_batch(torch.from_numpy(m).cuda(), torch.from_numpy(v).cuda(), ws, lengths=lens),
+                     lambda: G.mlpg_grad_batch(torch.from_numpy(v).cuda(), ws, go, lens)):
+            with pytest.raises(AssertionError):
+                call()
+    for lens in bad_flat:
+        for call in (lambda: G.mlpg_batch(m.reshape(60, -1), v.reshape(60, -1), ws, lengths=lens),
+                     lambda: G.mlpg_batch(torch.from_numpy(m).cuda().reshape(60, -1),
+                                          torch.from_numpy(v).cuda().reshape(60, -1), ws, lengths=lens),
+                     lambda: G.mlpg_grad_batch(torch.from_numpy(v).cuda().reshape(60, -1), ws, go.reshape(60, -1),
+                                               lens)):
+            with pytest.raises(AssertionError):
+                call()
+    assert _lib.launch_count() == n0

@@ -12,7 +12,7 @@ are checked against `variant_mirror` in a child process (`variant_mirror.profile
 The module is named to sort after every module that asserts kernel names from the pytest process: with these
 cases run before them, torch.profiler came back empty for the UnitVarianceMLPG variant cases in a full GPU run on
 an H100 (they pass alone and after these modules alone), so their names are collected in child processes and
-their numbers come last."""
+their numbers come last.  The `delta_features` CPU-tensor case is here for the same reason."""
 import ctypes
 
 import numpy as np
@@ -378,3 +378,18 @@ def test_kernel_names_follow_the_mirror():
                                                                             cases)):
         assert err == "None", (case, err)
         assert names and all(w in n for n in names), (case, w, names)
+
+
+def test_delta_features_cpu_tensor_is_computed_on_the_gpu():
+    """A CPU tensor goes to the GPU and comes back as a CPU tensor of its dtype, equal to the NumPy result."""
+    import torch
+
+    from nnmnkwii_b200.preprocessing import delta_features
+    rng = np.random.default_rng(5)
+    ws = [(0, 0, np.array([1.0])), (1, 1, np.array([-0.5, 0.0, 0.5])), (1, 1, np.array([1.0, -2.0, 1.0]))]
+    for dt in (np.float32, np.float64):
+        x = rng.standard_normal((120, 7)).astype(dt)
+        ref = delta_features(x, ws, lengths=[50, 70])
+        y = delta_features(torch.from_numpy(x), ws, lengths=[50, 70])
+        assert y.device.type == "cpu" and y.dtype == torch.from_numpy(x).dtype
+        assert np.array_equal(y.numpy(), ref)
