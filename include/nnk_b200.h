@@ -214,6 +214,24 @@ int nnk_gather_rows(const void* X, int32_t dtype, int64_t x_pair_stride, int32_t
 int nnk_trim_lengths(const void* X, int32_t dtype, int64_t pair_stride, int32_t ld, int32_t T, int32_t D, double eps,
                      int32_t n_pairs, int32_t* len, void* stream);
 
+/* ---- inverse from a Cholesky factor (util/linalg.py:7-36, util/_linalg.pyx:45-71), float64 ----------
+ * B row-major (N, N) matrices back to back in, B full (N, N) results out; P must not alias the input
+ * (it is the substitutions' scratch).  No workspace.
+ *   nnk_cholesky_inv:        P = (L L^T)^-1 (lower != 0, lower triangle of each input read) or
+ *                            (U^T U)^-1 (lower == 0, upper triangle read) -- dpotri + mirror.  P is
+ *                            exactly symmetric: one triangle is computed and mirrored.
+ *   nnk_cholesky_inv_banded: P = (R R^T)^-1, only the band R[t, t-j], 0 <= j < width, read.  Bit-identical
+ *                            to the reference's row recurrence on finite input (signs of zeros aside).
+ * A zero or non-finite diagonal entry sets *status_word (device, zero-initialised by the caller;
+ * nnk_status_decode: utt = batch item, frame = row + 1, first item / row wins); the results of that
+ * item are then undefined, and no input faults.
+ * NNK_REQUIRE: N, T, B >= 0; width >= 1; non-NULL pointers when there is work; P != input.
+ * NNK_ERR_UNSUPPORTED: min(width, T) > 9 (l + u + 1 of every window set the MLPG kernels accept).      */
+int nnk_cholesky_inv(const double* L, int32_t lower, int32_t N, int32_t B, double* P, uint64_t* status_word,
+                     void* stream);
+int nnk_cholesky_inv_banded(const double* R, int32_t width, int32_t T, int32_t B, double* P, uint64_t* status_word,
+                            void* stream);
+
 /* ---- delta features (SURVEY section 8f row 2; preprocessing/generic.py:229-288) ------------------
  * out[:, w*D + d] = np.correlate(x[:, d], coef_w, mode="same") per utterance of a flat (sum_T, D)
  * batch: window centred at len(coef_w) // 2, zeros outside the utterance, float64 arithmetic,

@@ -177,6 +177,8 @@ SIGNATURES = {
     "nnk_dtw_workspace_bytes": (size_t, [i32, i32, i32, i32, i32]),
     "nnk_gather_rows": (ctypes.c_int, [vp, i32, i64, i32, vp, i32, vp, vp, i64, i32, i32, i32, vp]),
     "nnk_trim_lengths": (ctypes.c_int, [vp, i32, i64, i32, i32, i32, f64, i32, vp, vp]),
+    "nnk_cholesky_inv": (ctypes.c_int, [vp, i32, i32, i32, vp, vp, vp]),
+    "nnk_cholesky_inv_banded": (ctypes.c_int, [vp, i32, i32, i32, vp, vp, vp]),
     "nnk_delta_features": (ctypes.c_int, [vp, i32, i32, i64, vp, vp, i32, i32, P(NnkWindows), vp, i64, vp]),
     "nnk_metric_workspace_bytes": (i64, [i32, i32]),
     "nnk_frame_metric": (ctypes.c_int, [vp, vp, i32, i32, i32, i32, i64, i64, vp, i32, vp, vp, vp, i64, vp]),
