@@ -127,6 +127,34 @@ int nnk_mlpg_solve(const nnk_mlpg_args_t* args, void* stream);
 /* Scratch needed by the calls above for `n_utt` utterances of at most max_T frames.         */
 size_t nnk_mlpg_workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T, const nnk_windows_t* win);
 
+/* Parameter generation considering global variance (Toda, Black & Tokuda 2007, Sec. IV; diagonal GV
+ * covariance).  Per chain c (mu = gv_mean[c.out_col], p = 1 / gv_var[c.out_col], T frames) and with
+ * c_m = P^-1 b the nnk_mlpg_fwd trajectory, maximises
+ *   F(c) = omega (b^T c - c^T P c / 2) - p (v(c) - mu)^2 / 2,  v(c) = population variance of c over T
+ * starting from c0 = mean(c_m) + sqrt(mu / v(c_m)) (c_m - mean(c_m)) (c0 = c_m when v(c_m) == 0), with
+ * n_iter trials of c' = c + alpha ((c_m - c) + P^-1 g / omega), g = dv/dc * (-p (v - mu)): c' is kept
+ * when F(c') >= F(c), otherwise alpha halves (alpha starts at `step`; a rejected trial still counts).
+ * omega = weight, or 1 / (nw T) when weight == 0.  float64 arithmetic, output in args->dtype; pass-through
+ * chains are copied.  Same arguments, status word and failure rule as nnk_mlpg_fwd; the workspace must hold
+ * nnk_mlpg_gv_workspace_bytes() (the factors plus four columns per frame: d, c_m, c, trial c).        */
+typedef struct nnk_mlpg_gv {
+  const double* gv_mean;      /* device, indexed by chain out_col: target GV, >= 0                   */
+  const double* gv_var;       /* device, indexed by chain out_col: variance of the GV, > 0             */
+  int32_t n_iter;             /* >= 0 trials                                                           */
+  double step;                /* > 0 initial step alpha                                                */
+  double weight;              /* omega > 0, or 0 => 1 / (nw T) per utterance                           */
+} nnk_mlpg_gv_t;
+int nnk_mlpg_gv(const nnk_mlpg_args_t* args, const nnk_mlpg_gv_t* gv, void* stream);
+size_t nnk_mlpg_gv_workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T, const nnk_windows_t* win);
+
+/* Per-segment moments of the columns of a row-major float32 / float64 matrix (row stride ld elements):
+ * segment u is rows utt_off[u] .. utt_off[u] + len - 1, len = utt_len[u] (device int32, or NULL =>
+ * utt_off[u+1] - utt_off[u]), every len >= 1.  mean (n_utt, D) (may be NULL) and var (n_utt, D) float64,
+ * var = population variance, two passes (mean, then squared deviations), float64 accumulation in a fixed
+ * order.  Serves paramgen.global_variance / gv_statistics.                                          */
+int nnk_segment_moments(const void* X, int32_t dtype, int32_t D, int64_t ld, const int64_t* utt_off,
+                        const int32_t* utt_len, int32_t n_utt, double* mean, double* var, void* stream);
+
 /* Host-buffer convenience = what a cgo/ctypes binding of paramgen.mlpg would call: one utterance,
  * one stream, host pointers (means (T, D), variances (T, D) or (D,), out (T, D / nw)), copies
  * included, synchronous.  Returns NNK_ERR_NOT_PD with *bad_frame = 1-based frame on failure.    */

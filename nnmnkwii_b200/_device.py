@@ -183,9 +183,12 @@ def _defer_check(status, device):
 
 
 def run_mlpg(mode, *, means, variances, rhs, out, offsets, lengths, order, chains, n_chain, max_T, windows_c,
-             in_ld, var_ld, go_ld, out_ld, dtype_code, go_f64, n_utt, device, check=True, out_offsets=None, status=None):
-    """Fill nnk_mlpg_args_t and enqueue nnk_mlpg_{fwd,grad,solve} on torch's current stream of
-    ``device`` (the C ABI switches to the device that owns ``out`` for the launch).
+             in_ld, var_ld, go_ld, out_ld, dtype_code, go_f64, n_utt, device, check=True, out_offsets=None, status=None,
+             gv=None):
+    """Fill nnk_mlpg_args_t and enqueue nnk_mlpg_{fwd,grad,solve,gv} on torch's current stream of
+    ``device`` (the C ABI switches to the device that owns ``out`` for the launch).  Mode "gv" takes
+    ``gv = (gv_mean, gv_var, n_iter, step, weight)`` with float64 device tensors indexed by output column
+    and ``weight`` 0 for 1 / (nw T).
     ``check``: True = synchronising status check, "deferred" = non-blocking (see poll_errors), False = none."""
     poll_errors()
     a = NnkMlpgArgs()
@@ -205,7 +208,8 @@ def run_mlpg(mode, *, means, variances, rhs, out, offsets, lengths, order, chain
     a.max_T = max_T
     a.go_f64 = go_f64
     a.win = windows_c
-    need = lib.nnk_mlpg_workspace_bytes(n_utt, n_chain, max_T, ctypes.byref(windows_c))
+    sizing = lib.nnk_mlpg_gv_workspace_bytes if mode == "gv" else lib.nnk_mlpg_workspace_bytes
+    need = sizing(n_utt, n_chain, max_T, ctypes.byref(windows_c))
     if need == 0 and n_utt and n_chain and max_T:
         raise NotImplementedError("window set not supported by the CUDA kernels")
     per_utt = need // max(1, n_utt)
@@ -216,8 +220,15 @@ def run_mlpg(mode, *, means, variances, rhs, out, offsets, lengths, order, chain
     if status is None:  # a caller-owned word accumulates the first failure over several launches
         status = torch.zeros(1, dtype=torch.int64, device=device)
     a.status_word = status.data_ptr()
-    fn = {"fwd": lib.nnk_mlpg_fwd, "grad": lib.nnk_mlpg_grad, "solve": lib.nnk_mlpg_solve}[mode]
-    _lib.check(fn(ctypes.byref(a), current_stream_ptr(device)), "nnk_mlpg_" + mode)
+    if mode == "gv":
+        g = _lib.NnkMlpgGv()
+        g.gv_mean, g.gv_var = gv[0].data_ptr(), gv[1].data_ptr()
+        g.n_iter, g.step, g.weight = int(gv[2]), float(gv[3]), float(gv[4])
+        rc = lib.nnk_mlpg_gv(ctypes.byref(a), ctypes.byref(g), current_stream_ptr(device))
+    else:
+        fn = {"fwd": lib.nnk_mlpg_fwd, "grad": lib.nnk_mlpg_grad, "solve": lib.nnk_mlpg_solve}[mode]
+        rc = fn(ctypes.byref(a), current_stream_ptr(device))
+    _lib.check(rc, "nnk_mlpg_" + mode)
     if check == "deferred":
         _defer_check(status, device)
     elif check:

@@ -59,6 +59,16 @@ class NnkMlpgArgs(ctypes.Structure):
     ]
 
 
+class NnkMlpgGv(ctypes.Structure):
+    _fields_ = [
+        ("gv_mean", ctypes.c_void_p),
+        ("gv_var", ctypes.c_void_p),
+        ("n_iter", ctypes.c_int32),
+        ("step", ctypes.c_double),
+        ("weight", ctypes.c_double),
+    ]
+
+
 class NnkGmm(ctypes.Structure):
     _fields_ = [
         ("src_means", ctypes.c_void_p), ("tgt_means", ctypes.c_void_p), ("prec_chol", ctypes.c_void_p),
@@ -165,6 +175,9 @@ SIGNATURES = {
     "nnk_mlpg_grad": (ctypes.c_int, _MLPG),
     "nnk_mlpg_solve": (ctypes.c_int, _MLPG),
     "nnk_mlpg_workspace_bytes": (size_t, [i32, i32, i32, P(NnkWindows)]),
+    "nnk_mlpg_gv": (ctypes.c_int, [P(NnkMlpgArgs), P(NnkMlpgGv), vp]),
+    "nnk_mlpg_gv_workspace_bytes": (size_t, [i32, i32, i32, P(NnkWindows)]),
+    "nnk_segment_moments": (ctypes.c_int, [vp, i32, i32, i64, vp, vp, i32, vp, vp, vp]),
     "nnk_mlpg_host": (ctypes.c_int, [vp, vp, i32, i32, i64, i64, P(NnkWindows), vp, P(i32)]),
     "nnk_mlpg_batch_host": (ctypes.c_int, [vp, vp, i32, i32, i64, i64, i64, vp, i32, vp, i32, P(NnkWindows), vp,
                                            P(NnkStatus)]),

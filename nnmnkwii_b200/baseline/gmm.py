@@ -21,7 +21,7 @@ import numpy as np
 from scipy import linalg
 from sklearn.mixture import GaussianMixture as _SkGaussianMixture
 
-from ..paramgen import mlpg_batch
+from ..paramgen import mlpg_batch, mlpg_gv_batch
 
 
 def _compute_precision_cholesky_full(covariances):
@@ -159,14 +159,33 @@ class MLPG(MLPGBase):
         windows (list): window triples, see :func:`nnmnkwii_b200.paramgen.mlpg`.
         swap (bool): if True source -> target, otherwise target -> source.
         diff (bool): convert GMM -> DIFFGMM if True.
+        gv (tuple): additive: ``(gv_mean, gv_var)`` of the target's static features, each of length
+            ``static_dim`` (e.g. :func:`nnmnkwii_b200.paramgen.gv_statistics` of the training targets).
+            When given, :meth:`transform` and :meth:`transform_batch` generate with
+            :func:`nnmnkwii_b200.paramgen.mlpg_gv_batch` (Toda, Black & Tokuda 2007, Sec. IV) instead of
+            plain MLPG.  Not defined for ``diff=True`` (``ValueError``), and not applied on the
+            posterior-mean path (source features of ``static_dim`` columns), which runs no MLPG.
     """
 
-    def __init__(self, gmm, windows=None, swap=False, diff=False):
+    def __init__(self, gmm, windows=None, swap=False, diff=False, gv=None):
         super(MLPG, self).__init__(gmm, swap, diff)
         if windows is None:
             windows = [(0, 0, np.array([1.0])), (1, 1, np.array([-0.5, 0.0, 0.5]))]
         self.windows = windows
         self.static_dim = gmm.means_.shape[-1] // 2 // len(windows)
+        self.gv = None
+        if gv is not None:
+            if diff:
+                raise ValueError("gv is not defined for difference features (diff=True)")
+            gv_mean, gv_var = (np.asarray(a, dtype=np.float64).ravel() for a in gv)
+            from ..paramgen import StreamLayout, _gv_args
+            _gv_args(gv_mean, gv_var, StreamLayout.single(self.static_dim * len(windows), len(windows)), 0, 1.0, None)
+            self.gv = (gv_mean, gv_var)
+
+    def _generate(self, E, Dv, lengths):
+        if self.gv is None:
+            return mlpg_batch(E, Dv, self.windows, lengths=lengths)
+        return mlpg_gv_batch(E, Dv, self.windows, self.gv[0], self.gv[1], lengths=lengths)
 
     def _means_vars(self, x, c):
         """E (Eq. 22) and D (Eq. 23) of the sub-optimum mixture sequence (Eq. 37), on the device."""
@@ -180,7 +199,7 @@ class MLPG(MLPGBase):
             return super(MLPG, self).transform(src)
         x, c = self._to_device(src)
         E, Dv = self._means_vars(x, c)
-        return mlpg_batch(E, Dv, self.windows, lengths=[T]).cpu().numpy()
+        return self._generate(E, Dv, [T]).cpu().numpy()
 
     def transform_batch(self, srcs):
         """Additive: convert a list of utterances in one pass (one posterior / mapping evaluation and
@@ -195,7 +214,7 @@ class MLPG(MLPGBase):
         else:
             x, c = self._to_device(flat)
             E, Dv = self._means_vars(x, c)
-            y = mlpg_batch(E, Dv, self.windows, lengths=lens).cpu().numpy()
+            y = self._generate(E, Dv, lens).cpu().numpy()
         del torch
         off = np.concatenate([[0], np.cumsum(lens)])
         return [y[off[i]:off[i + 1]] for i in range(len(lens))]

@@ -23,6 +23,8 @@
 // warp-specialised, TMA-staged mlpg_fwd_as_kernel of nnk_mlpg_as.cuh.  launch_mlpg takes the staged kernel
 // for forward solves and float32-grad_output gradients whose window set fills its template instance
 // (nw == NW), with NT <= 5 and rows narrow enough for as_geometry; everything else runs mlpg_kernel.
+#include <type_traits>
+
 #include "nnk_mlpg.cuh"
 #include "nnk_mlpg_as.cuh"
 
@@ -39,10 +41,115 @@ __device__ __forceinline__ double load_go(const void* go, int is_f64, int64_t id
                 : (double)ld_stream(reinterpret_cast<const float*>(go) + idx);
 }
 
+// ---- global-variance refinement (MODE_GV, nnk_mlpg_gv) --------------------------------------------------
+// One chain (one lane).  The sweeps below have left per frame t, in the lane's scratch column col (stride 32):
+//   0: zs_t = (L^-1 b)_t / d_t,   1..S: l_j[t] = L[t+j][t],   NT: d_t,   NT+1: c_m,t = (P^-1 b)_t
+// of P = L D L^T.  gv_refine maximises
+//   F(c) = omega (b^T c - c^T P c / 2) - prec (v(c) - mu)^2 / 2,   v(c) = (1/T) sum_t (c_t - mean(c))^2
+// (Toda, Black & Tokuda 2007, Eq. 44 with a diagonal GV covariance) from c0 = mean + sqrt(mu / v(c_m)) (c_m - mean)
+// by n_iter trials of the P-preconditioned step  delta = (c_m - c) + P^-1 g / omega,  g_t = -(2/T) prec (v - mu)
+// (c_t - mean):  c + alpha delta replaces c when F does not decrease, otherwise alpha halves.  F comes from the
+// factors: with e = L^T c,  b^T c = sum_t d_t zs_t e_t  and  c^T P c = sum_t d_t e_t^2.  The current and the trial
+// trajectory live in columns NT+2 / NT+3 and swap roles on acceptance.  Every sum runs over t in a fixed order, so
+// results do not depend on the batch around the chain.
+template <int S, int NTS, typename Tout>
+__device__ __forceinline__ void gv_refine(double* ws, int T, double sum_cm, double mu, double prec, double omega,
+                                          int n_iter, double step, Tout* out, int64_t out_ld) {
+  constexpr int NT = S + 1, C_D = NT, C_CM = NT + 1, SP = S > 0 ? S : 1;
+  auto at = [&](int t, int col) -> double& { return ws[(size_t)t * (NTS * 32) + col * 32]; };
+  const double invT = 1.0 / (double)T;
+  auto variance = [&](int col, double mean) {
+    double v = 0.0;
+    for (int t = 0; t < T; ++t) {
+      const double dv = at(t, col) - mean;
+      v = fma(dv, dv, v);
+    }
+    return v * invT;
+  };
+  // x_t goes to column dst; returns sum_t d_t e_t (zs_t - e_t / 2) with e = L^T x, and sum_t x_t in sx.  With
+  // SOLVE, dst holds (L^-1 g)_t / d_t on entry and x_t = c_t + alpha ((c_m,t - c_t) + z_t / omega), z = P^-1 g;
+  // otherwise x_t = c0_t = mean + scale (c_m,t - mean).
+  auto back_pass = [&](auto solve_tag, int src, int dst, double a, double b, double& sx) {
+    constexpr bool SOLVE = decltype(solve_tag)::value;
+    double xw[S + 1], zw[S + 1];
+#pragma unroll
+    for (int j = 0; j <= S; ++j) { xw[j] = 0.0; zw[j] = 0.0; }
+    double q = 0.0;
+    sx = 0.0;
+    for (int t = T - 1; t >= 0; --t) {
+      double l[S + 1];
+#pragma unroll
+      for (int j = 1; j <= S; ++j) l[j] = at(t, j);
+#pragma unroll
+      for (int j = S; j > 0; --j) { xw[j] = xw[j - 1]; zw[j] = zw[j - 1]; }
+      const double cm = at(t, C_CM);
+      double x;
+      if constexpr (SOLVE) {
+        double z = at(t, dst);
+#pragma unroll
+        for (int j = 1; j <= S; ++j) z = fma(-l[j], zw[j], z);
+        zw[0] = z;
+        const double c = at(t, src);
+        x = c + a * ((cm - c) + z / b);
+      } else {
+        x = a + b * (cm - a);
+      }
+      xw[0] = x;
+      at(t, dst) = x;
+      double e = x;
+#pragma unroll
+      for (int j = 1; j <= S; ++j) e = fma(l[j], xw[j], e);
+      q = fma(at(t, C_D) * e, at(t, 0) - 0.5 * e, q);
+      sx += x;
+    }
+    return q;
+  };
+
+  // start point
+  const double mean_m = sum_cm * invT;
+  const double vm = variance(C_CM, mean_m);
+  int cur = NT + 2, nxt = NT + 3;
+  double sx;
+  double q = back_pass(std::false_type{}, C_CM, cur, mean_m, vm > 0.0 ? sqrt(mu / vm) : 1.0, sx);
+  double mean = sx * invT, v = variance(cur, mean);
+  double f = omega * q - 0.5 * prec * (v - mu) * (v - mu);
+
+  double alpha = step;
+  for (int it = 0; it < n_iter; ++it) {
+    // forward substitution of g: column nxt = (L^-1 g) / d
+    const double gs = -2.0 * invT * prec * (v - mu);
+    double pend[SP];  // pend[k]: sum of the eliminated terms of frame t + k
+#pragma unroll
+    for (int k = 0; k < SP; ++k) pend[k] = 0.0;
+    for (int t = 0; t < T; ++t) {
+      const double w = gs * (at(t, cur) - mean) - pend[0];
+      if constexpr (S > 0) {
+#pragma unroll
+        for (int k = 0; k + 1 < S; ++k) pend[k] = fma(at(t, k + 1), w, pend[k + 1]);
+        pend[S - 1] = at(t, S) * w;
+      }
+      at(t, nxt) = w / at(t, C_D);
+    }
+    double sx2;
+    const double q2 = back_pass(std::true_type{}, cur, nxt, alpha, omega, sx2);
+    const double mean2 = sx2 * invT, v2 = variance(nxt, mean2);
+    const double f2 = omega * q2 - 0.5 * prec * (v2 - mu) * (v2 - mu);
+    if (f2 >= f) {
+      const int tmp = cur; cur = nxt; nxt = tmp;
+      f = f2; mean = mean2; v = v2;
+    } else {
+      alpha *= 0.5;
+    }
+  }
+  for (int t = 0; t < T; ++t) st_stream(out + (int64_t)t * out_ld, (Tout)at(t, cur));
+}
+
 template <typename Tin, int NW, int L, int U, int MODE, int PF>
 __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgParams<Tin, NW, L, U> p) {
   constexpr int S = L + U;
   constexpr int NT = S + 1;
+  constexpr int NTS = WsCols<MODE, NT>::value;
+  constexpr bool FWDLIKE = (MODE == MODE_FWD || MODE == MODE_GV);  // means in, trajectories out
   const int lane = threadIdx.x;
   const int item = blockIdx.x;
   const int urank = p.urank0 + item / p.n_groups;
@@ -64,11 +171,11 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
 
   const Tin* mptr = p.means + row0 * p.in_ld + ch.in_col;
   const Tin* vptr = p.vars + (var_global ? 0 : row0 * p.var_ld) + ch.in_col;
-  double* ws = p.ws + (size_t)item * ((size_t)p.max_T * NT * 32) + lane;
+  double* ws = p.ws + (size_t)item * ((size_t)p.max_T * NTS * 32) + lane;
 
   // ---- pass-through chains (flags & 1): plain copy (fwd) / gradient of a copy (grad) -----------
   if (active && (ch.flags & 1)) {
-    if (MODE == MODE_FWD) {
+    if (FWDLIKE) {
       Tin* o = reinterpret_cast<Tin*>(p.out) + orow0 * p.out_ld + ch.out_col;
       for (int t = 0; t < T; ++t) o[(int64_t)t * p.out_ld] = mptr[(int64_t)t * p.in_ld];
     } else if (MODE == MODE_GRAD) {
@@ -90,11 +197,11 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
 #pragma unroll
       for (int w = 0; w < NW; ++w) {
         if (w < nw) {
-          if (MODE == MODE_FWD) m[w] = ld_stream(mptr + (int64_t)t * p.in_ld + w * ch.win_stride);
+          if (FWDLIKE) m[w] = ld_stream(mptr + (int64_t)t * p.in_ld + w * ch.win_stride);
           v[w] = var_global ? gv[w] : ld_stream(vptr + (int64_t)t * p.var_ld + w * ch.win_stride);
         }
       }
-      if (MODE != MODE_FWD) g = load_go(p.go, p.go_f64, (row0 + t) * p.go_ld + chain);
+      if (!FWDLIKE) g = load_go(p.go, p.go_f64, (row0 + t) * p.go_ld + chain);
     }
   };
   // tau_w[t] with the reference's edge rule; tm = tau * mu (paramgen/_mlpg.py:188-195)
@@ -170,7 +277,7 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
           acc[m] = a;
         }
         double bb;
-        if (MODE == MODE_FWD) {
+        if (FWDLIKE) {
           bb = 0.0;
 #pragma unroll
           for (int w = 0; w < NW; ++w)
@@ -198,8 +305,9 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
           report_not_pd(p.status, utt, chain, t + 1);
         }
         const double ivd = __drcp_rn(d);
-        double* wsp = ws + (size_t)t * (NT * 32);
+        double* wsp = ws + (size_t)t * (NTS * 32);
         wsp[0] = bb * ivd;
+        if (MODE == MODE_GV) wsp[NT * 32] = d;
 #pragma unroll
         for (int k = S; k >= 2; --k) {
           zz[k] = zz[k - 1];
@@ -231,7 +339,7 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
 #pragma unroll
     for (int j = 0; j <= S; ++j) l[j] = 0.0;
     if (t >= 0) {
-      const double* wsp = ws + (size_t)t * (NT * 32);
+      const double* wsp = ws + (size_t)t * (NTS * 32);
       z = wsp[0];
 #pragma unroll
       for (int j = 1; j <= S; ++j) l[j] = wsp[j * 32];
@@ -241,6 +349,7 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
   for (int j = 0; j < PF; ++j) load_ws(T - 1 - j, rz[j], rl[j]);
 
   const int t_end = (MODE == MODE_GRAD) ? -L : 0;
+  double sum_cm = 0.0;  // MODE_GV: sum of c_m over frames, T-1 down to 0
   for (int t0 = T - 1; t0 >= t_end; t0 -= PF) {
 #pragma unroll
     for (int jj = 0; jj < PF; ++jj) {
@@ -254,7 +363,10 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
         if (t < 0) y = 0.0;
         yw[0] = y;
         load_ws(t - PF, rz[jj], rl[jj]);
-        if (MODE != MODE_GRAD) {
+        if (MODE == MODE_GV) {
+          ws[(size_t)t * (NTS * 32) + (NT + 1) * 32] = y;  // c_m, refined below
+          sum_cm += y;
+        } else if (MODE != MODE_GRAD) {
           if (solve) st_stream(reinterpret_cast<Tin*>(p.out) + (orow0 + t) * p.out_ld + ch.out_col, (Tin)y);
         } else {
           // row r = t + L of the gradient: tau_w[r] * sum_k c[w][L+k] x[r+k],  x[r+k] = yw[L+k]
@@ -281,6 +393,15 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
           }
         }
       }
+    }
+  }
+
+  if constexpr (MODE == MODE_GV) {
+    if (solve) {
+      Tin* o = reinterpret_cast<Tin*>(p.out) + orow0 * p.out_ld + ch.out_col;
+      gv_refine<S, NTS>(ws, T, sum_cm, p.gv_mean[ch.out_col], 1.0 / p.gv_var[ch.out_col],
+                        p.gv_weight > 0.0 ? p.gv_weight : 1.0 / ((double)nw * (double)T), p.gv_n_iter, p.gv_step,
+                        o, p.out_ld);
     }
   }
 }
@@ -356,8 +477,9 @@ static int launch_as(const MlpgParams<Tin, NW, L, U>& p, const AsGeom& g, size_t
 }
 
 template <typename Tin, int NW, int L, int U, int MODE>
-static int launch_mlpg(const nnk_mlpg_args_t& a, cudaStream_t st) {
+static int launch_mlpg(const nnk_mlpg_args_t& a, const nnk_mlpg_gv_t* gv, cudaStream_t st) {
   constexpr int NT = L + U + 1;
+  constexpr int NTS = WsCols<MODE, NT>::value;
   constexpr int PF = (L + U <= 2) ? 4 : 2;
   constexpr int ES = (int)sizeof(Tin);
   constexpr bool GRAD = (MODE == MODE_GRAD);
@@ -368,14 +490,16 @@ static int launch_mlpg(const nnk_mlpg_args_t& a, cudaStream_t st) {
   p.utt_off = a.utt_off; p.out_off = a.out_off; p.utt_len = a.utt_len; p.order = a.order; p.chains = a.chains;
   p.n_utt = a.n_utt; p.n_chain = a.n_chain; p.n_groups = (a.n_chain + 31) / 32; p.max_T = a.max_T;
   p.ws = (double*)a.workspace; p.status = (unsigned long long*)a.status_word;
-  const size_t per_item = (size_t)a.max_T * NT * 32 * sizeof(double);
+  p.gv_mean = gv ? gv->gv_mean : nullptr; p.gv_var = gv ? gv->gv_var : nullptr;
+  p.gv_step = gv ? gv->step : 0.0; p.gv_weight = gv ? gv->weight : 0.0; p.gv_n_iter = gv ? gv->n_iter : 0;
+  const size_t per_item = (size_t)a.max_T * NTS * 32 * sizeof(double);
   size_t items_cap = per_item ? a.workspace_bytes / per_item : 0;
   int utt_per_launch = (int)(items_cap / (size_t)p.n_groups);
   if (utt_per_launch < 1) { set_error("workspace too small: need >= %zu bytes", per_item * p.n_groups); return NNK_ERR_WORKSPACE; }
   // The staged kernel serves forward solves and gradients with a float32 grad_out (what autograd hands over)
   // when the window set fills the instance (nw == NW) and the rows fit as_geometry's rings.  It is compiled only
-  // for NT <= 5 and never for nnk_mlpg_solve; everything else runs mlpg_kernel.
-  constexpr bool CAN_AS = (MODE != MODE_SOLVE) && (NT <= 5);
+  // for NT <= 5 and never for nnk_mlpg_solve or nnk_mlpg_gv; everything else runs mlpg_kernel.
+  constexpr bool CAN_AS = (MODE == MODE_FWD || MODE == MODE_GRAD) && (NT <= 5);
   // float32 forward solves with two or more chain groups: one CTA per pair of groups (an odd last group runs
   // with an empty second half), when that geometry fits two CTAs per SM.  Float64 rows and the gradient keep
   // one group per CTA, and so do band depths S > 2: at the 128 registers of two 256-thread CTAs per SM the
@@ -417,17 +541,17 @@ static int launch_mlpg(const nnk_mlpg_args_t& a, cudaStream_t st) {
 }
 
 template <typename Tin, int MODE>
-static int dispatch_inst(const nnk_mlpg_args_t& a, cudaStream_t st) {
+static int dispatch_inst(const nnk_mlpg_args_t& a, cudaStream_t st, const nnk_mlpg_gv_t* gv = nullptr) {
   int inst = -1;
   if (pick_instance(a.win, inst) < 0) {
     set_error("unsupported window set: nw=%d (max %d) or half-width > %d", a.win.nw, NNK_MAX_WIN, NNK_MAX_HALF);
     return NNK_ERR_UNSUPPORTED;
   }
   switch (inst) {
-    case 0: return launch_mlpg<Tin, 1, 0, 0, MODE>(a, st);
-    case 1: return launch_mlpg<Tin, 3, 1, 1, MODE>(a, st);
-    case 2: return launch_mlpg<Tin, 3, 2, 2, MODE>(a, st);
-    default: return launch_mlpg<Tin, NNK_MAX_WIN, NNK_MAX_HALF, NNK_MAX_HALF, MODE>(a, st);
+    case 0: return launch_mlpg<Tin, 1, 0, 0, MODE>(a, gv, st);
+    case 1: return launch_mlpg<Tin, 3, 1, 1, MODE>(a, gv, st);
+    case 2: return launch_mlpg<Tin, 3, 2, 2, MODE>(a, gv, st);
+    default: return launch_mlpg<Tin, NNK_MAX_WIN, NNK_MAX_HALF, NNK_MAX_HALF, MODE>(a, gv, st);
   }
 }
 
@@ -447,13 +571,21 @@ static int check_args(const nnk_mlpg_args_t* a, bool grad) {
 
 using namespace nnk;
 
-extern "C" size_t nnk_mlpg_workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T, const nnk_windows_t* win) {
+static size_t workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T, const nnk_windows_t* win, int extra_cols) {
   int inst = -1;
   if (!win) return 0;
   const int S = pick_instance(*win, inst);
   if (S < 0) return 0;
   const size_t groups = (size_t)((n_chain + 31) / 32);
-  return (size_t)n_utt * groups * (size_t)max_T * (size_t)(S + 1) * 32 * sizeof(double);
+  return (size_t)n_utt * groups * (size_t)max_T * (size_t)(S + 1 + extra_cols) * 32 * sizeof(double);
+}
+
+extern "C" size_t nnk_mlpg_workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T, const nnk_windows_t* win) {
+  return workspace_bytes(n_utt, n_chain, max_T, win, 0);
+}
+
+extern "C" size_t nnk_mlpg_gv_workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T, const nnk_windows_t* win) {
+  return workspace_bytes(n_utt, n_chain, max_T, win, WsCols<MODE_GV, 0>::value);
 }
 
 #ifdef NNK_AS_PROF
@@ -492,4 +624,18 @@ extern "C" int nnk_mlpg_grad(const nnk_mlpg_args_t* a, void* stream) {
   DeviceGuard guard(a->out);
   cudaStream_t st = (cudaStream_t)stream;
   return a->dtype == NNK_F32 ? dispatch_inst<float, MODE_GRAD>(*a, st) : dispatch_inst<double, MODE_GRAD>(*a, st);
+}
+
+extern "C" int nnk_mlpg_gv(const nnk_mlpg_args_t* a, const nnk_mlpg_gv_t* gv, void* stream) {
+  int r = check_args(a, false);
+  if (r < 0) return r;
+  NNK_REQUIRE(gv != nullptr, NNK_ERR_ARG, "gv is NULL");
+  NNK_REQUIRE(gv->n_iter >= 0, NNK_ERR_ARG, "n_iter must be >= 0");
+  NNK_REQUIRE(gv->step > 0.0, NNK_ERR_ARG, "step must be > 0");
+  NNK_REQUIRE(!(gv->weight < 0.0) && gv->weight == gv->weight, NNK_ERR_ARG, "weight must be > 0 (or 0 for 1 / (nw T))");
+  if (r > 0) return NNK_OK;
+  NNK_REQUIRE(gv->gv_mean && gv->gv_var, NNK_ERR_ARG, "NULL gv_mean / gv_var");
+  DeviceGuard guard(a->out);
+  cudaStream_t st = (cudaStream_t)stream;
+  return a->dtype == NNK_F32 ? dispatch_inst<float, MODE_GV>(*a, st, gv) : dispatch_inst<double, MODE_GV>(*a, st, gv);
 }

@@ -4,7 +4,15 @@
 
 namespace nnk {
 
-enum { MODE_FWD = 0, MODE_GRAD = 1, MODE_SOLVE = 2 };
+// MODE_GV: the forward solve followed by the global-variance refinement of nnk_mlpg_gv (mlpg_kernel only)
+enum { MODE_FWD = 0, MODE_GRAD = 1, MODE_SOLVE = 2, MODE_GV = 3 };
+
+// scratch columns per frame of one work item: the S + 1 factor columns, and in MODE_GV four more
+// (pivot d, c_m, and the current / trial trajectory)
+template <int MODE, int NT>
+struct WsCols {
+  static constexpr int value = NT + (MODE == MODE_GV ? 4 : 0);
+};
 
 template <int NW, int L, int U>
 struct WinTab {
@@ -34,6 +42,11 @@ struct MlpgParams {
   double* ws;
   unsigned long long* status;
   WinTab<NW, L, U> win;
+  // MODE_GV only (see nnk_mlpg_gv_t); the other modes leave them zero
+  const double* gv_mean;
+  const double* gv_var;
+  double gv_step, gv_weight;
+  int gv_n_iter;
 };
 
 }  // namespace nnk

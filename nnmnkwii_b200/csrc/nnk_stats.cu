@@ -265,6 +265,56 @@ static void launch_affine(const void* x, const void* a, const void* b, void* out
   else column_affine_kernel<Tin, T, 1><<<(unsigned)g, AF_BLOCK, 0, st>>>(xp, ap, bp, op, n, D);
 }
 
+// segment_moments_kernel (nnk_segment_moments): per-segment column mean and population variance, two passes.
+// Block = 32 columns x SM_RS row slices of one segment; slice k sums rows k, k + SM_RS, ... in order and the
+// slices are folded in index order, so the result depends only on the segment's rows.
+constexpr int SM_RS = 8;
+
+template <typename Tin>
+__global__ void __launch_bounds__(32 * SM_RS)
+    segment_moments_kernel(const Tin* __restrict__ x, int D, int64_t ld, const int64_t* __restrict__ utt_off,
+                           const int32_t* __restrict__ utt_len, int u0, double* __restrict__ mean,
+                           double* __restrict__ var) {
+  __shared__ double part[SM_RS][32];
+  __shared__ double col_mean[32];
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  const int c = blockIdx.x * 32 + tx;
+  const int u = u0 + blockIdx.y;
+  const int64_t r0 = utt_off[u];
+  const int64_t n = utt_len ? (int64_t)utt_len[u] : utt_off[u + 1] - r0;
+  const bool on = c < D;
+  const Tin* col = x + r0 * ld + (on ? c : 0);
+  double s = 0.0;
+  if (on)
+    for (int64_t r = ty; r < n; r += SM_RS) s += (double)col[r * ld];
+  part[ty][tx] = s;
+  __syncthreads();
+  if (ty == 0) {
+    double t = 0.0;
+#pragma unroll
+    for (int k = 0; k < SM_RS; ++k) t += part[k][tx];
+    col_mean[tx] = t / (double)n;
+  }
+  __syncthreads();
+  const double m = col_mean[tx];
+  double s2 = 0.0;
+  if (on)
+    for (int64_t r = ty; r < n; r += SM_RS) {
+      const double d = (double)col[r * ld] - m;
+      s2 = fma(d, d, s2);
+    }
+  __syncthreads();
+  part[ty][tx] = s2;
+  __syncthreads();
+  if (ty == 0 && on) {
+    double t = 0.0;
+#pragma unroll
+    for (int k = 0; k < SM_RS; ++k) t += part[k][tx];
+    var[(int64_t)u * D + c] = t / (double)n;
+    if (mean) mean[(int64_t)u * D + c] = m;
+  }
+}
+
 }  // namespace nnk
 
 using namespace nnk;
@@ -324,5 +374,26 @@ extern "C" int nnk_column_affine(const void* x, int32_t x_dtype, int32_t dtype, 
   else launch_affine<double, double>(x, a, b, out, n, D, form, st);
   count_launch();
   NNK_CUDA_CHECK(cudaGetLastError());
+  return NNK_OK;
+}
+
+extern "C" int nnk_segment_moments(const void* X, int32_t dtype, int32_t D, int64_t ld, const int64_t* utt_off,
+                                   const int32_t* utt_len, int32_t n_utt, double* mean, double* var, void* stream) {
+  NNK_REQUIRE(dtype == NNK_F32 || dtype == NNK_F64, NNK_ERR_ARG, "dtype must be NNK_F32 or NNK_F64");
+  NNK_REQUIRE(D >= 0 && n_utt >= 0 && ld >= D, NNK_ERR_ARG, "bad sizes");
+  if (D == 0 || n_utt == 0) return NNK_OK;
+  NNK_REQUIRE(X && utt_off && var, NNK_ERR_ARG, "NULL device pointer");
+  DeviceGuard guard(var);
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 block(32, SM_RS);
+  for (int u0 = 0; u0 < n_utt; u0 += 65535) {
+    const dim3 grid((D + 31) / 32, n_utt - u0 < 65535 ? n_utt - u0 : 65535);
+    if (dtype == NNK_F32)
+      segment_moments_kernel<float><<<grid, block, 0, st>>>((const float*)X, D, ld, utt_off, utt_len, u0, mean, var);
+    else
+      segment_moments_kernel<double><<<grid, block, 0, st>>>((const double*)X, D, ld, utt_off, utt_len, u0, mean, var);
+    count_launch();
+    NNK_CUDA_CHECK(cudaGetLastError());
+  }
   return NNK_OK;
 }

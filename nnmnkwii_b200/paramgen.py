@@ -17,6 +17,10 @@ fallback: without the library / a GPU these functions raise.
 
 Additive, batched entry points (the reference has none -- its notebooks loop over utterances and
 streams in Python): :class:`StreamLayout`, :func:`merlin_layout`, :func:`mlpg_batch`.
+
+Additive, parameter generation considering global variance (Toda, Black & Tokuda 2007, Sec. IV):
+:func:`mlpg_gv`, :func:`mlpg_gv_batch` and the GV statistics :func:`global_variance`,
+:func:`gv_statistics` (csrc/nnk_mlpg.cu ``nnk_mlpg_gv``, csrc/nnk_stats.cu ``nnk_segment_moments``).
 """
 import ctypes
 
@@ -29,6 +33,7 @@ __all__ = [
     "mlpg_grad_batch",
     "build_win_mats", "mlpg", "mlpg_grad", "full_window_mat", "unit_variance_mlpg_matrix", "reshape_means",
     "StreamLayout", "merlin_layout", "mlpg_batch",
+    "mlpg_gv", "mlpg_gv_batch", "global_variance", "gv_statistics",
 ]
 
 
@@ -202,7 +207,7 @@ def mlpg_batch(means, variances, windows, lengths=None, offsets=None, layout=Non
     return out if out.dtype == dtype else out.astype(dtype)
 
 
-def _mlpg_batch_device(means, variances, windows, lengths, offsets, layout, padded, check):
+def _mlpg_batch_device(means, variances, windows, lengths, offsets, layout, padded, check, gv=None):
     import torch
 
     from . import _device as dev
@@ -227,16 +232,205 @@ def _mlpg_batch_device(means, variances, windows, lengths, offsets, layout, padd
         v = v.contiguous()
     out = torch.zeros((n_rows, layout.D_out), dtype=work, device=device)
     if n_utt and max_T and layout.n_chain:
+        if gv is not None:
+            gv = (torch.from_numpy(gv[0]).to(device), torch.from_numpy(gv[1]).to(device)) + tuple(gv[2:])
         dev.run_mlpg(
-            "fwd", means=m, variances=v, rhs=None, out=out,
+            "fwd" if gv is None else "gv", means=m, variances=v, rhs=None, out=out,
             offsets=torch.from_numpy(off).to(device), lengths=dev.lengths_on(lens, device) if padded else None,
             order=torch.from_numpy(order).to(device), chains=dev.chains_on_device(layout.chains, device),
             n_chain=layout.n_chain, max_T=max_T, windows_c=_lib.make_windows(windows),
             in_ld=D, var_ld=0 if var1d else D, go_ld=0, out_ld=layout.D_out,
-            dtype_code=dev.torch_dtype_code(work), go_f64=0, n_utt=n_utt, device=device, check=check)
+            dtype_code=dev.torch_dtype_code(work), go_f64=0, n_utt=n_utt, device=device, check=check, gv=gv)
     if padded:
         out = out.reshape(m.shape[0], m.shape[1], layout.D_out)
     return out if work == dtype else out.to(dtype)
+
+
+# ---------------------------------------------------------------------------------------------------
+# global variance (additive)
+# ---------------------------------------------------------------------------------------------------
+def _host_vector(x, name):
+    from ._device import is_tensor
+    if is_tensor(x):
+        x = x.detach().cpu().numpy()
+    try:
+        return np.ascontiguousarray(np.asarray(x, dtype=np.float64).ravel())
+    except (TypeError, ValueError):
+        raise ValueError("%s must be a sequence of numbers" % name)
+
+
+def _gv_args(gv_mean, gv_var, layout, n_iter, step, weight):
+    """Checked GV parameters ``(gv_mean, gv_var, n_iter, step, weight)`` (float64 host vectors of
+    ``layout.D_out`` entries; ``weight`` 0 = the default ``1 / (nw T)``).  Entries of copied columns
+    are not used and not checked."""
+    gm, gvv = _host_vector(gv_mean, "gv_mean"), _host_vector(gv_var, "gv_var")
+    for name, a in (("gv_mean", gm), ("gv_var", gvv)):
+        if a.shape != (layout.D_out,):
+            raise ValueError("%s must have one entry per output column (%d), got %d" % (name, layout.D_out, a.size))
+    used = layout.chains["out_col"][layout.chains["flags"] == 0]
+    if not np.all(np.isfinite(gm[used])) or np.any(gm[used] < 0):
+        raise ValueError("gv_mean must be finite and >= 0")
+    if not np.all(np.isfinite(gvv[used]) & (gvv[used] > 0)):
+        raise ValueError("gv_var must be finite and > 0")
+    if isinstance(n_iter, bool) or int(n_iter) != n_iter or n_iter < 0:
+        raise ValueError("n_iter must be an integer >= 0, got %r" % (n_iter,))
+    if not (np.isfinite(step) and step > 0):
+        raise ValueError("step must be finite and > 0, got %r" % (step,))
+    if weight is not None and not (np.isfinite(weight) and weight > 0):
+        raise ValueError("weight must be finite and > 0 (or None), got %r" % (weight,))
+    gm, gvv = gm.copy(), gvv.copy()
+    gm[np.setdiff1d(np.arange(layout.D_out), used)] = 0.0  # copied columns: never read
+    gvv[np.setdiff1d(np.arange(layout.D_out), used)] = 1.0
+    return gm, gvv, int(n_iter), float(step), 0.0 if weight is None else float(weight)
+
+
+def mlpg_gv_batch(means, variances, windows, gv_mean, gv_var, lengths=None, offsets=None, layout=None, n_iter=20,
+                  step=1.0, weight=None, check=True, out=None):
+    r"""Batched parameter generation considering global variance (additive API).
+
+    Per utterance and smoothed output column, starting from the :func:`mlpg_batch` trajectory
+    :math:`c_m = P^{-1} b`, maximises
+
+    .. math:: F(c) = \omega (b^T c - \tfrac12 c^T P c) - \tfrac{1}{2 \sigma^2} (v(c) - \mu)^2
+
+    with :math:`v(c)` the population variance of :math:`c` over the utterance's frames (Toda, Black &
+    Tokuda 2007, Sec. IV, diagonal GV covariance).  The start point rescales :math:`c_m` to variance
+    :math:`\mu`; each of the ``n_iter`` trials takes the step ``alpha * ((c_m - c) + P^-1 g / omega)``
+    (``g`` the gradient of the GV term) and keeps it when :math:`F` does not decrease, otherwise halves
+    ``alpha`` (which starts at ``step``).  See DESIGN.md 3.15.
+
+    Args:
+        means, variances, windows, lengths, offsets, layout, check: as :func:`mlpg_batch` (flat or padded,
+            per-frame or global ``(D,)`` variances, NumPy arrays or torch CUDA tensors).
+        gv_mean, gv_var: target GV :math:`\mu` (``>= 0``) and its variance :math:`\sigma^2` (``> 0``), one
+            entry per output column (``layout.D_out``), e.g. from :func:`gv_statistics`; copied columns
+            (Merlin's vuv) ignore theirs.
+        n_iter: trials (``>= 0``; 0 returns the rescaled start point).
+        step: initial step ``alpha`` (``> 0``).
+        weight: :math:`\omega` (``> 0``); default ``1 / (num_windows * T)`` per utterance.
+        out: optional ``(sum_T, D_out)`` NumPy buffer of the working dtype (flat host form only).
+
+    Returns:
+        Trajectories shaped and typed like :func:`mlpg_batch`'s.  Arithmetic is float64.
+    """
+    import torch
+
+    from . import _device as dev
+    padded = means.ndim == 3
+    D = means.shape[-1]
+    if layout is None:
+        layout = StreamLayout.single(D, len(windows))
+    if layout.D_in != D:
+        raise ValueError("layout covers %d input columns, means have %d" % (layout.D_in, D))
+    if padded and lengths is None:
+        raise ValueError("padded (B, Tmax, D) input needs lengths")
+    gv = _gv_args(gv_mean, gv_var, layout, n_iter, step, weight)
+    if dev.is_tensor(means):
+        return _mlpg_batch_device(means, variances, windows, lengths, offsets, layout, padded, check, gv=gv)
+    dtype = np.asarray(means).dtype
+    v_np = np.asarray(variances)
+    work = dtype if (dtype in (np.float32, np.float64) and v_np.dtype == dtype) else np.dtype(np.float64)
+    dev.require_cuda()
+    device = dev.cuda_device()
+    m = torch.from_numpy(np.ascontiguousarray(means, dtype=work)).to(device)
+    v = torch.from_numpy(np.ascontiguousarray(v_np, dtype=work)).to(device)
+    y = _mlpg_batch_device(m, v, windows, lengths, offsets, layout, padded, check, gv=gv).cpu().numpy()
+    if out is not None:
+        if padded or out.shape != y.shape or out.dtype != work or not out.flags.c_contiguous:
+            raise ValueError("out must be a C-contiguous %s array of dtype %s" % (y.shape, work))
+        out[...] = y
+        y = out
+    return y if y.dtype == dtype else y.astype(dtype)
+
+
+def mlpg_gv(mean_frames, variance_frames, windows, gv_mean, gv_var, n_iter=20, step=1.0, weight=None):
+    """Parameter generation considering global variance for one utterance, ``(T, D) -> (T, static_dim)``:
+    :func:`mlpg`'s arguments plus the GV parameters of :func:`mlpg_gv_batch` (``gv_mean`` / ``gv_var`` of
+    length ``static_dim``).  NumPy in, NumPy out (a CUDA tensor stays a CUDA tensor)."""
+    T, D = mean_frames.shape
+    return mlpg_gv_batch(mean_frames, variance_frames, windows, gv_mean, gv_var, lengths=[T], n_iter=n_iter,
+                         step=step, weight=weight)
+
+
+def _moments(x, lengths, offsets, want_mean):
+    """Per-utterance column mean (optional) and population variance on the device, float64 tensors
+    ``(n_utt, D)``; ``(T, D)`` input is one utterance."""
+    import torch
+
+    from . import _device as dev
+    shape = tuple(x.shape)
+    if len(shape) == 3:
+        if lengths is None:
+            raise ValueError("padded (B, Tmax, D) input needs lengths")
+        B, Tmax, D = shape
+        lens = dev.check_lengths(lengths, B)
+        if lens.size and int(lens.max()) > Tmax:
+            raise ValueError("lengths exceed Tmax = %d" % Tmax)
+        off = np.arange(B + 1, dtype=np.int64) * Tmax
+    elif len(shape) == 2:
+        n_rows, D = shape
+        if offsets is not None:
+            off = np.asarray(dev.check_lengths(offsets, len(offsets)), dtype=np.int64)
+            if len(off) < 1 or off[0] != 0 or off[-1] != n_rows or np.any(np.diff(off) < 0):
+                raise ValueError("offsets must rise from 0 to %d" % n_rows)
+        elif lengths is not None:
+            lens = dev.check_lengths(lengths, len(lengths))
+            off = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+            if off[-1] != n_rows:
+                raise ValueError("lengths sum to %d, x has %d rows" % (off[-1], n_rows))
+        else:
+            off = np.array([0, n_rows], dtype=np.int64)
+        lens = np.diff(off)
+    else:
+        raise ValueError("x must be (T, D), (sum_T, D) or (B, Tmax, D)")
+    if lens.size and int(lens.min()) < 1:
+        raise ValueError("every utterance needs at least one frame (a zero-length utterance has no variance)")
+    dev.require_cuda()
+    xt = dev.to_device(x)
+    if xt.dtype not in (torch.float32, torch.float64):
+        xt = xt.to(torch.float64)
+    xt = xt.contiguous()
+    n_utt = len(lens)
+    device = xt.device
+    var = torch.empty((n_utt, D), dtype=torch.float64, device=device)
+    mean = torch.empty((n_utt, D), dtype=torch.float64, device=device) if want_mean else None
+    if n_utt and D:
+        off_t = torch.from_numpy(off).to(device)
+        len_t = dev.lengths_on(lens, device)
+        _lib.check(_lib.lib.nnk_segment_moments(
+            xt.data_ptr(), dev.torch_dtype_code(xt.dtype), D, D, off_t.data_ptr(), len_t.data_ptr(), n_utt,
+            mean.data_ptr() if want_mean else None, var.data_ptr(), dev.current_stream_ptr(device)),
+            "nnk_segment_moments")
+    return mean, var
+
+
+def global_variance(x, lengths=None, offsets=None):
+    """Global variance (per-utterance, per-column population variance over frames), float64.
+
+    Args:
+        x: ``(T, D)`` (one utterance), a padded ``(B, Tmax, D)`` batch with ``lengths``, or a flat
+            ``(sum_T, D)`` batch with ``offsets`` (or ``lengths``).  NumPy array or torch tensor,
+            float32 / float64 (accumulated in float64, two passes, fixed order).
+
+    Returns:
+        ``(D,)`` for ``(T, D)`` input without ``lengths`` / ``offsets``, otherwise ``(B, D)``; a NumPy
+        array for NumPy input, a tensor on the input's device for a tensor.  A zero-length utterance
+        raises ``ValueError``.
+    """
+    from . import _device as dev
+    _, var = _moments(x, lengths, offsets, False)
+    if x.ndim == 2 and lengths is None and offsets is None:
+        var = var[0]
+    return dev.like_input(var, x)
+
+
+def gv_statistics(x, lengths=None, offsets=None):
+    """``(gv_mean, gv_var)``: mean and population variance over utterances of :func:`global_variance`
+    (same arguments), each ``(D,)`` float64 -- the GV model :func:`mlpg_gv_batch` takes."""
+    from . import _device as dev
+    _, gv = _moments(x, lengths, offsets, False)
+    mean, var = _moments(gv, None, None, True)
+    return dev.like_input(mean[0], x), dev.like_input(var[0], x)
 
 
 # ---------------------------------------------------------------------------------------------------
