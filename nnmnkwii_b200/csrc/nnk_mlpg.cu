@@ -53,7 +53,7 @@ __device__ __forceinline__ double load_go(const void* go, int is_f64, int64_t id
 // trajectory live in columns NT+2 / NT+3 and swap roles on acceptance.  Every sum runs over t in a fixed order, so
 // results do not depend on the batch around the chain.
 template <int S, int NTS, typename Tout>
-__device__ __forceinline__ void gv_refine(double* ws, int T, double sum_cm, double mu, double prec, double omega,
+__device__ __forceinline__ void gv_refine(double* ws, int T, double mu, double prec, double omega,
                                           int n_iter, double step, Tout* out, int64_t out_ld) {
   constexpr int NT = S + 1, C_D = NT, C_CM = NT + 1, SP = S > 0 ? S : 1;
   auto at = [&](int t, int col) -> double& { return ws[(size_t)t * (NTS * 32) + col * 32]; };
@@ -105,8 +105,13 @@ __device__ __forceinline__ void gv_refine(double* ws, int T, double sum_cm, doub
     return q;
   };
 
-  // start point
-  const double mean_m = sum_cm * invT;
+  // start point.  The mean of c_m is taken about its last frame, so that a c_m with one value at every frame has
+  // v(c_m) == 0 exactly: (sum_t c_m,t) * (1 / T) can miss that value by an ulp, which sqrt(mu / v) would scale
+  // up to the target variance.
+  const double c_last = at(T - 1, C_CM);
+  double dsum = 0.0;
+  for (int t = T - 1; t >= 0; --t) dsum += at(t, C_CM) - c_last;
+  const double mean_m = c_last + dsum * invT;
   const double vm = variance(C_CM, mean_m);
   int cur = NT + 2, nxt = NT + 3;
   double sx;
@@ -349,7 +354,6 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
   for (int j = 0; j < PF; ++j) load_ws(T - 1 - j, rz[j], rl[j]);
 
   const int t_end = (MODE == MODE_GRAD) ? -L : 0;
-  double sum_cm = 0.0;  // MODE_GV: sum of c_m over frames, T-1 down to 0
   for (int t0 = T - 1; t0 >= t_end; t0 -= PF) {
 #pragma unroll
     for (int jj = 0; jj < PF; ++jj) {
@@ -365,7 +369,6 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
         load_ws(t - PF, rz[jj], rl[jj]);
         if (MODE == MODE_GV) {
           ws[(size_t)t * (NTS * 32) + (NT + 1) * 32] = y;  // c_m, refined below
-          sum_cm += y;
         } else if (MODE != MODE_GRAD) {
           if (solve) st_stream(reinterpret_cast<Tin*>(p.out) + (orow0 + t) * p.out_ld + ch.out_col, (Tin)y);
         } else {
@@ -399,7 +402,7 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
   if constexpr (MODE == MODE_GV) {
     if (solve) {
       Tin* o = reinterpret_cast<Tin*>(p.out) + orow0 * p.out_ld + ch.out_col;
-      gv_refine<S, NTS>(ws, T, sum_cm, p.gv_mean[ch.out_col], 1.0 / p.gv_var[ch.out_col],
+      gv_refine<S, NTS>(ws, T, p.gv_mean[ch.out_col], 1.0 / p.gv_var[ch.out_col],
                         p.gv_weight > 0.0 ? p.gv_weight : 1.0 / ((double)nw * (double)T), p.gv_n_iter, p.gv_step,
                         o, p.out_ld);
     }

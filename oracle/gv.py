@@ -49,7 +49,7 @@ def build_system(mean, var, windows):
             ok = (r + k1 >= 0) & (r + k1 < T)
             np.add.at(b, (r + k1)[ok], tau[ok, w] * mean[ok, w] * coef[l + k1])
     Pu = np.zeros((S + 1, T))
-    for k in range(S + 1):
+    for k in range(min(S, T - 1) + 1):  # a diagonal at k >= T lies outside the matrix
         Pu[S - k, k:] = Pd[k, :T - k]
     return Pu, b
 
@@ -59,7 +59,7 @@ def band_matvec(Pu, c):
     S = Pu.shape[0] - 1
     T = len(c)
     y = Pu[S] * c
-    for k in range(1, S + 1):
+    for k in range(1, min(S, T - 1) + 1):
         d = Pu[S - k, k:]
         y[:T - k] += d * c[k:]
         y[k:] += d * c[:T - k]

@@ -6,7 +6,9 @@ KC = 1 or 2, K buckets 16 / 24 / 32), the shift-invariant sweep (`nnk_uv_apply_t
 8 / 16 / 24 / 32 / 48 / 64, nw = 1..3) or the per-row table (`nnk_uv_apply`: K > 64, a shift-invariant run
 shorter than 64 rows, or a float64 R).  Where a path begins depends on the float32 R the device builds, so
 each case scans a short list of window sets (host-side K values in the comments, at T = 400) and takes the
-first one whose band lands where the case wants; the kernel name is then asserted from the profiler."""
+first one whose band lands where the case wants; the kernel name is then asserted from the profiler.  The names
+are collected in a child process (`variant_mirror.profiled_in_child`): late in a long pytest process,
+torch.profiler has returned empty profiles for these calls on an H100."""
 import numpy as np
 import pytest
 
@@ -100,56 +102,27 @@ def _dense_ref(R64, x, go, nw, reshaped):
     return y, g
 
 
-def _run_and_check(Rt, band, bound_kind):
-    """Forward and backward, plain and reshaped layouts, odd and even static_dim."""
-    import torch
-    from nnmnkwii_b200.autograd import UnitVarianceMLPG
-    fwd_path, bwd_path = _paths(band)
-    T, nw = band.T, band.nw
-    R64 = Rt.double().cpu().numpy()
-    dtype = "double" if Rt.dtype == torch.float64 else "float"
-    rng = np.random.default_rng(band.K)
-    for sd in (5, 6):
-        for reshaped in (False, True):
-            shape = (2, nw * T, sd) if reshaped else (2, T, nw * sd)
-            xh = rng.standard_normal(shape).astype(np.float32 if dtype == "float" else np.float64)
-            goh = rng.standard_normal((2, T, sd)).astype(xh.dtype)
-            x = torch.from_numpy(xh).cuda().requires_grad_(True)
-            y, err, names = M.profiled(lambda: UnitVarianceMLPG.apply(x, Rt))
-            assert err is None, err
-            _expect_kernel(names, fwd_path, "fwd", dtype)
-            go = torch.from_numpy(goh).cuda()
-            g, err, names = M.profiled(lambda: torch.autograd.grad(y, x, go, retain_graph=True)[0])
-            assert err is None, err
-            _expect_kernel(names, bwd_path, "bwd", dtype)
-            y_ref, g_ref = _dense_ref(R64, xh.astype(np.float64), goh.astype(np.float64), nw, reshaped)
-            got_y, got_g = y.detach().cpu().numpy(), g.cpu().numpy()
-            assert got_y.shape == y_ref.shape and got_g.shape == g_ref.shape
-            if bound_kind == "table":
-                tol = 2e-6 if dtype == "float" else 1e-13
-                assert rel_err(got_y, y_ref) < tol and rel_err(got_g, g_ref) < tol, (sd, reshaped)
-            else:
-                # shift-invariant rows: the bound _uvmlpg.py documents, (2K+1) nw 2^-23 max|R| max|x| per output
-                peak = np.abs(R64).max()
-                scale = (2 * band.K + 1) * nw * 2.0 ** -23 * peak
-                assert np.abs(got_y - y_ref).max() <= scale * np.abs(xh).max(), (sd, reshaped)
-                assert np.abs(got_g - g_ref).max() <= scale * np.abs(goh).max(), (sd, reshaped)
+def _inputs(band, dtype, sd, reshaped):
+    nw, T = band.nw, band.T
+    rng = np.random.default_rng(band.K + 10 * sd + reshaped)
+    shape = (2, nw * T, sd) if reshaped else (2, T, nw * sd)
+    xh = rng.standard_normal(shape).astype(np.float32 if dtype == "float" else np.float64)
+    goh = rng.standard_normal((2, T, sd)).astype(xh.dtype)
+    return xh, goh
 
 
-@pytest.mark.parametrize("want,family,cands", [
+COMBOS = [(sd, reshaped) for sd in (5, 6) for reshaped in (False, True)]
+
+
+FACT = [
     ("fact<16,1>", std_c, (5.0, 4.0, 3.0)),
     ("fact<24,1>", std_c, (1.5, 2.0, 1.0)),
     ("fact<32,1>", std_c, (0.7, 0.6, 0.8)),
     ("fact<16,2>", five_c, (5.0, 8.0, 3.0)),
     ("fact<24,2>", five_c, (2.0, 1.5, 3.0)),
     ("fact<32,2>", five_c, (1.0, 0.7)),
-], ids=lambda v: v if isinstance(v, str) else None)
-def test_factored_buckets(want, family, cands):
-    ws, Rt, band = _band_for(want, family, cands)
-    _run_and_check(Rt, band, "bound")
-
-
-@pytest.mark.parametrize("want,family,cands", [
+]
+TOEP = [
     ("toep<8,1>", one_c, (0.05, 0.02)),
     ("toep<16,1>", one_c, (0.15, 0.1, 0.2)),
     ("toep<24,1>", one_c, (0.3, 0.25, 0.33)),
@@ -162,22 +135,120 @@ def test_factored_buckets(want, family, cands):
     ("toep<16,3>", seven3_c, (8.0, 10.0, 12.0)),
     ("toep<48,3>", seven3_c, (1.0, 0.9)),
     ("toep<64,3>", seven3_c, (0.6, 0.55)),
-], ids=lambda v: v if isinstance(v, str) else None)
-def test_toeplitz_buckets(want, family, cands):
+]
+# every case of `_run_and_check`, as `_case` rebuilds it
+CASES = ([("band", want, family.__name__, cands) for want, family, cands in FACT + TOEP]
+         + [("band", "table", "std_c", (0.3, 0.25)), ("short", 0), ("short", 1), ("f64", 0), ("f64", 1)])
+
+
+def _key(case):
+    return tuple(tuple(c) if isinstance(c, (list, tuple)) else c for c in case)
+
+
+@pytest.fixture(scope="module")
+def uv_names():
+    """(case, sd, reshaped, direction) -> names of the UV kernels of that call, all profiled in one child."""
+    cases = [([list(c) if isinstance(c, tuple) else c for c in case], sd, reshaped, d)
+             for case in CASES for sd, reshaped in COMBOS for d in ("fwd", "bwd")]
+    res = M.profiled_in_child("test_kernel_variants_uv_gpu", "launch", [(list(c), r"\buv_\w*kernel\b") for c in cases])
+    out = {}
+    for (case, sd, reshaped, d), (names, err) in zip(cases, res):
+        assert err == "None", (case, err)
+        out[(_key(case), sd, reshaped, d)] = names
+    return out
+
+
+def _run_and_check(names_of, case, Rt, band, bound_kind):
+    """Forward and backward, plain and reshaped layouts, odd and even static_dim; ``names_of`` (the `uv_names`
+    fixture) names the kernel of each call."""
+    import torch
+    from nnmnkwii_b200.autograd import UnitVarianceMLPG
+    fwd_path, bwd_path = _paths(band)
+    T, nw = band.T, band.nw
+    R64 = Rt.double().cpu().numpy()
+    dtype = "double" if Rt.dtype == torch.float64 else "float"
+    for sd, reshaped in COMBOS:
+        for direction, path in (("fwd", fwd_path), ("bwd", bwd_path)):
+            _expect_kernel(names_of[(_key(case), sd, reshaped, direction)], path, direction, dtype)
+        xh, goh = _inputs(band, dtype, sd, reshaped)
+        x = torch.from_numpy(xh).cuda().requires_grad_(True)
+        y = UnitVarianceMLPG.apply(x, Rt)
+        g = torch.autograd.grad(y, x, torch.from_numpy(goh).cuda(), retain_graph=True)[0]
+        y_ref, g_ref = _dense_ref(R64, xh.astype(np.float64), goh.astype(np.float64), nw, reshaped)
+        got_y, got_g = y.detach().cpu().numpy(), g.cpu().numpy()
+        assert got_y.shape == y_ref.shape and got_g.shape == g_ref.shape
+        if bound_kind == "table":
+            tol = 2e-6 if dtype == "float" else 1e-13
+            assert rel_err(got_y, y_ref) < tol and rel_err(got_g, g_ref) < tol, (sd, reshaped)
+        else:
+            # shift-invariant rows: the bound _uvmlpg.py documents, (2K+1) nw 2^-23 max|R| max|x| per output
+            peak = np.abs(R64).max()
+            scale = (2 * band.K + 1) * nw * 2.0 ** -23 * peak
+            assert np.abs(got_y - y_ref).max() <= scale * np.abs(xh).max(), (sd, reshaped)
+            assert np.abs(got_g - g_ref).max() <= scale * np.abs(goh).max(), (sd, reshaped)
+
+
+FAMILIES = {"std_c": std_c, "five_c": five_c, "one_c": one_c, "seven_c": seven_c, "seven3_c": seven3_c}
+_launched = {}
+
+
+def _case(case):
+    """(R, band) of a case: ("band", want, family, cands), ("short", dT) or ("f64", i)."""
+    import torch
+    from nnmnkwii_b200 import _uvmlpg as uv
+    from nnmnkwii_b200 import paramgen as G
+    if case[0] == "band":
+        _, Rt, band = _band_for(case[1], FAMILIES[case[2]], case[3])
+        return Rt, band
+    if case[0] == "short":
+        return _short_run_bands()[case[1]]
+    ws = (windows_set()[2], five_c(1.0))[case[1]]
+    Rt = torch.from_numpy(G.unit_variance_mlpg_matrix(ws, 300)).cuda().double()
+    return Rt, uv.band_of(Rt, Rt.device)
+
+
+def launch(case, sd, reshaped, direction):
+    """One call of `_run_and_check` in a child process: the forward of (case, sd, reshaped), or the backward of
+    the forward made before."""
+    import torch
+    from nnmnkwii_b200.autograd import UnitVarianceMLPG
+    key = (_key(case), sd, reshaped)
+    if direction == "fwd":
+        Rt, band = _launched.get(key[0]) or _case(case)
+        _launched[key[0]] = (Rt, band)
+        xh, goh = _inputs(band, "double" if Rt.dtype == torch.float64 else "float", sd, reshaped)
+        x = torch.from_numpy(xh).cuda().requires_grad_(True)
+        go = torch.from_numpy(goh).cuda()
+        torch.cuda.synchronize()
+        _launched[key] = (x, go, UnitVarianceMLPG.apply(x, Rt))
+    else:
+        x, go, y = _launched[key]
+        torch.autograd.grad(y, x, go, retain_graph=True)
+    torch.cuda.synchronize()
+
+
+@pytest.mark.parametrize("want,family,cands", FACT, ids=lambda v: v if isinstance(v, str) else None)
+def test_factored_buckets(want, family, cands, uv_names):
     ws, Rt, band = _band_for(want, family, cands)
-    _run_and_check(Rt, band, "bound")
+    _run_and_check(uv_names, ("band", want, family.__name__, cands), Rt, band, "bound")
 
 
-def test_table_path_wide_band_float32():
+@pytest.mark.parametrize("want,family,cands", TOEP, ids=lambda v: v if isinstance(v, str) else None)
+def test_toeplitz_buckets(want, family, cands, uv_names):
+    ws, Rt, band = _band_for(want, family, cands)
+    _run_and_check(uv_names, ("band", want, family.__name__, cands), Rt, band, "bound")
+
+
+def test_table_path_wide_band_float32(uv_names):
     """Static coefficient 0.3: K > 64, beyond every shift-invariant kernel."""
     ws, Rt, band = _band_for("table", std_c, (0.3, 0.25))
     assert band.K > 64
-    _run_and_check(Rt, band, "table")
+    _run_and_check(uv_names, ("band", "table", "std_c", (0.3, 0.25)), Rt, band, "table")
 
 
-def test_table_path_short_shift_invariant_run_float32():
-    """Standard windows at the largest T whose shift-invariant run is still shorter than 64 rows (K < 64):
-    the per-row table; one frame more reaches 64 rows and leaves the table on at least one side."""
+def _short_run_bands():
+    """Standard windows: (R, band) at the largest T in 80..129 whose bands both take the per-row table, and one
+    frame more."""
     import torch
     from nnmnkwii_b200 import _uvmlpg as uv
     from nnmnkwii_b200 import paramgen as G
@@ -187,19 +258,27 @@ def test_table_path_short_shift_invariant_run_float32():
         Rt = torch.from_numpy(G.unit_variance_mlpg_matrix(ws, T)).cuda()
         bands[T] = (Rt, uv.band_of(Rt, Rt.device))
     T_last = max(T for T, (_, b) in bands.items() if _paths(b) == ("table", "table"))
-    assert T_last + 1 in bands and _paths(bands[T_last + 1][1]) != ("table", "table")
-    Rt, band = bands[T_last]
-    assert band.K <= 64 and T_last >= uv.TOEPLITZ_MIN_ROWS
-    _run_and_check(Rt, band, "table")
-    _run_and_check(*bands[T_last + 1], "bound")
+    assert T_last + 1 in bands
+    return bands[T_last], bands[T_last + 1]
 
 
-def test_table_path_float64():
+def test_table_path_short_shift_invariant_run_float32(uv_names):
+    """Standard windows at the largest T whose shift-invariant run is still shorter than 64 rows (K < 64):
+    the per-row table; one frame more reaches 64 rows and leaves the table on at least one side."""
+    from nnmnkwii_b200 import _uvmlpg as uv
+    (Rt, band), nxt = _short_run_bands()
+    assert _paths(nxt[1]) != ("table", "table")
+    assert band.K <= 64 and band.T >= uv.TOEPLITZ_MIN_ROWS
+    _run_and_check(uv_names, ("short", 0), Rt, band, "table")
+    _run_and_check(uv_names, ("short", 1), *nxt, "bound")
+
+
+def test_table_path_float64(uv_names):
     import torch
     from nnmnkwii_b200 import _uvmlpg as uv
     from nnmnkwii_b200 import paramgen as G
-    for ws in (windows_set()[2], five_c(1.0)):
+    for i, ws in enumerate((windows_set()[2], five_c(1.0))):
         Rt = torch.from_numpy(G.unit_variance_mlpg_matrix(ws, 300)).cuda().double()
         band = uv.band_of(Rt, Rt.device)
         assert _paths(band) == ("table", "table")
-        _run_and_check(Rt, band, "table")
+        _run_and_check(uv_names, ("f64", i), Rt, band, "table")

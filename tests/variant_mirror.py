@@ -312,26 +312,30 @@ import importlib
 import variant_mirror as M
 mod = importlib.import_module(sys.argv[3])
 launch = getattr(mod, sys.argv[4])
+repeats = sys.argv[6] == "1"
 out = []
 for case, family in json.loads(sys.argv[5]):
     _, err, names = M.profiled(lambda: launch(*case), family)
-    out.append([sorted(set(M.launched(names, family))), repr(err)])
+    names = M.launched(names, family)
+    out.append([sorted(names if repeats else set(names)), repr(err)])
 print(json.dumps(out))
 """
 
 
-def profiled_in_child(module, launcher, cases):
+def profiled_in_child(module, launcher, cases, repeats=False):
     """``[(kernel names of family, repr(error))]`` of ``module.launcher(*case)`` for each ``(case, family)`` of
     ``cases``, each call profiled by `profiled` in a child Python process.  Profiling many calls in the pytest
     process has made torch.profiler lose the records of later modules' calls on an H100; a child process
-    keeps the profiler state of those modules clean."""
+    keeps the profiler state of those modules clean.  The names are distinct, or with ``repeats`` one per
+    launch, so that a caller can count launches."""
     import json
     import os
     import subprocess
     import sys
     here = os.path.dirname(os.path.abspath(__file__))
     root = os.path.dirname(here)
-    res = subprocess.run([sys.executable, "-c", _CHILD_SCRIPT, here, root, module, launcher, json.dumps(cases)],
+    res = subprocess.run([sys.executable, "-c", _CHILD_SCRIPT, here, root, module, launcher, json.dumps(cases),
+                          "1" if repeats else "0"],
                          capture_output=True, text=True, timeout=900, cwd=root)
     assert res.returncode == 0, res.stderr[-3000:]
     return json.loads(res.stdout.strip().splitlines()[-1])
