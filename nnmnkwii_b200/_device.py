@@ -88,7 +88,10 @@ def workspace(device, nbytes):
 
     The allocator is stream-aware -- a block freed after a launch on stream A is only handed out again
     to stream A (or after A has been synchronised) -- so concurrent streams / threads never share a
-    factor scratch, and a steady-state loop gets the same block back without a cudaMalloc."""
+    factor scratch, and a steady-state loop gets the same block back without a cudaMalloc.  That holds
+    because the scratch is allocated on, and only used by, the current stream of ``device``; a tensor
+    kept beyond one call and read from other streams needs ``keep_for_current_stream``.  The block is
+    not cleared: it holds whatever an earlier call left in it."""
     return torch.empty(int(max(nbytes, 256)), dtype=torch.uint8, device=device)
 
 
@@ -102,8 +105,21 @@ def simple_chains(static_dim):
     return ch
 
 
+def keep_for_current_stream(t, device):
+    """Mark cached tensor ``t`` as used by the work about to be enqueued on the current stream of ``device``.
+
+    A cache entry's block belongs to the stream that was current when it was made.  When the cache drops
+    the entry, the allocator may hand that block to the next allocation on that stream at once, even if a
+    kernel on another stream has yet to read it.  ``record_stream`` makes the allocator wait for the work
+    enqueued so far on the current stream before it reuses the block (a no-op on the owning stream)."""
+    t.record_stream(torch.cuda.current_stream(device))
+    return t
+
+
 def constant_on_device(a, device):
-    """Device copy of a small host constant (chain table, filter weights), kept in a bounded cache."""
+    """Device copy of a small host constant (chain table, filter weights), kept in a bounded cache.  The
+    caller enqueues its reads on the current stream of ``device``; an eviction never recycles the block
+    before they have run (see keep_for_current_stream)."""
     key = (a.tobytes(), a.dtype.str, a.shape, str(device))
     t = _const_cache.get(key)
     if t is None:
@@ -111,7 +127,7 @@ def constant_on_device(a, device):
         if len(_const_cache) >= 64:
             _const_cache.clear()
         _const_cache[key] = t
-    return t
+    return keep_for_current_stream(t, device)
 
 
 def chains_on_device(chains_np, device):

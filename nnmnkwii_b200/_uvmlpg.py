@@ -80,11 +80,14 @@ def _factor_taps(taps, K, peak):
 
 
 def band_of(R, device):
-    """Band tables of R (cached on (data_ptr, version, shape, device))."""
+    """Band tables of R (cached on (data_ptr, version, shape, device)).  The caller reads them on the
+    current stream of ``device``; an eviction never recycles their blocks before those reads have run."""
     assert R.dim() == 2 and R.shape[1] % R.shape[0] == 0
     key = (R.data_ptr(), R._version, tuple(R.shape), R.dtype, str(R.device), str(device))
     hit = _band_cache.get(key)
     if hit is not None and hit[0]() is R:
+        dev.keep_for_current_stream(hit[1].Rb, device)
+        dev.keep_for_current_stream(hit[1].RbT, device)
         return hit[1]
     Rd = R.detach().to(device)
     if Rd.dtype not in (torch.float32, torch.float64):

@@ -93,6 +93,10 @@ class UnitVarianceMLPG(Function):
 
     ``f : (T x D) -> (T, static_dim)`` or ``f : (T*num_windows, static_dim) -> (T, static_dim)``,
     2-D or 3-D (batched) ``means``; ``R`` from :func:`nnmnkwii_b200.paramgen.unit_variance_mlpg_matrix`.
+
+    The band tables of ``R`` are cached on its storage pointer and torch's version counter.  Changing ``R``
+    in place through torch bumps that counter; changing it through a NumPy view or ``R.data`` does not, and
+    the stale tables are then used.  Pass a new tensor after such a change.
     """
 
     @staticmethod

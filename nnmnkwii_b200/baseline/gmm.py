@@ -229,7 +229,10 @@ _ILL_DEFINED = ("Fitting the mixture model failed because some components have i
 
 class _EmState(object):
     """Device buffers of one fit: the frames, the responsibilities, the parameters, the workspace of
-    csrc/nnk_gmm_em.cu and the filled ``nnk_gmm_em_args_t``."""
+    csrc/nnk_gmm_em.cu and the filled ``nnk_gmm_em_args_t``.  Each step runs on the current stream at the
+    time of the call.  The buffers belong to the stream current at construction, so a step on another
+    stream must be ordered after that stream's work, and the object must outlive the steps it enqueued
+    (within ``fit_predict`` both hold: one stream, synchronising steps)."""
 
     def __init__(self, X, K, reg_covar):
         import torch
@@ -255,11 +258,12 @@ class _EmState(object):
             setattr(a, name, getattr(self, name).data_ptr())
         a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws.numel()
         self.args = a
-        self.stream = dev.current_stream_ptr(X.device)
 
     def _call(self, name):
+        from .. import _device as dev
         from .. import _lib
-        _lib.check(getattr(_lib.lib, name)(ctypes.byref(self.args), self.stream), name)
+        # the caller's current stream at each step, like every other launcher
+        _lib.check(getattr(_lib.lib, name)(ctypes.byref(self.args), dev.current_stream_ptr(self.X.device)), name)
 
     def estep(self):
         self._call("nnk_gmm_em_estep")
@@ -345,7 +349,9 @@ def _kmeans_plusplus_draws(N, K, random_state):
 
 class _KMeansState(object):
     """Device buffers of one k-means run over the frames ``X`` (csrc/nnk_kmeans.cu) and the filled
-    ``nnk_kmeans_args_t``.  ``centre``: KMeans reads the rows minus their mean, kmeans_plusplus the raw rows."""
+    ``nnk_kmeans_args_t``.  ``centre``: KMeans reads the rows minus their mean, kmeans_plusplus the raw rows.
+    Steps run on the current stream at the time of the call; the buffers belong to the stream current at
+    construction, with the same ordering and lifetime rules as ``_EmState``."""
 
     def __init__(self, X, K, centre):
         import torch
@@ -374,11 +380,12 @@ class _KMeansState(object):
             setattr(a, name, getattr(self, name).data_ptr())
         a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws.numel()
         self.args = a
-        self.stream = dev.current_stream_ptr(X.device)
 
     def _call(self, name):
+        from .. import _device as dev
         from .. import _lib
-        _lib.check(getattr(_lib.lib, name)(ctypes.byref(self.args), self.stream), name)
+        # the caller's current stream at each step, like every other launcher
+        _lib.check(getattr(_lib.lib, name)(ctypes.byref(self.args), dev.current_stream_ptr(self.X.device)), name)
 
     def read_status(self):
         """Synchronises: the small status record of the last call."""

@@ -9,7 +9,9 @@ _basis_cache = {}
 def _basis(device, alpha, D, order, fftlen):
     """float64 basis of (device, alpha, D, order, fftlen), built once on the device (csrc/nnk_postfilter.cu).
 
-    The build is synchronised before the basis enters the cache, so a later call on any stream may read it."""
+    The build is synchronised before the basis enters the cache, so a later call on any stream may read it.
+    The caller reads it on the current stream of ``device``; an eviction never recycles its block before
+    that read has run."""
     import torch
 
     from . import _device as dev
@@ -29,7 +31,7 @@ def _basis(device, alpha, D, order, fftlen):
         if len(_basis_cache) >= 32:
             _basis_cache.clear()
         _basis_cache[key] = b
-    return b
+    return dev.keep_for_current_stream(b, device)
 
 
 def merlin_post_filter(mgc, alpha, minimum_phase_order=511, fftlen=1024, coef=1.4, weight=None):
