@@ -25,11 +25,11 @@
 
 namespace nnk {
 
+// The parameters of all four kernels: the common part, then each path's own fields.
 struct DtwParams {
   const void* X;
   const void* Y;
-  int is_f64;
-  int n_pairs;
+  int is_f64;  // fastdtw_kernel only: the exact kernels take the dtype as a template parameter
   int64_t x_pair_stride, y_pair_stride;
   int x_ld, y_ld, D;
   const int32_t* len_x;
@@ -43,13 +43,69 @@ struct DtwParams {
   double* dist;
   long long* cells;
   int max_tx, max_ty;
-  unsigned char* ws;
-  size_t ws_pair_bytes, series_doubles, bp_bytes;
-  int smem_bp_cap;  // bytes of back-pointer space available in shared memory (fast mode)
-  size_t cost_cap;  // doubles of per-pair cost buffer (fast mode)
-  unsigned long long* prof;  // optional [8] cycle counters (NNK_DTW_PROF=1): build, window, cost, wavefront, backtrack
   double logdb;
+  // FastDTW
+  unsigned char* ws;
+  size_t ws_pair_bytes, series_doubles;
+  int smem_bp_cap;  // bytes of back-pointer space available in shared memory
+  size_t cost_cap;  // doubles of per-pair cost buffer
+  unsigned long long* prof;  // optional [8] cycle counters (NNK_DTW_PROF=1): build, window, cost, wavefront, backtrack
+  // exact, two-pass: the chunk being run
+  int first;             // rank of the chunk's first pair in `order`
+  int n_pairs;           // pairs in this chunk
+  double* cost;          // [chunk][max_tx * max_ty]
+  unsigned char* bp;     // [chunk][max_tx * max_ty]
+  // exact, fused
+  uint32_t* bp_words;    // [pair slot][max_tx][wpr]
+  int wpr;               // back-pointer words per row = ceil(max_ty / 16)
 };
+
+// A pair with an empty series has an empty path.
+__device__ __forceinline__ void store_empty_pair(const DtwParams& p, int pair) {
+  if (threadIdx.x == 0) { p.path_len[pair] = 0; p.dist[pair] = 0.0; if (p.cells) p.cells[pair] = 0; }
+}
+
+// The back-track wrote path_i / path_j[:n] from the last cell back: reverse them in place (all NT threads of
+// the block), then store the length (-1: the path did not fit path_ld) and the cell count.
+template <int NT>
+__device__ __forceinline__ void store_path(const DtwParams& p, int pair, int n, long long cells) {
+  if (n > 0) {
+    int32_t* pi = p.path_i + (size_t)pair * p.path_ld;
+    int32_t* pj = p.path_j + (size_t)pair * p.path_ld;
+    for (int a = threadIdx.x; a < n / 2; a += NT) {
+      const int b = n - 1 - a;
+      const int32_t ti = pi[a], tj = pj[a];
+      pi[a] = pi[b]; pj[a] = pj[b];
+      pi[b] = ti; pj[b] = tj;
+    }
+  }
+  if (threadIdx.x == 0) {
+    p.path_len[pair] = n;
+    if (p.cells) p.cells[pair] = cells;
+  }
+}
+
+// One cell of the recurrence, D[i,j] = first-min(up, left, diagonal), each candidate being that predecessor
+// plus the cell's cost: the fastdtw package's tie order.  `dir` is the 2-bit back-pointer: 0 up, 1 left,
+// 2 diagonal.  Callers add the cost to each predecessor next to its load: adding it here, after all three
+// loads, gives dtw_dp_kernel<16> 107 registers instead of 76 (CUDA 12.9).
+struct Relaxed {
+  double best;
+  uint32_t dir;
+};
+__device__ __forceinline__ Relaxed relax(double up, double left, double diag) {
+  Relaxed r{up, 0};
+  if (left < r.best) { r.best = left; r.dir = 1; }
+  if (diag < r.best) { r.best = diag; r.dir = 2; }
+  return r;
+}
+
+// doubles per staged frame: even, and stride/2 odd, so that LDS.128 is bank-conflict free
+__host__ __device__ __forceinline__ int dtw_row_stride(int D) {
+  int dp = (D + 1) & ~1;
+  if (((dp >> 1) & 1) == 0) dp += 2;
+  return dp;
+}
 
 // numpy DOUBLE_pairwise_sum order over a[k] = (x[k]-y[k])^2 without materialising a[]; the operands
 // are widened to float64 first (fastdtw: np.asanyarray(x, dtype='float')), which is exact
@@ -89,9 +145,32 @@ __device__ double pairwise_sumsq(const T* x, const T* y, int n) {
   return __dadd_rn(pairwise_sumsq(x, y, n2), pairwise_sumsq(x + n2, y + n2, n - n2));
 }
 
-template <typename T>
-__device__ __forceinline__ double local_cost(const T* x, const T* y, int D, int kind, double logdb) {
-  const double r = sqrt(pairwise_sumsq(x, y, D));
+// pairwise_sumsq for a frame of x held in registers, D in [8*NB8, 8*NB8 + 7] (ntail = D - 8*NB8): the
+// eight accumulators over blocks 0..NB8-1, numpy's fold of them, then the tail in order
+template <int NB8>
+__device__ __forceinline__ double sumsq_reg(const double (&xreg)[NB8 * 8 + 8], const double* yr, int ntail) {
+  double r[8];
+#pragma unroll
+  for (int q = 0; q < 8; ++q) { const double z = __dsub_rn(xreg[q], yr[q]); r[q] = __dmul_rn(z, z); }
+#pragma unroll
+  for (int bk = 1; bk < NB8; ++bk) {
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const double z = __dsub_rn(xreg[bk * 8 + q], yr[bk * 8 + q]);
+      r[q] = __dadd_rn(r[q], __dmul_rn(z, z));
+    }
+  }
+  double res = __dadd_rn(__dadd_rn(__dadd_rn(r[0], r[1]), __dadd_rn(r[2], r[3])),
+                         __dadd_rn(__dadd_rn(r[4], r[5]), __dadd_rn(r[6], r[7])));
+#pragma unroll
+  for (int e = 0; e < 7; ++e)
+    if (e < ntail) { const double z = __dsub_rn(xreg[NB8 * 8 + e], yr[NB8 * 8 + e]); res = __dadd_rn(res, __dmul_rn(z, z)); }
+  return res;
+}
+
+// the local cost from the sum of squares: cost_kind 0 = euclid, 1 = melcd
+__device__ __forceinline__ double local_cost(double sumsq, int kind, double logdb) {
+  const double r = sqrt(sumsq);
   return kind == 1 ? __dmul_rn(logdb, r) : r;
 }
 
@@ -115,6 +194,13 @@ __device__ __forceinline__ void cp_async8(void* dst, const void* src) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
 }
 
+// lanes 8m..8m+7 hold r_0..r_7: lane 8m ends with numpy's ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7))
+__device__ __forceinline__ double fold8_lanes(double r) {
+  r = __dadd_rn(r, __shfl_xor_sync(0xffffffffu, r, 1));
+  r = __dadd_rn(r, __shfl_xor_sync(0xffffffffu, r, 2));
+  return __dadd_rn(r, __shfl_xor_sync(0xffffffffu, r, 4));
+}
+
 #define FD_TICK(slot)                                                            \
   do {                                                                           \
     if (p.prof && tid == 0) {                                                    \
@@ -131,10 +217,7 @@ __global__ void __launch_bounds__(FD_BLOCK) fastdtw_kernel(const DtwParams p) {
   const int pair = p.order ? p.order[blockIdx.x] : blockIdx.x;
   const int Tx0 = p.len_x[pair], Ty0 = p.len_y[pair];
   const int D = p.D;
-  if (Tx0 <= 0 || Ty0 <= 0) {
-    if (tid == 0) { p.path_len[pair] = 0; p.dist[pair] = 0.0; if (p.cells) p.cells[pair] = 0; }
-    return;
-  }
+  if (Tx0 <= 0 || Ty0 <= 0) { store_empty_pair(p, pair); return; }
   // ---- shared memory carve-up -------------------------------------------------------------------
   const int mtx = p.max_tx;
   double* cring = reinterpret_cast<double*>(smem);            // [FD_PD + 1][32] prefetched costs
@@ -222,12 +305,11 @@ __global__ void __launch_bounds__(FD_BLOCK) fastdtw_kernel(const DtwParams p) {
       }
     }
     __syncthreads();
-    if (warp == 0) {  // exclusive prefix sum of the row widths (warp scan, 32 rows per step) + widest row
-      int carry = 0, wmax = 0;
+    if (warp == 0) {  // exclusive prefix sum of the row widths (warp scan, 32 rows per step)
+      int carry = 0;
       for (int base = 0; base < Tx; base += 32) {
         const int i = base + lane;
         const int wdt = (i < Tx) ? max(0, hi[i] - lo[i]) : 0;
-        wmax = max(wmax, wdt);
         int incl = wdt;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
@@ -237,9 +319,7 @@ __global__ void __launch_bounds__(FD_BLOCK) fastdtw_kernel(const DtwParams p) {
         if (i < Tx) off[i] = carry + incl - wdt;
         carry += __shfl_sync(0xffffffffu, incl, 31);
       }
-      wmax = __reduce_max_sync(0xffffffffu, wmax);
       if (lane == 0) { off[Tx] = carry; s_cells += carry; s_wmax = 0; }
-      (void)wmax;
     }
     for (int a = tid; a < Tx; a += FD_BLOCK) { if (a < mtx / 2 + 1) { jmn[a] = INT_MAX; jmx[a] = -1; } }
     __syncthreads();
@@ -310,32 +390,25 @@ __global__ void __launch_bounds__(FD_BLOCK) fastdtw_kernel(const DtwParams p) {
 #pragma unroll
             for (int m = 1; m < 4; ++m)
               if (gl + 8 * m < n8) { z = __dsub_rn(xv[u][m], yv[u][m]); r = __dadd_rn(r, __dmul_rn(z, z)); }
-            r = __dadd_rn(r, __shfl_xor_sync(0xffffffffu, r, 1));
-            r = __dadd_rn(r, __shfl_xor_sync(0xffffffffu, r, 2));
-            r = __dadd_rn(r, __shfl_xor_sync(0xffffffffu, r, 4));
+            r = fold8_lanes(r);
             z = __dsub_rn(xt[u], yt[u]);
             const double at = __dmul_rn(z, z);
             for (int e = 0; e < ntail; ++e) r = __dadd_rn(r, __shfl_sync(0xffffffffu, at, e, 8));  // tail, in order
-            const double rt = sqrt(r);
-            if (val[u] && gl == 0) cbuf[cidx[u]] = p.cost_kind == 1 ? __dmul_rn(p.logdb, rt) : rt;
+            if (val[u] && gl == 0) cbuf[cidx[u]] = local_cost(r, p.cost_kind, p.logdb);
           }
         } else {
 #pragma unroll
           for (int u = 0; u < 2; ++u) {
             const double* xr = xl + (size_t)ii[u] * D;
             const double* yr = yl + (size_t)jj[u] * D;
-            double dt;
+            double r;
             if (D >= 8 && D <= 128) {
-              double r = strided8(xr, yr, gl, n8);
-              r = __dadd_rn(r, __shfl_xor_sync(0xffffffffu, r, 1));
-              r = __dadd_rn(r, __shfl_xor_sync(0xffffffffu, r, 2));
-              r = __dadd_rn(r, __shfl_xor_sync(0xffffffffu, r, 4));
+              r = fold8_lanes(strided8(xr, yr, gl, n8));
               for (int e = n8; e < D; ++e) r = __dadd_rn(r, sq(xr, yr, e));
-              const double rt = sqrt(r);
-              dt = p.cost_kind == 1 ? __dmul_rn(p.logdb, rt) : rt;
             } else {
-              dt = local_cost(xr, yr, D, p.cost_kind, p.logdb);
+              r = pairwise_sumsq(xr, yr, D);
             }
+            const double dt = local_cost(r, p.cost_kind, p.logdb);
             if (val[u] && gl == 0) cbuf[cidx[u]] = dt;
           }
         }
@@ -404,16 +477,11 @@ __global__ void __launch_bounds__(FD_BLOCK) fastdtw_kernel(const DtwParams p) {
           const bool vu = i > 0 && j >= p_lo && j < p_hi;
           const bool vl = j - 1 >= r_lo;
           const bool vd = i > 0 && j - 1 >= p_lo && j - 1 < p_hi;
-          const double up = (vu ? upv : CUDART_INF) + dt;
-          const double left = (vl ? D1 : CUDART_INF) + dt;
-          const double diag = ((i == 0 && j == 0) ? 0.0 : (vd ? dgv : CUDART_INF)) + dt;
-          double best = up;
-          unsigned char dir = 0;
-          if (left < best) { best = left; dir = 1; }
-          if (diag < best) { best = diag; dir = 2; }
-          newD = best;
-          bp[(size_t)(r_off + j - r_lo)] = dir;
-          if (i == Tx - 1 && j == Ty - 1) dist_last = best;
+          const Relaxed c = relax((vu ? upv : CUDART_INF) + dt, (vl ? D1 : CUDART_INF) + dt,
+                                  ((i == 0 && j == 0) ? 0.0 : (vd ? dgv : CUDART_INF)) + dt);
+          newD = c.best;
+          bp[(size_t)(r_off + j - r_lo)] = (unsigned char)c.dir;
+          if (i == Tx - 1 && j == Ty - 1) dist_last = c.best;
         }
         D2 = D1;
         D1 = newD;
@@ -434,19 +502,14 @@ __global__ void __launch_bounds__(FD_BLOCK) fastdtw_kernel(const DtwParams p) {
         const double* d2 = Dglob + (size_t)((k + 1) % 3) * mtx;
         for (int i = imin + lane; i <= imax; i += 32) {
           const int j = k - i;
-          const double dt = local_cost(xl + (size_t)i * D, yl + (size_t)j * D, D, p.cost_kind, p.logdb);
+          const double dt = local_cost(pairwise_sumsq(xl + (size_t)i * D, yl + (size_t)j * D, D), p.cost_kind, p.logdb);
           const bool vu = i > 0 && j >= lo[i - 1] && j < hi[i - 1];
           const bool vl = j - 1 >= lo[i];
           const bool vd = i > 0 && j - 1 >= lo[i - 1] && j - 1 < hi[i - 1];
-          const double up = (vu ? d1[i - 1] : CUDART_INF) + dt;
-          const double left = (vl ? d1[i] : CUDART_INF) + dt;
-          const double diag = ((i == 0 && j == 0) ? 0.0 : (vd ? d2[i - 1] : CUDART_INF)) + dt;
-          double best = up;
-          unsigned char dir = 0;
-          if (left < best) { best = left; dir = 1; }
-          if (diag < best) { best = diag; dir = 2; }
-          dk[i] = best;
-          bp[(size_t)(off[i] + j - lo[i])] = dir;
+          const Relaxed c = relax((vu ? d1[i - 1] : CUDART_INF) + dt, (vl ? d1[i] : CUDART_INF) + dt,
+                                  ((i == 0 && j == 0) ? 0.0 : (vd ? d2[i - 1] : CUDART_INF)) + dt);
+          dk[i] = c.best;
+          bp[(size_t)(off[i] + j - lo[i])] = (unsigned char)c.dir;
         }
         __threadfence_block();
         __syncwarp();
@@ -493,22 +556,7 @@ __global__ void __launch_bounds__(FD_BLOCK) fastdtw_kernel(const DtwParams p) {
     __syncthreads();
     FD_TICK(4);
   }
-  // ---- finalise: reverse the level-0 path in place ------------------------------------------------------
-  const int n = s_n;
-  if (n > 0) {
-    int32_t* pi = p.path_i + (size_t)pair * p.path_ld;
-    int32_t* pj = p.path_j + (size_t)pair * p.path_ld;
-    for (int a2 = tid; a2 < n / 2; a2 += FD_BLOCK) {
-      const int b2 = n - 1 - a2;
-      const int32_t ti = pi[a2], tj = pj[a2];
-      pi[a2] = pi[b2]; pj[a2] = pj[b2];
-      pi[b2] = ti; pj[b2] = tj;
-    }
-  }
-  if (tid == 0) {
-    p.path_len[pair] = n;
-    if (p.cells) p.cells[pair] = s_cells;
-  }
+  store_path<FD_BLOCK>(p, pair, s_n, s_cells);
 }
 
 // ---- exact DTW (radius < 0): cost pass + wavefront pass --------------------------------------------
@@ -527,30 +575,6 @@ __device__ __forceinline__ long long diag_off(int k, int Tx, int Ty) {
   return a * (a + 1) / 2 + (b - a) * a + m * a - m * (m + 1) / 2;
 }
 
-struct DtwExactParams {
-  const void* X;
-  const void* Y;
-  int n_pairs;           // pairs in this chunk
-  int first;             // rank of the chunk's first pair in `order`
-  int64_t x_pair_stride, y_pair_stride;
-  int x_ld, y_ld, D;
-  const int32_t* len_x;
-  const int32_t* len_y;
-  const int32_t* order;
-  int cost_kind;
-  int32_t* path_i;
-  int32_t* path_j;
-  int path_ld;
-  int32_t* path_len;
-  double* dist;
-  long long* cells;
-  int max_tx, max_ty;
-  double* cost;          // [chunk][max_tx * max_ty]
-  unsigned char* bp;     // [chunk][max_tx * max_ty]
-  double logdb;
-  int chd;               // 256-cell chunks per diagonal
-};
-
 // Tiled cost pass.  A block owns a TI x TJ tile of cells: the TI frames of x and TJ frames of y are
 // staged ONCE in shared memory as float64 (coalesced loads, one conversion per element instead of
 // one per cell); thread t owns row i0 + t and sweeps the tile along anti-diagonals (lane l of a warp
@@ -559,16 +583,10 @@ struct DtwExactParams {
 // with its eight static accumulators, float64, no FMA contraction.
 constexpr int DTW_TI = 128, DTW_TJ = 64;
 
-__device__ __forceinline__ int dtw_row_stride(int D) {  // doubles; even, and stride/2 odd: LDS.128 conflict-free
-  int dp = (D + 1) & ~1;
-  if (((dp >> 1) & 1) == 0) dp += 2;
-  return dp;
-}
-
 // NB8 = number of 8-element blocks of the pairwise reduction known at compile time (D in
-// [8*NB8, 8*NB8 + 7]); NB8 == 0 selects the generic run-time loops (D < 8 or D > 63).
+// [8*NB8, 8*NB8 + 7]); NB8 == 0 selects pairwise_sumsq's run-time loops (D < 8 or D > 39).
 template <typename T, int NB8>
-__global__ void __launch_bounds__(DTW_TI) dtw_cost_kernel(const DtwExactParams p) {
+__global__ void __launch_bounds__(DTW_TI) dtw_cost_kernel(const DtwParams p) {
   extern __shared__ __align__(16) unsigned char smem_c[];
   const int slot = blockIdx.y;
   const int pair = p.order ? p.order[p.first + slot] : p.first + slot;
@@ -612,49 +630,15 @@ __global__ void __launch_bounds__(DTW_TI) dtw_cost_kernel(const DtwExactParams p
     if (row_ok && jl >= 0 && jl < nj) {
       const double* yr = ys + (size_t)jl * DP;
       double res;
-      if (NB8 > 0) {
-        double r[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) { const double z = __dsub_rn(xreg[q], yr[q]); r[q] = __dmul_rn(z, z); }
-#pragma unroll
-        for (int bk = 1; bk < NB8; ++bk) {
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const double z = __dsub_rn(xreg[bk * 8 + q], yr[bk * 8 + q]);
-            r[q] = __dadd_rn(r[q], __dmul_rn(z, z));
-          }
-        }
-        res = __dadd_rn(__dadd_rn(__dadd_rn(r[0], r[1]), __dadd_rn(r[2], r[3])),
-                        __dadd_rn(__dadd_rn(r[4], r[5]), __dadd_rn(r[6], r[7])));
-#pragma unroll
-        for (int e = 0; e < 7; ++e)
-          if (e < ntail) { const double z = __dsub_rn(xreg[NB8 * 8 + e], yr[NB8 * 8 + e]); res = __dadd_rn(res, __dmul_rn(z, z)); }
-      } else if (D < 8) {
-        res = -0.0;
-        for (int e = 0; e < D; ++e) res = __dadd_rn(res, sq(xr, yr, e));
-      } else if (D <= 128) {
-        double r[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) r[q] = sq(xr, yr, q);
-        const int n8 = D - (D % 8);
-        for (int e = 8; e < n8; e += 8) {
-#pragma unroll
-          for (int q = 0; q < 8; ++q) r[q] = __dadd_rn(r[q], sq(xr, yr, e + q));
-        }
-        res = __dadd_rn(__dadd_rn(__dadd_rn(r[0], r[1]), __dadd_rn(r[2], r[3])),
-                        __dadd_rn(__dadd_rn(r[4], r[5]), __dadd_rn(r[6], r[7])));
-        for (int e = n8; e < D; ++e) res = __dadd_rn(res, sq(xr, yr, e));
-      } else {
-        res = pairwise_sumsq(xr, yr, D);
-      }
-      const double rt = sqrt(res);
-      cost[(size_t)diag_off(k, Tx, Ty) + (i - max(0, k - (Ty - 1)))] = p.cost_kind == 1 ? __dmul_rn(p.logdb, rt) : rt;
+      if constexpr (NB8 > 0) res = sumsq_reg<NB8>(xreg, yr, ntail);
+      else res = pairwise_sumsq(xr, yr, D);
+      cost[(size_t)diag_off(k, Tx, Ty) + (i - max(0, k - (Ty - 1)))] = local_cost(res, p.cost_kind, p.logdb);
     }
   }
 }
 
 template <int MC>
-__global__ void __launch_bounds__(256) dtw_dp_kernel(const DtwExactParams p) {
+__global__ void __launch_bounds__(256) dtw_dp_kernel(const DtwParams p) {
   extern __shared__ __align__(16) unsigned char smem[];
   double* Dbuf = reinterpret_cast<double*>(smem);  // [3][max_tx]
   __shared__ int s_n;
@@ -662,10 +646,7 @@ __global__ void __launch_bounds__(256) dtw_dp_kernel(const DtwExactParams p) {
   const int slot = blockIdx.x;
   const int pair = p.order ? p.order[p.first + slot] : p.first + slot;
   const int Tx = p.len_x[pair], Ty = p.len_y[pair];
-  if (Tx <= 0 || Ty <= 0) {
-    if (tid == 0) { p.path_len[pair] = 0; p.dist[pair] = 0.0; if (p.cells) p.cells[pair] = 0; }
-    return;
-  }
+  if (Tx <= 0 || Ty <= 0) { store_empty_pair(p, pair); return; }
   const int mtx = p.max_tx;
   const double* cost = p.cost + (size_t)slot * ((size_t)p.max_tx * p.max_ty);
   unsigned char* bp = p.bp + (size_t)slot * ((size_t)p.max_tx * p.max_ty);
@@ -699,15 +680,10 @@ __global__ void __launch_bounds__(256) dtw_dp_kernel(const DtwExactParams p) {
       if (i <= imax) {
         const int j = k - i;
         const double dt = ccur[m];
-        const double up = (i > 0 ? d1[i - 1] : CUDART_INF) + dt;
-        const double left = (j > 0 ? d1[i] : CUDART_INF) + dt;
-        const double diag = ((i == 0 && j == 0) ? 0.0 : ((i > 0 && j > 0) ? d2[i - 1] : CUDART_INF)) + dt;
-        double best = up;
-        unsigned char dir = 0;
-        if (left < best) { best = left; dir = 1; }
-        if (diag < best) { best = diag; dir = 2; }
-        dk[i] = best;
-        bp[off + (i - imin)] = dir;
+        const Relaxed c = relax((i > 0 ? d1[i - 1] : CUDART_INF) + dt, (j > 0 ? d1[i] : CUDART_INF) + dt,
+                                ((i == 0 && j == 0) ? 0.0 : ((i > 0 && j > 0) ? d2[i - 1] : CUDART_INF)) + dt);
+        dk[i] = c.best;
+        bp[off + (i - imin)] = (unsigned char)c.dir;
       }
     }
     off += ncur;
@@ -733,21 +709,7 @@ __global__ void __launch_bounds__(256) dtw_dp_kernel(const DtwExactParams p) {
     s_n = ok ? n : -1;
   }
   __syncthreads();
-  const int n = s_n;
-  if (n > 0) {
-    int32_t* pi = p.path_i + (size_t)pair * p.path_ld;
-    int32_t* pj = p.path_j + (size_t)pair * p.path_ld;
-    for (int a = tid; a < n / 2; a += 256) {
-      const int b = n - 1 - a;
-      const int32_t ti = pi[a], tj = pj[a];
-      pi[a] = pi[b]; pj[a] = pj[b];
-      pi[b] = ti; pj[b] = tj;
-    }
-  }
-  if (tid == 0) {
-    p.path_len[pair] = n;
-    if (p.cells) p.cells[pair] = (long long)Tx * Ty;
-  }
+  store_path<256>(p, pair, s_n, (long long)Tx * Ty);
 }
 
 // ---- exact DTW, fused (the production path for frames of 8..39 dims that fit shared memory) -----------------
@@ -780,38 +742,14 @@ constexpr int DTW_POLL = 8;    // steps between progress checks / publications
 constexpr int DTW_TRIP = 2;    // columns per loop trip (cost evaluations in flight per lane)
 static_assert(DTW_POLL % DTW_TRIP == 0, "progress checks fall on trip boundaries");
 
-struct DtwFusedParams {
-  const void* X;
-  const void* Y;
-  int64_t x_pair_stride, y_pair_stride;
-  int x_ld, y_ld, D;
-  const int32_t* len_x;
-  const int32_t* len_y;
-  const int32_t* order;
-  int cost_kind;
-  int32_t* path_i;
-  int32_t* path_j;
-  int path_ld;
-  int32_t* path_len;
-  double* dist;
-  long long* cells;
-  int max_tx, max_ty;
-  uint32_t* bp;  // [pair slot][max_tx][wpr]
-  int wpr;       // back-pointer words per row = ceil(max_ty / 16)
-  double logdb;
-};
-
 template <typename T, int NB8>
-__global__ void __launch_bounds__(DTW_FR, 1) dtw_fused_kernel(const DtwFusedParams p) {
+__global__ void __launch_bounds__(DTW_FR, 1) dtw_fused_kernel(const DtwParams p) {
   extern __shared__ __align__(16) unsigned char smem_f[];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int slot = blockIdx.x;
   const int pair = p.order ? p.order[slot] : slot;
   const int Tx = p.len_x[pair], Ty = p.len_y[pair];
-  if (Tx <= 0 || Ty <= 0) {
-    if (tid == 0) { p.path_len[pair] = 0; p.dist[pair] = 0.0; if (p.cells) p.cells[pair] = 0; }
-    return;
-  }
+  if (Tx <= 0 || Ty <= 0) { store_empty_pair(p, pair); return; }
   const int D = p.D, DP = dtw_row_stride(D);
   const int max_groups = (p.max_tx + 31) / 32;
   double* Ys = reinterpret_cast<double*>(smem_f);              // [max_ty][DP]
@@ -826,7 +764,7 @@ __global__ void __launch_bounds__(DTW_FR, 1) dtw_fused_kernel(const DtwFusedPara
   }
   for (int e = tid; e < 2 * (max_groups + 1); e += DTW_FR) prog[e] = 0;
   __syncthreads();
-  uint32_t* bp = p.bp + (size_t)slot * ((size_t)p.max_tx * p.wpr);
+  uint32_t* bp = p.bp_words + (size_t)slot * ((size_t)p.max_tx * p.wpr);
   const int ntail = D - NB8 * 8;
   const int ngroups = (Tx + 31) / 32;
   const int nsteps = Ty + 31;
@@ -867,25 +805,7 @@ __global__ void __launch_bounds__(DTW_FR, 1) dtw_fused_kernel(const DtwFusedPara
 #pragma unroll
       for (int q = 0; q < DTW_TRIP; ++q) {
         const int jc = min(max(s0 + q - lane, 0), Ty - 1);
-        const double* yr = Ys + (size_t)jc * DP;
-        double r8[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) { const double z = __dsub_rn(xreg[e], yr[e]); r8[e] = __dmul_rn(z, z); }
-#pragma unroll
-        for (int bk = 1; bk < NB8; ++bk) {
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const double z = __dsub_rn(xreg[bk * 8 + e], yr[bk * 8 + e]);
-            r8[e] = __dadd_rn(r8[e], __dmul_rn(z, z));
-          }
-        }
-        double res = __dadd_rn(__dadd_rn(__dadd_rn(r8[0], r8[1]), __dadd_rn(r8[2], r8[3])),
-                               __dadd_rn(__dadd_rn(r8[4], r8[5]), __dadd_rn(r8[6], r8[7])));
-#pragma unroll
-        for (int e = 0; e < 7; ++e)
-          if (e < ntail) { const double z = __dsub_rn(xreg[NB8 * 8 + e], yr[NB8 * 8 + e]); res = __dadd_rn(res, __dmul_rn(z, z)); }
-        const double rt = sqrt(res);
-        cst[q] = p.cost_kind == 1 ? __dmul_rn(p.logdb, rt) : rt;
+        cst[q] = local_cost(sumsq_reg<NB8>(xreg, Ys + (size_t)jc * DP, ntail), p.cost_kind, p.logdb);
       }
       // ---- two relaxation steps ----
 #pragma unroll
@@ -905,18 +825,12 @@ __global__ void __launch_bounds__(DTW_FR, 1) dtw_fused_kernel(const DtwFusedPara
         }
         if (row_ok && j >= 0 && j < Ty) {
           const double dt = cst[q];
-          const double up = u + dt;
-          const double left = myD + dt;     // myD == +inf before the lane's first column
-          const double diag = uprev + dt;
-          double best = up;
-          uint32_t dir = 0;
-          if (left < best) { best = left; dir = 1; }
-          if (diag < best) { best = diag; dir = 2; }
-          myD = best;
-          if (lane == 31 && feeds) bcur[j & (DTW_CW - 1)] = best;
-          bpw |= dir << (2 * (j & 15));
+          const Relaxed c = relax(u + dt, myD + dt, uprev + dt);  // myD == +inf before the lane's first column
+          myD = c.best;
+          if (lane == 31 && feeds) bcur[j & (DTW_CW - 1)] = c.best;
+          bpw |= c.dir << (2 * (j & 15));
           if ((j & 15) == 15 || j == Ty - 1) { bprow[j >> 4] = bpw; bpw = 0; }
-          if (i == Tx - 1 && j == Ty - 1) p.dist[pair] = best;
+          if (i == Tx - 1 && j == Ty - 1) p.dist[pair] = c.best;
         }
         uprev = u;
       }
@@ -953,42 +867,42 @@ __global__ void __launch_bounds__(DTW_FR, 1) dtw_fused_kernel(const DtwFusedPara
     if (lane == 0) s_n = ok ? n : -1;
   }
   __syncthreads();
-  const int n = s_n;
-  if (n > 0) {
-    int32_t* pi = p.path_i + (size_t)pair * p.path_ld;
-    int32_t* pj = p.path_j + (size_t)pair * p.path_ld;
-    for (int a = tid; a < n / 2; a += DTW_FR) {
-      const int b = n - 1 - a;
-      const int32_t ti = pi[a], tj = pj[a];
-      pi[a] = pi[b]; pj[a] = pj[b];
-      pi[b] = ti; pj[b] = tj;
-    }
-  }
-  if (tid == 0) {
-    p.path_len[pair] = n;
-    if (p.cells) p.cells[pair] = (long long)Tx * Ty;
-  }
+  store_path<DTW_FR>(p, pair, s_n, (long long)Tx * Ty);
 }
 
 static size_t dtw_fused_smem(int max_tx, int max_ty, int D) {
-  int dp = (D + 1) & ~1;
-  if (((dp >> 1) & 1) == 0) dp += 2;
   const size_t groups = (size_t)(max_tx + 31) / 32;
-  return sizeof(double) * ((size_t)max_ty * dp + (size_t)DTW_NBR * DTW_CW) + sizeof(int) * 2 * (groups + 1) + 16;
+  return sizeof(double) * ((size_t)max_ty * dtw_row_stride(D) + (size_t)DTW_NBR * DTW_CW) + sizeof(int) * 2 * (groups + 1) + 16;
 }
 // the fused kernel serves frames of 8..39 dimensions whose Y series fits shared memory as float64;
 // max_dyn is the dynamic shared memory a block may request: the opt-in limit less the kernel's static part
 static bool dtw_fused_ok(int max_tx, int max_ty, int D, size_t max_dyn) {
   return D >= 8 && D < 40 && dtw_fused_smem(max_tx, max_ty, D) <= max_dyn;
 }
-template <typename T>
-static const void* dtw_fused_fn(int nb8) {
+// the instances for a dtype and a count of 8-element blocks of the frame (nb8 = D / 8 inside 8..39, else 0)
+static const void* dtw_fused_instance(bool f64, int nb8) {
   switch (nb8) {
-    case 1: return (const void*)dtw_fused_kernel<T, 1>;
-    case 2: return (const void*)dtw_fused_kernel<T, 2>;
-    case 3: return (const void*)dtw_fused_kernel<T, 3>;
-    default: return (const void*)dtw_fused_kernel<T, 4>;
+    case 1: return f64 ? (const void*)dtw_fused_kernel<double, 1> : (const void*)dtw_fused_kernel<float, 1>;
+    case 2: return f64 ? (const void*)dtw_fused_kernel<double, 2> : (const void*)dtw_fused_kernel<float, 2>;
+    case 3: return f64 ? (const void*)dtw_fused_kernel<double, 3> : (const void*)dtw_fused_kernel<float, 3>;
+    default: return f64 ? (const void*)dtw_fused_kernel<double, 4> : (const void*)dtw_fused_kernel<float, 4>;
   }
+}
+static const void* dtw_cost_instance(bool f64, int nb8) {
+  switch (nb8) {
+    case 1: return f64 ? (const void*)dtw_cost_kernel<double, 1> : (const void*)dtw_cost_kernel<float, 1>;
+    case 2: return f64 ? (const void*)dtw_cost_kernel<double, 2> : (const void*)dtw_cost_kernel<float, 2>;
+    case 3: return f64 ? (const void*)dtw_cost_kernel<double, 3> : (const void*)dtw_cost_kernel<float, 3>;
+    case 4: return f64 ? (const void*)dtw_cost_kernel<double, 4> : (const void*)dtw_cost_kernel<float, 4>;
+    default: return f64 ? (const void*)dtw_cost_kernel<double, 0> : (const void*)dtw_cost_kernel<float, 0>;
+  }
+}
+// opts `fn` in to `smem` bytes of dynamic shared memory, then launches it with the parameters `p`
+static cudaError_t dtw_launch(const void* fn, dim3 grid, int block, size_t smem, cudaStream_t st, DtwParams p) {
+  const cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  void* args[] = {&p};
+  return cudaLaunchKernel(fn, grid, dim3(block), args, smem, st);
 }
 // pairs per chunk of the exact mode: 9 bytes per cell (float64 cost + back-pointer), <= ~2 GiB per chunk
 static int dtw_exact_chunk(int n_pairs, int max_tx, int max_ty) {
@@ -1055,8 +969,7 @@ __global__ void trim_len_kernel(const T* __restrict__ X, int64_t pair_stride, in
 
 static size_t dtw_series_doubles(int max_t, int D) { return (size_t)2 * (size_t)max_t * D + 8; }
 
-static size_t dtw_smem_bytes(int max_tx, int D, int bp_cap) {
-  (void)D;
+static size_t dtw_smem_bytes(int max_tx, int bp_cap) {
   size_t b = sizeof(double) * (FD_PD + 1) * 32;
   b += sizeof(int) * ((size_t)max_tx * 2 + (max_tx + 1) + 2 * (max_tx / 2 + 1)) + (size_t)bp_cap;
   return b + 16;
@@ -1104,52 +1017,29 @@ extern "C" int nnk_dtw_align(const nnk_dtw_args_t* a, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const bool full = a->radius < 0;
   const int mt = a->max_tx > a->max_ty ? a->max_tx : a->max_ty;
-  DtwParams p;
-  p.X = a->X; p.Y = a->Y; p.is_f64 = a->dtype == NNK_F64; p.n_pairs = a->n_pairs;
+  DtwParams p{};
+  p.X = a->X; p.Y = a->Y; p.is_f64 = a->dtype == NNK_F64;
   p.x_pair_stride = a->x_pair_stride; p.y_pair_stride = a->y_pair_stride; p.x_ld = a->x_ld; p.y_ld = a->y_ld; p.D = a->D;
   p.len_x = a->len_x; p.len_y = a->len_y; p.order = a->order; p.cost_kind = a->cost_kind; p.radius = a->radius;
   p.path_i = a->path_i; p.path_j = a->path_j; p.path_ld = a->path_ld; p.path_len = a->path_len; p.dist = a->dist;
   p.cells = (long long*)a->cells; p.max_tx = a->max_tx; p.max_ty = a->max_ty;
-  p.ws = (unsigned char*)a->workspace;
-  p.series_doubles = dtw_series_doubles(mt, a->D);
+  p.logdb = 10.0 / log(10.0) * sqrt(2.0);  // metrics/__init__.py:5
   const size_t need = nnk_dtw_workspace_bytes(a->n_pairs, a->max_tx, a->max_ty, a->D, a->radius);
   NNK_REQUIRE(a->workspace_bytes >= need, NNK_ERR_WORKSPACE, "DTW workspace too small");
-  p.ws_pair_bytes = need / (size_t)a->n_pairs;
-  p.bp_bytes = 0;
-  p.logdb = 10.0 / log(10.0) * sqrt(2.0);  // metrics/__init__.py:5
   int dev = 0, max_smem = 0;
   NNK_CUDA_CHECK(cudaGetDevice(&dev));
   NNK_CUDA_CHECK(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  const int nb8 = (a->D >= 8 && a->D < 40) ? a->D / 8 : 0;  // registers hold a frame of up to 39 dims
   size_t fused_dyn = 0;  // dynamic shared memory the fused instance for this D may request
-  if (full && a->D >= 8 && a->D < 40) {
+  if (full && nb8 > 0) {
     cudaFuncAttributes fa;
-    NNK_CUDA_CHECK(cudaFuncGetAttributes(&fa, a->dtype == NNK_F64 ? dtw_fused_fn<double>(a->D / 8) : dtw_fused_fn<float>(a->D / 8)));
+    NNK_CUDA_CHECK(cudaFuncGetAttributes(&fa, dtw_fused_instance(p.is_f64, nb8)));
     fused_dyn = (size_t)max_smem > fa.sharedSizeBytes ? (size_t)max_smem - fa.sharedSizeBytes : 0;
   }
   if (full && dtw_fused_ok(a->max_tx, a->max_ty, a->D, fused_dyn)) {
-    DtwFusedParams f;
-    f.X = a->X; f.Y = a->Y; f.x_pair_stride = a->x_pair_stride; f.y_pair_stride = a->y_pair_stride;
-    f.x_ld = a->x_ld; f.y_ld = a->y_ld; f.D = a->D; f.len_x = a->len_x; f.len_y = a->len_y; f.order = a->order;
-    f.cost_kind = a->cost_kind; f.path_i = a->path_i; f.path_j = a->path_j; f.path_ld = a->path_ld;
-    f.path_len = a->path_len; f.dist = a->dist; f.cells = (long long*)a->cells; f.max_tx = a->max_tx; f.max_ty = a->max_ty;
-    f.bp = reinterpret_cast<uint32_t*>(a->workspace);
-    f.wpr = (a->max_ty + 15) / 16;
-    f.logdb = p.logdb;
-    const size_t fsmem = dtw_fused_smem(a->max_tx, a->max_ty, a->D);
-    const int nb8 = a->D / 8;
-#define NNK_FUSED(TT_, NB_)                                                                                         \
-  do {                                                                                                              \
-    NNK_CUDA_CHECK(cudaFuncSetAttribute(dtw_fused_kernel<TT_, NB_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem)); \
-    dtw_fused_kernel<TT_, NB_><<<a->n_pairs, DTW_FR, fsmem, st>>>(f);                                               \
-  } while (0)
-    if (a->dtype == NNK_F64) {
-      switch (nb8) { case 1: NNK_FUSED(double, 1); break; case 2: NNK_FUSED(double, 2); break; case 3: NNK_FUSED(double, 3); break;
-                     default: NNK_FUSED(double, 4); }
-    } else {
-      switch (nb8) { case 1: NNK_FUSED(float, 1); break; case 2: NNK_FUSED(float, 2); break; case 3: NNK_FUSED(float, 3); break;
-                     default: NNK_FUSED(float, 4); }
-    }
-#undef NNK_FUSED
+    p.bp_words = reinterpret_cast<uint32_t*>(a->workspace);
+    p.wpr = (a->max_ty + 15) / 16;
+    NNK_CUDA_CHECK(dtw_launch(dtw_fused_instance(p.is_f64, nb8), a->n_pairs, DTW_FR, dtw_fused_smem(a->max_tx, a->max_ty, a->D), st, p));
     count_launch();
     NNK_CUDA_CHECK(cudaGetLastError());
     return NNK_OK;
@@ -1159,70 +1049,45 @@ extern "C" int nnk_dtw_align(const nnk_dtw_args_t* a, void* stream) {
     NNK_REQUIRE(smem <= (size_t)max_smem, NNK_ERR_UNSUPPORTED, "sequence too long for the wavefront buffers in shared memory");
     NNK_REQUIRE(a->max_tx <= 256 * 16, NNK_ERR_UNSUPPORTED, "exact DTW supports up to 4096 frames");
     const int mc = (a->max_tx + 255) / 256;
-    NNK_CUDA_CHECK(cudaFuncSetAttribute(dtw_dp_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    NNK_CUDA_CHECK(cudaFuncSetAttribute(dtw_dp_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    NNK_CUDA_CHECK(cudaFuncSetAttribute(dtw_dp_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const void* dp_fn = mc <= 4 ? (const void*)dtw_dp_kernel<4> : mc <= 8 ? (const void*)dtw_dp_kernel<8> : (const void*)dtw_dp_kernel<16>;
+    const size_t csmem = (size_t)(DTW_TI + DTW_TJ) * dtw_row_stride(a->D) * sizeof(double);
+    NNK_REQUIRE(csmem <= (size_t)max_smem, NNK_ERR_UNSUPPORTED, "feature dimension too large for the cost tiles");
+    const int tiles_i = (a->max_tx + DTW_TI - 1) / DTW_TI, tiles_j = (a->max_ty + DTW_TJ - 1) / DTW_TJ;
     const int ch = dtw_exact_chunk(a->n_pairs, a->max_tx, a->max_ty);
     const size_t cells = (size_t)a->max_tx * (size_t)a->max_ty;
-    DtwExactParams q;
-    q.X = a->X; q.Y = a->Y; q.x_pair_stride = a->x_pair_stride; q.y_pair_stride = a->y_pair_stride;
-    q.x_ld = a->x_ld; q.y_ld = a->y_ld; q.D = a->D; q.len_x = a->len_x; q.len_y = a->len_y; q.order = a->order;
-    q.cost_kind = a->cost_kind; q.path_i = a->path_i; q.path_j = a->path_j; q.path_ld = a->path_ld;
-    q.path_len = a->path_len; q.dist = a->dist; q.cells = (long long*)a->cells; q.max_tx = a->max_tx; q.max_ty = a->max_ty;
-    q.cost = reinterpret_cast<double*>(a->workspace);
-    q.bp = reinterpret_cast<unsigned char*>(a->workspace) + (size_t)ch * cells * sizeof(double);
-    q.logdb = p.logdb;
-    q.chd = 0;
+    p.cost = reinterpret_cast<double*>(a->workspace);
+    p.bp = reinterpret_cast<unsigned char*>(a->workspace) + (size_t)ch * cells * sizeof(double);
     for (int first = 0; first < a->n_pairs; first += ch) {
-      q.first = first;
-      q.n_pairs = (a->n_pairs - first < ch) ? a->n_pairs - first : ch;
-      const int tiles_i = (a->max_tx + DTW_TI - 1) / DTW_TI, tiles_j = (a->max_ty + DTW_TJ - 1) / DTW_TJ;
-      dim3 grid((unsigned)(tiles_i * tiles_j), (unsigned)q.n_pairs);
-      int dp = (a->D + 1) & ~1;
-      if (((dp >> 1) & 1) == 0) dp += 2;
-      const size_t csmem = (size_t)(DTW_TI + DTW_TJ) * dp * sizeof(double);
-      NNK_REQUIRE(csmem <= (size_t)max_smem, NNK_ERR_UNSUPPORTED, "feature dimension too large for the cost tiles");
-      const int nb8 = (a->D >= 8 && a->D < 40) ? a->D / 8 : 0;  // registers hold a frame of up to 39 dims
-#define NNK_COST(TT_, NB_)                                                                                              \
-  do {                                                                                                                  \
-    NNK_CUDA_CHECK(cudaFuncSetAttribute(dtw_cost_kernel<TT_, NB_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)csmem)); \
-    dtw_cost_kernel<TT_, NB_><<<grid, DTW_TI, csmem, st>>>(q);                                                          \
-  } while (0)
-      if (a->dtype == NNK_F64) {
-        switch (nb8) { case 1: NNK_COST(double, 1); break; case 2: NNK_COST(double, 2); break; case 3: NNK_COST(double, 3); break;
-                       case 4: NNK_COST(double, 4); break; default: NNK_COST(double, 0); }
-      } else {
-        switch (nb8) { case 1: NNK_COST(float, 1); break; case 2: NNK_COST(float, 2); break; case 3: NNK_COST(float, 3); break;
-                       case 4: NNK_COST(float, 4); break; default: NNK_COST(float, 0); }
-      }
-#undef NNK_COST
-      if (mc <= 4) dtw_dp_kernel<4><<<q.n_pairs, 256, smem, st>>>(q);
-      else if (mc <= 8) dtw_dp_kernel<8><<<q.n_pairs, 256, smem, st>>>(q);
-      else dtw_dp_kernel<16><<<q.n_pairs, 256, smem, st>>>(q);
+      p.first = first;
+      p.n_pairs = (a->n_pairs - first < ch) ? a->n_pairs - first : ch;
+      const dim3 grid((unsigned)(tiles_i * tiles_j), (unsigned)p.n_pairs);
+      NNK_CUDA_CHECK(dtw_launch(dtw_cost_instance(p.is_f64, nb8), grid, DTW_TI, csmem, st, p));
+      NNK_CUDA_CHECK(dtw_launch(dp_fn, p.n_pairs, 256, smem, st, p));
       count_launch(2);
       NNK_CUDA_CHECK(cudaGetLastError());
     }
     return NNK_OK;
   } else {
     size_t bound = dtw_fast_cells_bound(a->max_tx, a->max_ty, a->radius);
-    size_t smem = dtw_smem_bytes(a->max_tx, a->D, (int)bound);
+    size_t smem = dtw_smem_bytes(a->max_tx, (int)bound);
     if (smem > (size_t)max_smem / 4) {  // keep >= 4 CTAs per SM; overflow back-pointers go to global scratch
-      const size_t base = dtw_smem_bytes(a->max_tx, a->D, 0);
+      const size_t base = dtw_smem_bytes(a->max_tx, 0);
       NNK_REQUIRE(base + 1024 <= (size_t)max_smem, NNK_ERR_UNSUPPORTED, "sequence too long for shared memory");
       bound = ((size_t)max_smem / 4 > base + 1024) ? (size_t)max_smem / 4 - base : 1024;
-      smem = dtw_smem_bytes(a->max_tx, a->D, (int)bound);
+      smem = dtw_smem_bytes(a->max_tx, (int)bound);
     }
+    p.ws = (unsigned char*)a->workspace;
+    p.ws_pair_bytes = need / (size_t)a->n_pairs;
+    p.series_doubles = dtw_series_doubles(mt, a->D);
     p.smem_bp_cap = (int)bound;
     p.cost_cap = dtw_fast_cells_bound(a->max_tx, a->max_ty, a->radius);
     static unsigned long long* d_prof = nullptr;
-    p.prof = nullptr;
     if (getenv("NNK_DTW_PROF")) {
       if (!d_prof) NNK_CUDA_CHECK(cudaMalloc(&d_prof, 8 * sizeof(unsigned long long)));
       NNK_CUDA_CHECK(cudaMemsetAsync(d_prof, 0, 8 * sizeof(unsigned long long), st));
       p.prof = d_prof;
     }
-    NNK_CUDA_CHECK(cudaFuncSetAttribute(fastdtw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    fastdtw_kernel<<<a->n_pairs, FD_BLOCK, smem, st>>>(p);
+    NNK_CUDA_CHECK(dtw_launch((const void*)fastdtw_kernel, a->n_pairs, FD_BLOCK, smem, st, p));
     if (p.prof) {  // debug only: synchronises
       unsigned long long h[8];
       NNK_CUDA_CHECK(cudaMemcpyAsync(h, d_prof, sizeof(h), cudaMemcpyDeviceToHost, st));

@@ -104,9 +104,10 @@ def test_exact_fused_limit_in_y(D):
             _check(out, xs, ys, kname, -1)
 
 
-@pytest.mark.parametrize("D", [3, 40, 64])
+@pytest.mark.parametrize("D", [3, 40, 64, 130])
 @pytest.mark.parametrize("dt", [np.float32, np.float64], ids=["f32", "f64"])
 def test_exact_two_pass_outside_the_fused_range(D, dt):
+    """D = 130 takes pairwise_sumsq's split of frames wider than 128 dims."""
     ms = M.max_smem_optin()
     Tx, Ty = 130, 140
     assert not M.dtw_fused_ok(Tx, Ty, D, ms)
@@ -174,12 +175,13 @@ def _fastdtw_case(lx, ly, D, radius, seed):
     return levels, M.fastdtw_caps(Tx, Ty, radius, M.max_smem_optin())
 
 
-@pytest.mark.parametrize("D", [5, 25, 40])
+@pytest.mark.parametrize("D", [5, 25, 40, 130])
 @pytest.mark.parametrize("radius", [3, 10, 30, 60])
 def test_fastdtw_radius(radius, D):
     """Radius 3 keeps every level within FD_MAXW = 24 rows per anti-diagonal (about 2r + 8 rows): the
     lane-per-row wavefront.  Radius 10 and up widens the windows (about 4r + 2 rows) past it: the
-    loop-over-cells wavefront.  D = 25 uses the batched cost loads (8 <= D <= 32), 5 and 40 do not."""
+    loop-over-cells wavefront.  D = 25 uses the batched cost loads (8 <= D <= 32), 5, 40 and 130 do not;
+    130 takes pairwise_sumsq's split of frames wider than 128 dims."""
     levels, (bp_cap, cost_cap) = _fastdtw_case([700, 523, 9], [690, 700, 64], D, radius, 17 * radius + D)
     widest = max(w for lv in levels for _, w in lv)
     if radius == 3:
