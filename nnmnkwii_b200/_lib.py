@@ -230,6 +230,12 @@ SIGNATURES = {
 }
 EXPORTS = list(SIGNATURES)
 
+# the modulation-spectrum kernels (include/nnk_modspec.h), in the same library
+NNK_MS_POWER, NNK_MS_SMOOTH, NNK_MS_INVERSE, NNK_MS_GRAD = 0, 1, 2, 3
+MODSPEC_SIGNATURES = {
+    "nnk_modspec": (ctypes.c_int, [i32, i32, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp, f64, f64, i32, i32, vp]),
+}
+
 
 class NnkError(RuntimeError):
     pass
@@ -244,7 +250,7 @@ def _load():
     L.nnk_abi_version.restype = ctypes.c_int
     if L.nnk_abi_version() != ABI_VERSION:
         raise ImportError("libnnk_b200.so ABI %d != binding ABI %d: rebuild" % (L.nnk_abi_version(), ABI_VERSION))
-    for name, (restype, argtypes) in SIGNATURES.items():
+    for name, (restype, argtypes) in list(SIGNATURES.items()) + list(MODSPEC_SIGNATURES.items()):
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, argtypes
     return L

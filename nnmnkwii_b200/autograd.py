@@ -8,6 +8,11 @@ Differences that are additions, not signature changes:
   * ``UnitVarianceMLPG`` keeps the ``(means, R)`` signature; the dense ``R`` (``T x nw*T``) is
     reduced once to its numerical band and applied as a banded stencil sweep
     (csrc/nnk_uvmlpg.cu) instead of two dense GEMMs that multiply ~95 % zeros.
+
+The modulation-spectrum part (nnmnkwii/autograd/_impl/modspec.py): ``ModSpec`` and ``modspec``, plus the batched
+``ModSpecBatch`` / ``modspec_batch``, on csrc/nnk_modspec.cu.  Like ``preprocessing.modspec`` their names are not
+in ``__all__``, which names the entry points of the buffers-and-streams catalogue; tests/test_modspec_gpu.py runs
+the same checks on them.
 """
 import numpy as np
 import torch
@@ -15,6 +20,8 @@ from torch.autograd import Function
 
 from . import _device as dev
 from . import paramgen as G
+from . import preprocessing as P
+from .preprocessing.modspec import _modspec_grad
 
 
 def _global_variance(variances):
@@ -144,6 +151,57 @@ class UnitVarianceMLPG(Function):
         if dim == 2:
             return grad.view(-1, D), None
         return grad, None
+
+
+class ModSpec(Function):
+    """Modulation spectrum as an autograd function, ``f : (T, D) -> (n // 2 + 1, D)`` (modspec.py:9-60).
+
+    Forward = :func:`nnmnkwii_b200.preprocessing.modspec`.  Backward is the adjoint of the power spectrum,
+    ``dL/dy_t = 2 Re(sum_k dL/dP_k conj(Y_k) e^{-2 pi i k t / n})``, the same kernel in its gradient mode: an
+    inverse FFT per column instead of the reference's dense ``(n // 2 + 1) x T`` cosine and sine tables.  Takes
+    CUDA tensors only and keeps their dtype (the reference takes CPU tensors and returns float32 gradients).
+    """
+
+    @staticmethod
+    def forward(ctx, y, n, norm):
+        assert y.dim() == 2
+        ctx.n, ctx.norm = n, norm
+        ctx.save_for_backward(y)
+        return P.modspec(y.detach(), n=n, norm=norm)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        (y,) = ctx.saved_tensors
+        return _modspec_grad(y, grad_output, ctx.n, ctx.norm), None, None
+
+
+class ModSpecBatch(Function):
+    """Additive: :class:`ModSpec` over a padded ``(B, T, D)`` batch with per-utterance ``lengths``, one kernel
+    launch forward and one backward; ``f : (B, T, D) -> (B, n // 2 + 1, D)``.  Frames past an utterance's length
+    take no part and get a zero gradient."""
+
+    @staticmethod
+    def forward(ctx, y, n, norm, lengths):
+        assert y.dim() == 3
+        ctx.n, ctx.norm = n, norm
+        ctx.lengths = [int(v) for v in (lengths.tolist() if torch.is_tensor(lengths) else lengths)]
+        ctx.save_for_backward(y)
+        return P.modspec(y.detach(), n=n, norm=norm, lengths=ctx.lengths)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        (y,) = ctx.saved_tensors
+        return _modspec_grad(y, grad_output, ctx.n, ctx.norm, ctx.lengths), None, None, None
+
+
+def modspec(y, n=2048, norm=None):
+    """Modulation spectrum of a ``(T, D)`` CUDA tensor, differentiable (modspec.py:63-72)."""
+    return ModSpec.apply(y, n, norm)
+
+
+def modspec_batch(y, lengths, n=2048, norm=None):
+    """Additive: batched :func:`modspec` (see :class:`ModSpecBatch`)."""
+    return ModSpecBatch.apply(y, n, norm, lengths)
 
 
 def mlpg(means, variances, windows):

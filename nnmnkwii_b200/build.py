@@ -15,7 +15,8 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "csrc", "_obj")
 LIB = os.environ.get("NNK_LIB_OUT") or os.path.join(HERE, "libnnk_b200.so")  # NNK_LIB_OUT: A/B builds
 SOURCES = ["nnk_core.cu", "nnk_mlpg.cu", "nnk_host.cu", "nnk_uvmlpg.cu", "nnk_dtw.cu", "nnk_delta.cu", "nnk_metrics.cu", "nnk_shard.cu", "nnk_gmm.cu",
-           "nnk_gmm_em.cu", "nnk_kmeans.cu", "nnk_postfilter.cu", "nnk_stats.cu", "nnk_wave.cu", "nnk_linalg.cu"]
+           "nnk_gmm_em.cu", "nnk_kmeans.cu", "nnk_postfilter.cu", "nnk_stats.cu", "nnk_wave.cu", "nnk_linalg.cu",
+           "nnk_modspec.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
@@ -45,7 +46,8 @@ def build(force=False, verbose=False):
         force = True
     srcs = [s for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
-    headers.append(os.path.join(os.path.dirname(HERE), "include", "nnk_b200.h"))
+    include = os.path.join(os.path.dirname(HERE), "include")
+    headers += [os.path.join(include, f) for f in os.listdir(include) if f.endswith(".h")]
     jobs = []
     objs = []
     for s in srcs:

@@ -1,7 +1,7 @@
 """Pre-processing pieces on the DTW hot path (drop-in for the names the aligners need from
 ``nnmnkwii.preprocessing``), corpus normalisation (``normalize``: meanvar / meanstd / minmax and the
 scale family), F0 interpolation (``f0``), pre-emphasis and mu-law (``waveform``) and the frame-length
-helpers."""
+helpers; the modulation spectrum (``modspec``: modspec / modphase / inv_modspec / modspec_smoothing)."""
 import numpy as np
 
 
@@ -114,6 +114,9 @@ from .normalize import (inv_minmax_scale, inv_scale, meanstd, meanvar, minmax, m
 from .f0 import interp1d  # noqa: E402
 from .waveform import (inv_mulaw, inv_mulaw_quantize, inv_preemphasis, mulaw, mulaw_quantize,  # noqa: E402
                        preemphasis)
+# ``__all__`` names the entry points of the buffers-and-streams catalogue (tests/stream_catalogue.py); the
+# modulation spectrum has the same checks in tests/test_modspec_gpu.py, so its names are imported, not listed
+from .modspec import inv_modspec, modphase, modspec, modspec_smoothing  # noqa: E402,F401
 
 __all__ = ["trim_zeros_frames", "delta_features", "meanvar", "meanstd", "minmax", "scale", "inv_scale",
            "minmax_scale_params", "minmax_scale", "inv_minmax_scale", "remove_zeros_frames", "interp1d",
