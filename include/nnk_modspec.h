@@ -18,6 +18,12 @@
  *                     bins 0 and n / 2 are ignored, as numpy.fft.irfft does.
  *   mode 3 (grad):    in2 = dL/d|Y|^2 (B, K, D); out = dL/dx = 2 fwd_scale Re(sum_k G_k conj(Y_k) e^{-2 pi i k t / n})
  *                     for t < len_b, (B, T_out, D).
+ *   mode 4 (log power): out = log(max(|Y_k|^2, tiny)), (B, K, D), tiny the smallest normal number of the dtype
+ *                     (FLT_MIN, DBL_MIN); out2 must be NULL.  No inverse FFT, like mode 0.
+ *   mode 5 (post-filter): in2 = (a, c) interleaved, (K, D, 2), shared by every utterance.  Bin 0 is kept; a bin
+ *                     k >= 1 of zero power stays 0, any other becomes Y_k / |Y_k| exp(s' / 2) with
+ *                     s' = a s + c, s = log(max(|Y_k|^2, tiny)); then, as mode 1,
+ *                     out = inv_scale * irfft_unnormalised(Y)[:len_b], (B, T_out, D).  out2 must be NULL.
  * Frames len_b <= t < T_out of out are written as 0.  n is 256, 512, 1024, 2048 or 4096 (else NNK_ERR_ARG);
  * every len_b must be <= n and <= T_out (<= T_in for the modes that read x). */
 #ifndef NNK_MODSPEC_H
@@ -33,6 +39,8 @@ extern "C" {
 #define NNK_MS_SMOOTH 1
 #define NNK_MS_INVERSE 2
 #define NNK_MS_GRAD 3
+#define NNK_MS_LOGPOWER 4
+#define NNK_MS_POSTFILTER 5
 
 int nnk_modspec(int32_t mode, int32_t dtype, int32_t n, const void* in, const void* in2, void* out, void* out2,
                 int32_t B, int32_t T_in, int32_t T_out, int32_t D, const int32_t* lengths, double fwd_scale,

@@ -231,7 +231,7 @@ SIGNATURES = {
 EXPORTS = list(SIGNATURES)
 
 # the modulation-spectrum kernels (include/nnk_modspec.h), in the same library
-NNK_MS_POWER, NNK_MS_SMOOTH, NNK_MS_INVERSE, NNK_MS_GRAD = 0, 1, 2, 3
+NNK_MS_POWER, NNK_MS_SMOOTH, NNK_MS_INVERSE, NNK_MS_GRAD, NNK_MS_LOGPOWER, NNK_MS_POSTFILTER = 0, 1, 2, 3, 4, 5
 MODSPEC_SIGNATURES = {
     "nnk_modspec": (ctypes.c_int, [i32, i32, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp, f64, f64, i32, i32, vp]),
 }

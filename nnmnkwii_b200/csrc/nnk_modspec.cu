@@ -10,6 +10,12 @@
 // in place.  A decimation-in-frequency inverse FFT of Z' leaves n irfft(C) in bit-reversed order, read straight
 // into the output frames.  The spectrum never leaves shared memory.  Twiddles W^j, j < M, are one table per CTA
 // (sincospi), which also serves the FFT stages (e^{-2 pi i p / len} = W^{p n / len}).
+//
+// The MS post-filter (postfilters.modspec_post_filter) is two modes of the same kernel: the log power, whose
+// moments over utterances are the filter's statistics, and the filter itself, which rescales each bin's log
+// power in the bin-pair pass and goes back to frames like smoothing.
+#include <cfloat>
+
 #include "nnk_common.cuh"
 #include "../../include/nnk_modspec.h"
 
@@ -40,6 +46,18 @@ template <typename V> __device__ __forceinline__ V unit_phase(V y) {
   return cx<V>(y.x / r, y.y / r);
 }
 
+// s = log(max(p, tiny)), tiny the dtype's smallest normal number: finite for a bin of zero power
+__device__ __forceinline__ float log_power(float p) { return logf(fmaxf(p, FLT_MIN)); }
+__device__ __forceinline__ double log_power(double p) { return log(fmax(p, DBL_MIN)); }
+
+// one post-filtered bin (k >= 1): Y / |Y| exp(s' / 2) with s' = a s + c, ac = (a, c); a bin of zero power stays 0
+template <typename V> __device__ __forceinline__ V postfilter_bin(V y, V ac) {
+  using T = decltype(V::x);
+  const T p = y.x * y.x + y.y * y.y;
+  if (p == T(0)) return cx<V>(0, 0);
+  return scale(unit_phase(y), exp((ac.x * log_power(p) + ac.y) * T(0.5)));
+}
+
 struct MsArgs {
   const void* in;
   const void* in2;
@@ -53,7 +71,10 @@ struct MsArgs {
 
 template <int LOGN> constexpr int ms_threads() { return (1 << (LOGN - 2)) < MS_MAX_THREADS ? (1 << (LOGN - 2)) : MS_MAX_THREADS; }
 
-template <typename T, int LOGN>
+// PF selects the post-filter instance (modes 4 and 5); the other instance runs modes 0 to 3.  Separate instances
+// keep log / exp out of the register allocation of modes 0 to 3: one runtime switch over all six modes gave the
+// float64 instances 64 registers and 24-36 B of spills instead of 72-80 registers and none.
+template <typename T, int LOGN, bool PF>
 __global__ void __launch_bounds__(ms_threads<LOGN>()) modspec_kernel(MsArgs a) {
   using V = typename Cx<T>::V;
   constexpr int N = 1 << LOGN, LOGM = LOGN - 1, M = N / 2, NT = ms_threads<LOGN>();
@@ -63,7 +84,8 @@ __global__ void __launch_bounds__(ms_threads<LOGN>()) modspec_kernel(MsArgs a) {
   V* tw = z + M;
   const int tid = threadIdx.x, d = blockIdx.x, D = a.D;
   const int mode = a.mode;
-  const bool reads_x = mode != NNK_MS_INVERSE, writes_frames = mode != NNK_MS_POWER;
+  const bool reads_x = PF || mode != NNK_MS_INVERSE;
+  const bool writes_frames = PF ? mode == NNK_MS_POSTFILTER : mode != NNK_MS_POWER;
   const T fs = (T)a.fwd_scale;
   for (int j = tid; j < M; j += NT) {  // W^j = e^{-2 pi i j / n}
     T s, c;
@@ -100,7 +122,7 @@ __global__ void __launch_bounds__(ms_threads<LOGN>()) modspec_kernel(MsArgs a) {
     for (int k = tid; k <= M / 2; k += NT) {
       const int j = M - k;
       V Ck, Cj;  // the half spectrum that goes back to frames, at bins k and j
-      if (mode == NNK_MS_INVERSE) {
+      if (!PF && mode == NNK_MS_INVERSE) {
         const T* P = reinterpret_cast<const T*>(a.in) + spec_row;
         const V* Ph = reinterpret_cast<const V*>(a.in2) + spec_row;
         Ck = scale(Ph[(size_t)k * D], sqrt(P[(size_t)k * D]));
@@ -120,18 +142,24 @@ __global__ void __launch_bounds__(ms_threads<LOGN>()) modspec_kernel(MsArgs a) {
           Xj = conj_(csub(E, WO));
         }
         const V Yk = scale(Xk, fs), Yj = scale(Xj, fs);
-        if (mode == NNK_MS_POWER) {
+        if (!writes_frames) {  // power (PF: log power)
           T* P = reinterpret_cast<T*>(a.out) + spec_row;
           V* Ph = reinterpret_cast<V*>(a.out2) + spec_row;
-          P[(size_t)k * D] = Yk.x * Yk.x + Yk.y * Yk.y;
-          if (a.out2) Ph[(size_t)k * D] = unit_phase(Yk);
+          const T pk = Yk.x * Yk.x + Yk.y * Yk.y;
+          P[(size_t)k * D] = PF ? log_power(pk) : pk;
+          if (!PF && a.out2) Ph[(size_t)k * D] = unit_phase(Yk);
           if (j != k) {
-            P[(size_t)j * D] = Yj.x * Yj.x + Yj.y * Yj.y;
-            if (a.out2) Ph[(size_t)j * D] = unit_phase(Yj);
+            const T pj = Yj.x * Yj.x + Yj.y * Yj.y;
+            P[(size_t)j * D] = PF ? log_power(pj) : pj;
+            if (!PF && a.out2) Ph[(size_t)j * D] = unit_phase(Yj);
           }
           continue;
         }
-        if (mode == NNK_MS_SMOOTH) {
+        if (PF) {  // bin 0 keeps the column's level; the (a, c) table is shared by every utterance
+          const V* AC = reinterpret_cast<const V*>(a.in2) + d;
+          Ck = k == 0 ? Yk : postfilter_bin(Yk, AC[(size_t)k * D]);
+          Cj = postfilter_bin(Yj, AC[(size_t)j * D]);
+        } else if (mode == NNK_MS_SMOOTH) {
           Ck = k < a.limit_bin ? Yk : (a.log_domain ? unit_phase(Yk) : cx<V>(0, 0));
           Cj = j < a.limit_bin ? Yj : (a.log_domain ? unit_phase(Yj) : cx<V>(0, 0));
         } else {  // gradient: sum over k of G_k Y_k e^{+i phi k t}, bins 0 and n / 2 counted twice
@@ -151,7 +179,7 @@ __global__ void __launch_bounds__(ms_threads<LOGN>()) modspec_kernel(MsArgs a) {
         if (j != k) z[j] = cadd(conj_(A), times_i(cmul(w, conj_(Bd))));
       }
     }
-    if (mode == NNK_MS_POWER) {
+    if (!writes_frames) {
       __syncthreads();  // z is rewritten by the next utterance
       continue;
     }
@@ -167,7 +195,7 @@ __global__ void __launch_bounds__(ms_threads<LOGN>()) modspec_kernel(MsArgs a) {
       }
       __syncthreads();
     }
-    const T os = (T)(mode == NNK_MS_GRAD ? a.fwd_scale : a.inv_scale);
+    const T os = (T)(!PF && mode == NNK_MS_GRAD ? a.fwd_scale : a.inv_scale);
     T* y = reinterpret_cast<T*>(a.out) + (size_t)b * a.T_out * D + d;
     for (int t = tid; t < a.T_out; t += NT) {
       T v = T(0);
@@ -181,27 +209,28 @@ __global__ void __launch_bounds__(ms_threads<LOGN>()) modspec_kernel(MsArgs a) {
   }
 }
 
-template <typename T, int LOGN>
+template <typename T, int LOGN, bool PF>
 static int launch_modspec(const MsArgs& a, cudaStream_t st) {
   constexpr int M = 1 << (LOGN - 1);
   const size_t smem = 2 * M * sizeof(typename Cx<T>::V);
   if (smem > 48 * 1024)  // per device: cheap enough to set on every launch
-    NNK_CUDA_CHECK(cudaFuncSetAttribute(modspec_kernel<T, LOGN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    NNK_CUDA_CHECK(cudaFuncSetAttribute(modspec_kernel<T, LOGN, PF>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)smem));
   const dim3 grid((unsigned)a.D, (unsigned)(a.B < 65535 ? a.B : 65535));
-  modspec_kernel<T, LOGN><<<grid, ms_threads<LOGN>(), smem, st>>>(a);
+  modspec_kernel<T, LOGN, PF><<<grid, ms_threads<LOGN>(), smem, st>>>(a);
   count_launch();
   NNK_CUDA_CHECK(cudaGetLastError());
   return NNK_OK;
 }
 
-template <typename T>
+template <typename T, bool PF>
 static int dispatch_modspec(int logn, const MsArgs& a, cudaStream_t st) {
   switch (logn) {
-    case 8: return launch_modspec<T, 8>(a, st);
-    case 9: return launch_modspec<T, 9>(a, st);
-    case 10: return launch_modspec<T, 10>(a, st);
-    case 11: return launch_modspec<T, 11>(a, st);
-    default: return launch_modspec<T, 12>(a, st);
+    case 8: return launch_modspec<T, 8, PF>(a, st);
+    case 9: return launch_modspec<T, 9, PF>(a, st);
+    case 10: return launch_modspec<T, 10, PF>(a, st);
+    case 11: return launch_modspec<T, 11, PF>(a, st);
+    default: return launch_modspec<T, 12, PF>(a, st);
   }
 }
 
@@ -212,20 +241,25 @@ using namespace nnk;
 extern "C" int nnk_modspec(int32_t mode, int32_t dtype, int32_t n, const void* in, const void* in2, void* out,
                            void* out2, int32_t B, int32_t T_in, int32_t T_out, int32_t D, const int32_t* lengths,
                            double fwd_scale, double inv_scale, int32_t limit_bin, int32_t log_domain, void* stream) {
-  NNK_REQUIRE(mode >= NNK_MS_POWER && mode <= NNK_MS_GRAD, NNK_ERR_ARG, "bad mode");
+  NNK_REQUIRE(mode >= NNK_MS_POWER && mode <= NNK_MS_POSTFILTER, NNK_ERR_ARG, "bad mode");
   NNK_REQUIRE(dtype == NNK_F32 || dtype == NNK_F64, NNK_ERR_ARG, "bad dtype");
   int logn = 0;
   while (logn < 31 && (1 << logn) < n) ++logn;
   NNK_REQUIRE(n > 0 && (1 << logn) == n && logn >= MS_LOGN_MIN && logn <= MS_LOGN_MAX, NNK_ERR_ARG,
               "n must be 256, 512, 1024, 2048 or 4096");
   NNK_REQUIRE(B >= 0 && T_in >= 0 && T_out >= 0 && D >= 0, NNK_ERR_ARG, "bad size");
-  if (B == 0 || D == 0 || (mode != NNK_MS_POWER && T_out == 0)) return NNK_OK;  // nothing to write
+  const bool spectrum = mode == NNK_MS_POWER || mode == NNK_MS_LOGPOWER;
+  if (B == 0 || D == 0 || (!spectrum && T_out == 0)) return NNK_OK;  // nothing to write
   NNK_REQUIRE(out, NNK_ERR_ARG, "NULL output");
   DeviceGuard guard(out);
   // utterances of no frames are an empty x: nothing is read from it
   NNK_REQUIRE(in || (mode != NNK_MS_INVERSE && T_in == 0), NNK_ERR_ARG, "NULL input");
-  NNK_REQUIRE(in2 || mode == NNK_MS_POWER || mode == NNK_MS_SMOOTH, NNK_ERR_ARG, "NULL second input");
+  NNK_REQUIRE(in2 || mode == NNK_MS_POWER || mode == NNK_MS_SMOOTH || mode == NNK_MS_LOGPOWER, NNK_ERR_ARG,
+              "NULL second input");
+  NNK_REQUIRE(!out2 || mode < NNK_MS_LOGPOWER, NNK_ERR_ARG, "out2 must be NULL for the log power and the post-filter");
   MsArgs a{in, in2, out, out2, B, T_in, T_out, D, lengths, fwd_scale, inv_scale, limit_bin, log_domain, mode};
   cudaStream_t st = (cudaStream_t)stream;
-  return dtype == NNK_F32 ? dispatch_modspec<float>(logn, a, st) : dispatch_modspec<double>(logn, a, st);
+  if (mode >= NNK_MS_LOGPOWER)
+    return dtype == NNK_F32 ? dispatch_modspec<float, true>(logn, a, st) : dispatch_modspec<double, true>(logn, a, st);
+  return dtype == NNK_F32 ? dispatch_modspec<float, false>(logn, a, st) : dispatch_modspec<double, false>(logn, a, st);
 }

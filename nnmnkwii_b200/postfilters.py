@@ -1,6 +1,9 @@
-"""Merlin's mel-cepstral post-filter on the GPU (drop-in for ``nnmnkwii.postfilters``, without pysptk)."""
+"""Post-filters on the GPU: Merlin's mel-cepstral post-filter (drop-in for ``nnmnkwii.postfilters``, without
+pysptk) and the modulation-spectrum post-filter with its statistics (additive)."""
 import numpy as np
 
+# ``__all__`` names the entry points of the buffers-and-streams catalogue (tests/stream_catalogue.py); the
+# modulation-spectrum post-filter has the same checks in tests/test_ms_postfilter_gpu.py, so it is not listed
 __all__ = ["merlin_post_filter"]
 
 _basis_cache = {}
@@ -98,3 +101,178 @@ def merlin_post_filter(mgc, alpha, minimum_phase_order=511, fftlen=1024, coef=1.
                                                  w.data_ptr(), fftlen, basis.data_ptr(), basis.numel(), out.data_ptr(), D,
                                                  dev.current_stream_ptr(device)), "nnk_postfilter_apply")
     return dev.like_input(out, mgc)
+
+
+# ---- modulation-spectrum post-filter (Takamichi et al., ICASSP 2014), utterance level ----------------------------------
+def _ms_input(x, n, lengths):
+    """(B, T, D, host lengths) of a trajectory or padded batch the MS post-filter takes; argument errors only."""
+    from .preprocessing.modspec import _batch, _check_n, _checked
+    _checked(x, "x")
+    _check_n(n)
+    B, T, D, lens, frames = _batch(x, lengths)
+    if frames > n:
+        raise ValueError("DFT length %d is shorter than the %d frames of x" % (n, frames))
+    return B, T, D, lens
+
+
+def modspec_statistics(x, n=4096, lengths=None):
+    """Statistics of the log modulation spectrum over a set of utterances, for :func:`modspec_post_filter`.
+
+    For each utterance and feature column, ``s_j = log(max(|rfft(x[:, d], n)_j|^2, tiny))`` (natural log; ``tiny``
+    is the smallest normal number of ``x``'s dtype and only matters for bins of exactly zero power): the log of
+    ``preprocessing.modspec`` with the default norm.  ``mean[j, d]`` and ``var[j, d]`` are the mean and the
+    population variance of ``s_j`` across the utterances, accumulated in float64 in a fixed order (two passes).
+
+    Runs on the GPU in two launches: the log power of every utterance into a temporary ``(B, n // 2 + 1, D)``
+    array in ``x``'s dtype (``nnk_modspec``, csrc/nnk_modspec.cu), then its moments (``nnk_segment_moments``).  The
+    temporary costs ``B * (n // 2 + 1) * D`` elements: about 250 MB for 512 float32 utterances at ``n = 4096``,
+    ``D = 60``.  The statistics are not accumulated in chunks, so the whole set goes in one call.
+
+    Pass the columns you will filter, typically ``mgc[:, 1:]``: the power coefficient (column 0) is usually left
+    alone.  Compute the natural statistics on natural speech and the generated ones on the model's output for
+    the same kind of utterances, with the same ``n``.
+
+    Args:
+        x: ``(T, D)`` trajectory (one utterance) or a padded ``(B, T, D)`` batch; float32 / float64 CUDA tensor or
+            NumPy array (a CPU tensor is refused).
+        n (int): DFT length, 256, 512, 1024, 2048 or 4096, at least every utterance's length.
+        lengths: with a ``(B, T, D)`` ``x``, frames of each utterance (default: ``T``); frames past a length are
+            never read.
+
+    Returns:
+        ``(mean, var)``, each float64 of shape ``(n // 2 + 1, D)``: NumPy arrays for NumPy ``x``, tensors on
+        ``x``'s device otherwise.
+
+    Raises:
+        ValueError: ``n`` not supported, an utterance longer than ``n``, no utterance, or an utterance of no
+            frames (it has no modulation spectrum), all before any device work.
+    """
+    import torch
+
+    from . import _device as dev
+    from . import _lib
+    from .preprocessing.modspec import _device_input, _launch
+    B, T, D, lens = _ms_input(x, n, lengths)
+    if B == 0:
+        raise ValueError("modspec_statistics needs at least one utterance")
+    if (T if lens is None else int(lens.min())) < 1:
+        raise ValueError("every utterance needs at least one frame (a zero-length utterance has no modulation "
+                         "spectrum)")
+    K = n // 2 + 1
+    xt = _device_input(x, B, T, D)
+    device = xt.device
+    logms = torch.empty((B, K, D), dtype=xt.dtype, device=device)
+    _launch(_lib.NNK_MS_LOGPOWER, n, xt, None, logms, None, B, T, 0, D, lens, 1.0, 0.0)
+    mean = torch.empty((K, D), dtype=torch.float64, device=device)
+    var = torch.empty((K, D), dtype=torch.float64, device=device)
+    if D:  # one segment of B rows and K * D columns
+        off = torch.tensor([0, B], dtype=torch.int64, device=device)
+        _lib.check(_lib.lib.nnk_segment_moments(logms.data_ptr(), dev.torch_dtype_code(logms.dtype), K * D, K * D,
+                                                off.data_ptr(), None, 1, mean.data_ptr(), var.data_ptr(),
+                                                dev.current_stream_ptr(device)), "nnk_segment_moments")
+    return dev.like_input(mean, x), dev.like_input(var, x)
+
+
+def _ms_stats(pairs, K, D):
+    """float64 host ``(mean, var)`` of each named statistics pair, checked: shape ``(K, D)``, finite means,
+    finite non-negative variances.  Shapes and types of every pair are checked before any value is read."""
+    from . import _device as dev
+    from .preprocessing.modspec import _checked
+    for name, pair in pairs:
+        if not isinstance(pair, (tuple, list)) or len(pair) != 2:
+            raise TypeError("%s must be a (mean, var) pair" % name)
+        for a, what in zip(pair, ("mean", "var")):
+            _checked(a, "%s %s" % (name, what))
+            if tuple(a.shape) != (K, D):
+                raise ValueError("%s %s is %s, expected (n // 2 + 1, D) = %s: statistics of another n or D?"
+                                 % (name, what, tuple(a.shape), (K, D)))
+    out = []
+    for name, pair in pairs:
+        m, v = (np.asarray(a.detach().cpu().numpy() if dev.is_tensor(a) else a, dtype=np.float64) for a in pair)
+        if not np.isfinite(m).all():
+            raise ValueError("%s mean is not finite" % name)
+        if not np.isfinite(v).all() or (v < 0).any():
+            raise ValueError("%s var must be finite and >= 0" % name)
+        out.append((m, v))
+    return out
+
+
+def _ms_table(natural, generated, k, K, D, dtype):
+    """The filter's ``(K, D, 2)`` table ``(a, c)``, ``s' = a s + c``, computed in float64 and stored in ``dtype``."""
+    (mu_n, v_n), (mu_g, v_g) = _ms_stats([("natural", natural), ("generated", generated)], K, D)
+    g = np.sqrt(np.divide(v_n, v_g, out=np.ones_like(v_n), where=v_g > 0))
+    return np.stack([(1.0 - k) + k * g, k * (mu_n - g * mu_g)], axis=-1).astype(dtype)
+
+
+def modspec_post_filter(x, natural, generated, k=1.0, n=4096, lengths=None):
+    """Modulation-spectrum (MS) post-filter of Takamichi et al., "A postfilter to modify the modulation spectrum
+    in HMM-based speech synthesis", ICASSP 2014, at the utterance level, on the GPU.
+
+    Generated trajectories are over-smoothed: their MS is too low at the higher modulation frequencies.  The
+    filter moves each utterance's log MS towards the statistics of natural speech.  For one utterance of
+    ``T <= n`` frames and one column, with ``Y = rfft(x[:, d], n)`` and ``s_j = log(max(|Y_j|^2, tiny))`` as in
+    :func:`modspec_statistics`, every bin ``j >= 1`` of non-zero power becomes (statistics taken at bin ``j``,
+    column ``d``; ``k`` is the emphasis weight)::
+
+        g   = sqrt(v_N / v_G)                    (1 where v_G == 0)
+        s'  = (1 - k) s_j + k (g (s_j - mu_G) + mu_N)
+        C_j = Y_j / |Y_j| exp(s' / 2)
+
+    and the result is ``irfft(C, n)[:T]``.  ``k = 0``, or equal natural and generated statistics, gives ``x``
+    back to rounding.
+
+    Deliberate choices:
+      * utterance level only: the filter sees each utterance's whole MS; the segment-level variant of the paper
+        is not offered;
+      * bin 0 is not filtered (``C_0 = Y_0``): it is ``T`` times the column's mean, which the acoustic model sets,
+        not modulation, so each column keeps its level.  A bin of zero power stays 0, so an all-zero column comes
+        out all zero;
+      * there is no ``norm`` argument: with one norm for the statistics and the filter, a norm shifts ``s``,
+        ``mu_N`` and ``mu_G`` by the same constant and leaves the result unchanged;
+      * ``k`` outside ``[0, 1]``, non-finite means and negative or non-finite variances raise ``ValueError``.
+
+    Each utterance and column is filtered on its own; frames past an utterance's length are written as 0, and a
+    zero-length utterance comes back as zeros.  Runs on the GPU (``nnk_modspec``, csrc/nnk_modspec.cu): one CTA
+    per (utterance, column) does the forward FFT, the per-bin filter and the inverse FFT in shared memory.  The
+    per-bin gain ``s' = a s + c`` is tabulated on the host in float64 from the statistics
+    (``a = (1 - k) + k g``, ``c = k (mu_N - g mu_G)``); statistics given as CUDA tensors are copied to the host
+    for that, which waits for the current stream.
+
+    Pass the columns the statistics were computed on, typically ``mgc[:, 1:]`` (leave the power coefficient
+    alone).
+
+    Args:
+        x: ``(T, D)`` trajectory or a padded ``(B, T, D)`` batch; float32 / float64 CUDA tensor or NumPy array (a
+            CPU tensor is refused).
+        natural: ``(mean, var)`` of natural speech from :func:`modspec_statistics`, each ``(n // 2 + 1, D)``,
+            NumPy arrays or CUDA tensors.
+        generated: ``(mean, var)`` of generated speech, likewise.
+        k (float): emphasis weight in ``[0, 1]``; 1 replaces the MS statistics completely.
+        n (int): DFT length, 256, 512, 1024, 2048 or 4096, at least every utterance's length; the ``n`` of the
+            statistics.
+        lengths: with a ``(B, T, D)`` ``x``, frames of each utterance (default: ``T``).
+
+    Returns:
+        The filtered trajectories: ``x``'s shape and dtype, NumPy for NumPy ``x``, a tensor on ``x``'s device
+        otherwise.
+
+    Raises:
+        ValueError: for any of the range checks above, an ``n`` not supported, an utterance longer than ``n``, or
+            statistics of the wrong shape; TypeError for inputs that are not float arrays.  Argument errors are
+            raised before any device work.
+    """
+    import torch
+
+    from . import _device as dev
+    from . import _lib
+    from .preprocessing.modspec import _device_input, _launch, _out
+    B, T, D, lens = _ms_input(x, n, lengths)
+    k = float(k)
+    if not 0.0 <= k <= 1.0:
+        raise ValueError("k must be in [0, 1], got %r" % k)
+    table = _ms_table(natural, generated, k, n // 2 + 1, D, dev.np_dtype(x))
+    xt = _device_input(x, B, T, D)
+    out = torch.empty_like(xt)
+    _launch(_lib.NNK_MS_POSTFILTER, n, xt, dev.to_device(table, xt.device), out, None, B, T, T, D, lens, 1.0,
+            1.0 / n)
+    return _out(out, x, x.ndim == 2)
