@@ -236,6 +236,37 @@ MODSPEC_SIGNATURES = {
     "nnk_modspec": (ctypes.c_int, [i32, i32, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp, f64, f64, i32, i32, vp]),
 }
 
+# the trajectory EM of GMM voice conversion (include/nnk_gmm_traj.h), in the same library
+NNK_GMM_TRAJ_EM, NNK_GMM_TRAJ_OBJECTIVE, NNK_GMM_TRAJ_TILE = 0, 1, 32
+
+
+class NnkGmmTrajArgs(ctypes.Structure):
+    _fields_ = [
+        ("x", ctypes.c_void_p),
+        ("x_ld", ctypes.c_int64),
+        ("lp", ctypes.c_void_p),
+        ("c", ctypes.c_void_p),
+        ("c_ld", ctypes.c_int64),
+        ("T", ctypes.c_int32),
+        ("n_utt", ctypes.c_int32),
+        ("utt_off", ctypes.c_void_p),
+        ("tile_off", ctypes.c_void_p),
+        ("n_tiles", ctypes.c_int32),
+        ("static_dim", ctypes.c_int32),
+        ("win", NnkWindows),
+        ("mode", ctypes.c_int32),
+        ("inv_Dm", ctypes.c_void_p),
+        ("log_norm", ctypes.c_void_p),
+        ("E_bar", ctypes.c_void_p),
+        ("V", ctypes.c_void_p),
+        ("ll_part", ctypes.c_void_p),
+    ]
+
+
+GMM_TRAJ_SIGNATURES = {
+    "nnk_gmm_traj_em": (ctypes.c_int, [P(NnkGmm), P(NnkGmmTrajArgs), vp]),
+}
+
 
 class NnkError(RuntimeError):
     pass
@@ -250,7 +281,8 @@ def _load():
     L.nnk_abi_version.restype = ctypes.c_int
     if L.nnk_abi_version() != ABI_VERSION:
         raise ImportError("libnnk_b200.so ABI %d != binding ABI %d: rebuild" % (L.nnk_abi_version(), ABI_VERSION))
-    for name, (restype, argtypes) in list(SIGNATURES.items()) + list(MODSPEC_SIGNATURES.items()):
+    for name, (restype, argtypes) in (list(SIGNATURES.items()) + list(MODSPEC_SIGNATURES.items())
+                                  + list(GMM_TRAJ_SIGNATURES.items())):
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, argtypes
     return L

@@ -16,6 +16,7 @@ float64 kernels of csrc/nnk_gmm.cu (C ABI ``nnk_gmm_logprob`` / ``nnk_gmm_map``)
 dim) temporaries, ``E`` and ``D`` are written directly in the layout the MLPG kernels read.
 """
 import ctypes
+import math
 
 import numpy as np
 from scipy import linalg
@@ -81,9 +82,7 @@ class MLPGBase(object):
         A = np.stack([np.linalg.solve(self.covarXX[m].T, self.covarYX[m].T).T for m in range(self.num_mixtures)])
         dim = self.src_means.shape[1]
         log_det = np.sum(np.log(np.diagonal(self._prec_chol, axis1=1, axis2=2)), axis=1)
-        # Eq. (23) with diagonal covariances (gmm.py:239-244)
-        Dm = np.stack([np.diag(self.covarYY[m]) - np.diag(self.covarYX[m]) / np.diag(self.covarXX[m]) * np.diag(self.covarXY[m])
-                       for m in range(self.num_mixtures)])
+        Dm = self._diag_variances()
         from .. import _lib
         tabs = {
             "src_means": t(self.src_means), "tgt_means": t(self.tgt_means), "prec_chol": t(self._prec_chol),
@@ -96,6 +95,11 @@ class MLPGBase(object):
         g.M, g.D = self.num_mixtures, dim
         self._dev = {"device": device, "tabs": tabs, "gmm": g}
         return self._dev
+
+    def _diag_variances(self):
+        """Eq. (23) with diagonal covariances (gmm.py:239-244), (M, D)."""
+        return np.stack([np.diag(self.covarYY[m]) - np.diag(self.covarYX[m]) / np.diag(self.covarXX[m]) * np.diag(self.covarXY[m])
+                         for m in range(self.num_mixtures)])
 
     def _to_device(self, src):
         import torch
@@ -115,14 +119,16 @@ class MLPGBase(object):
                                             dev.current_stream_ptr(x.device)), "nnk_gmm_logprob")
         return lp
 
-    def _map(self, x, c, mode, want_var=False):
-        """mode 0: (E, D, mix) of the arg-max mixture sequence (Eq. 37, 22, 23); mode 1: posterior mean (Eq. 13)."""
+    def _map(self, x, c, mode, want_var=False, lp=None):
+        """mode 0: (E, D, mix) of the arg-max mixture sequence (Eq. 37, 22, 23); mode 1: posterior mean (Eq. 13).
+        ``lp``: the ``_weighted_log_prob`` of ``x`` if the caller already has it."""
         import torch
 
         from .. import _device as dev
         from .. import _lib
         T, D = x.shape
-        lp = self._weighted_log_prob(x, c)
+        if lp is None:
+            lp = self._weighted_log_prob(x, c)
         E = torch.empty((T, D), dtype=torch.float64, device=x.device)
         Dv = torch.empty((T, D), dtype=torch.float64, device=x.device) if want_var else None
         _lib.check(_lib.lib.nnk_gmm_map(ctypes.byref(c["gmm"]), x.data_ptr(), x.stride(0), T, lp.data_ptr(), mode, E.data_ptr(),
@@ -218,6 +224,142 @@ class MLPG(MLPGBase):
         del torch
         off = np.concatenate([[0], np.cumsum(lens)])
         return [y[off[i]:off[i + 1]] for i in range(len(lens))]
+
+    def transform_em(self, src, n_iter=5, return_log_likelihood=False):
+        """Additive: source features ``(T, D)`` -> converted static features ``(T, static_dim)`` float64, by
+        maximum-likelihood conversion over all mixture sequences (Toda, Black & Tokuda 2007, Sec. III).
+
+        The trajectory ``c`` maximises ``L(c) = sum_t log sum_m exp(lp[t, m] + log N(Y_t; E_{m,t}, diag D_m))``
+        with ``Y = W c`` its static + dynamic sequence (windows never cross the utterance), ``E_{m,t}`` the
+        Eq. 22 mean, ``D_m`` the diagonal Eq. 23 variances :meth:`transform` uses and
+        ``lp[t, m] = log w_m + log N(x_t; mu_m, Sigma_xx,m)``.  EM from ``c_0 = transform(src)``: the E-step
+        gives the mixture posteriors ``gamma[t, m]`` of the current trajectory, the M-step is one MLPG solve with
+        precisions ``P_t = sum_m gamma[t, m] / D_m`` and means ``(sum_m gamma[t, m] E_{m,t} / D_m) / P_t``, so
+        ``L`` never decreases.  This is an exact EM for the diagonal-``D_m`` model of :meth:`transform`; the
+        paper's posterior uses the full conditional covariance instead.  E-step, M-step and the objective run
+        on the GPU in float64 with one host synchronisation, when the result comes back.
+
+        Args:
+            src: ``(T, D)`` source features with static and dynamic columns.
+            n_iter (int): EM iterations; 0 returns exactly what :meth:`transform` returns.
+            return_log_likelihood (bool): also return ``L`` at ``c_0 .. c_{n_iter}``, ``(n_iter + 1,)`` float64.
+
+        Raises ``ValueError`` when ``gv`` is set, when ``src`` has ``static_dim`` columns (the posterior-mean
+        path runs no MLPG), for ``n_iter < 0`` or a ``D_m`` entry that is not positive and finite, and
+        ``NotImplementedError`` for ``D > 96``; all before anything is launched."""
+        out = self.transform_em_batch([src], n_iter=n_iter, return_log_likelihood=return_log_likelihood)
+        if return_log_likelihood:
+            return out[0][0], out[1][0]
+        return out[0]
+
+    def transform_em_batch(self, srcs, n_iter=5, return_log_likelihood=False):
+        """Additive: :meth:`transform_em` of a list of utterances in one flat batch on the device (one E-step
+        launch and one batched MLPG solve per iteration for all of them).  Returns the list of
+        ``(T_i, static_dim)`` arrays, and with ``return_log_likelihood`` also an ``(n_utt, n_iter + 1)`` array."""
+        import torch
+
+        from .. import _device as dev
+        from .. import _lib
+        from ..paramgen import StreamLayout, _utterance_table
+        srcs = [np.asarray(s) for s in srcs]
+        n_iter = self._check_em(srcs, n_iter)
+        lens = [len(s) for s in srcs]
+        nw, S = len(self.windows), self.static_dim
+        if not lens or not sum(lens):
+            ys = [np.zeros((n, S)) for n in lens]
+            return (ys, np.zeros((len(lens), n_iter + 1))) if return_log_likelihood else ys
+        x, c = self._to_device(np.concatenate(srcs, axis=0))
+        T, D = x.shape
+        device = x.device
+        em = self._em_constants(c)
+
+        def up(a):  # asynchronous upload: nothing below waits for the device until the results come back
+            return torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(device, non_blocking=True)
+        off, ulens, order, max_T, n_utt = _utterance_table(lens, None, T)
+        layout = StreamLayout.single(D, nw)
+        win = _lib.make_windows(self.windows)
+        offsets, order_d, chains = up(off), up(order), dev.chains_on_device(layout.chains, device)
+        status = torch.zeros(1, dtype=torch.int64, device=device)
+        tiles = -(-ulens // _lib.NNK_GMM_TRAJ_TILE)
+        tile_off = np.concatenate([[0], np.cumsum(tiles)]).astype(np.int32)
+        tables = up(np.concatenate([off.astype(np.int32), tile_off]))
+        n_tiles = int(tile_off[-1])
+
+        def solve(E, V):  # the kernels and arguments of mlpg_batch(E, V, windows, lengths=lens)
+            y = torch.zeros((T, S), dtype=torch.float64, device=device)
+            dev.run_mlpg("fwd", means=E, variances=V, rhs=None, out=y, offsets=offsets, lengths=None, order=order_d,
+                         chains=chains, n_chain=layout.n_chain, max_T=max_T, windows_c=win, in_ld=D, var_ld=D,
+                         go_ld=0, out_ld=S, dtype_code=_lib.NNK_F64, go_f64=0, n_utt=n_utt, device=device,
+                         check=False, status=status)
+            return y
+
+        lp = self._weighted_log_prob(x, c)
+        E, V = self._map(x, c, 0, want_var=True, lp=lp)
+        y = solve(E, V)
+        ll = torch.zeros((n_iter + 1, max(n_tiles, 1)), dtype=torch.float64, device=device)
+        a = _lib.NnkGmmTrajArgs()
+        a.x, a.x_ld, a.lp, a.T, a.n_utt = x.data_ptr(), x.stride(0), lp.data_ptr(), T, n_utt
+        a.utt_off, a.tile_off, a.n_tiles = tables.data_ptr(), tables.data_ptr() + 4 * (n_utt + 1), n_tiles
+        a.static_dim, a.win = S, win
+        a.inv_Dm, a.log_norm = em["inv_Dm"].data_ptr(), em["log_norm"].data_ptr()
+        E_bar = torch.empty((T, D), dtype=torch.float64, device=device)
+        V_bar = torch.empty((T, D), dtype=torch.float64, device=device)
+        a.E_bar, a.V = E_bar.data_ptr(), V_bar.data_ptr()
+        for k in range(n_iter + (1 if return_log_likelihood else 0)):
+            a.c, a.c_ld = y.data_ptr(), y.stride(0)
+            a.mode = _lib.NNK_GMM_TRAJ_EM if k < n_iter else _lib.NNK_GMM_TRAJ_OBJECTIVE
+            a.ll_part = ll[k].data_ptr() if return_log_likelihood else None
+            _lib.check(_lib.lib.nnk_gmm_traj_em(ctypes.byref(c["gmm"]), ctypes.byref(a), dev.current_stream_ptr(device)),
+                       "nnk_gmm_traj_em")
+            if k < n_iter:
+                y = solve(E_bar, V_bar)
+        dev.raise_if_failed(status)
+        y = y.cpu().numpy()
+        bounds = np.concatenate([[0], np.cumsum(lens)])
+        ys = [y[bounds[i]:bounds[i + 1]] for i in range(len(lens))]
+        if not return_log_likelihood:
+            return ys
+        parts = ll.cpu().numpy()
+        L = np.array([[math.fsum(parts[k, tile_off[u]:tile_off[u + 1]]) for k in range(n_iter + 1)]
+                      for u in range(n_utt)])
+        return ys, L
+
+    def _check_em(self, srcs, n_iter):
+        """The arguments :meth:`transform_em_batch` refuses, before anything is launched; returns ``n_iter``."""
+        if self.gv is not None:
+            raise ValueError("transform_em does not combine EM with global variance (gv is set)")
+        D = self.src_means.shape[1]
+        for s in srcs:
+            if s.ndim != 2:
+                raise ValueError("transform_em expects (T, D) utterances (got shape %s)" % (s.shape,))
+            if s.shape[1] == self.static_dim:
+                raise ValueError("transform_em needs static and dynamic source features: the posterior-mean path "
+                                 "(%d columns) runs no MLPG" % s.shape[1])
+            if s.shape[1] != D:
+                raise ValueError("source features have %d columns, the GMM %d" % (s.shape[1], D))
+        if isinstance(n_iter, (bool, np.bool_)) or int(n_iter) != n_iter or n_iter < 0:
+            raise ValueError("n_iter must be a non-negative integer (got %r)" % (n_iter,))
+        Dm = self._diag_variances()
+        if not np.all(np.isfinite(Dm) & (Dm > 0)):
+            raise ValueError("transform_em needs positive, finite Eq. (23) variances D_m")
+        if D > 96:
+            raise NotImplementedError("feature dimension > 96 is not supported by the GMM kernels")
+        return int(n_iter)
+
+    def _em_constants(self, c):
+        """1 / D_m and -1/2 (sum_d log D_m,d + n log 2 pi) over all n = D columns and over the static ones (the
+        columns an utterance's edge frames keep, see include/nnk_gmm_traj.h) on the device, cached with the
+        other tables."""
+        if "em" not in c:
+            import torch
+            Dm = self._diag_variances()
+            inv = np.ascontiguousarray(1.0 / Dm)
+            S = self.static_dim
+            log_norm = -0.5 * np.stack([np.sum(np.log(Dm), axis=1) + Dm.shape[1] * np.log(2.0 * np.pi),
+                                        np.sum(np.log(Dm[:, :S]), axis=1) + S * np.log(2.0 * np.pi)], axis=1)
+            c["em"] = {k: torch.from_numpy(np.ascontiguousarray(v, dtype=np.float64)).to(c["device"])
+                       for k, v in (("inv_Dm", inv), ("log_norm", log_norm))}
+        return c["em"]
 
 
 _EM_MAX_FEATURES = 128

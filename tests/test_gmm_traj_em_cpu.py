@@ -1,0 +1,132 @@
+"""Without a GPU: the float64 restatement of the trajectory EM (oracle/gmm_traj_em.py) never lowers its
+objective and starts from the reference's MLPG.transform; the binding of include/nnk_gmm_traj.h matches the
+header; the C entry point refuses bad arguments before touching the device."""
+import ctypes
+import importlib.util
+import os
+import re
+
+import numpy as np
+import pytest
+
+from conftest import ROOT
+
+import oracle.gmm_traj_em as OT
+
+_spec = importlib.util.spec_from_file_location("make_gmm_traj_golden",
+                                               os.path.join(ROOT, "tests", "golden", "make_gmm_traj_golden.py"))
+MG = importlib.util.module_from_spec(_spec)
+_spec.loader.exec_module(MG)
+
+
+@pytest.mark.parametrize("swap,diff", [(False, False), (True, False), (False, True), (True, True)])
+@pytest.mark.parametrize("S,nw,M", [(2, 2, 4), (3, 3, 3)])
+def test_oracle_objective_never_decreases(S, nw, M, swap, diff):
+    rng = np.random.default_rng(7 * S + nw + M)
+    g = MG.joint_gmm(rng, M, S * nw)
+    src = rng.standard_normal((40, S * nw))
+    _, L = OT.transform_em(g, MG.WINDOWS[:nw], src, 20, swap=swap, diff=diff)
+    assert L.shape == (21,) and np.all(np.isfinite(L))
+    assert np.all(np.diff(L) >= -1e-12 * np.abs(L[:-1]))
+    assert L[-1] > L[0]
+
+
+def test_oracle_starts_from_the_reference_transform():
+    golden = np.load(os.path.join(ROOT, "tests", "golden", "gmm_traj_reference_golden.npz"))
+    import types
+    for i, (T, S, nw, M, swap, diff) in enumerate(MG.cases()):
+        g = types.SimpleNamespace(weights_=golden["weights_%d" % i], means_=golden["means_%d" % i],
+                                  covariances_=golden["covariances_%d" % i], covariance_type="full")
+        c, L = OT.transform_em(g, MG.WINDOWS[:nw], golden["src_%d" % i], 0, swap=swap, diff=diff)
+        want = golden["y_%d" % i]
+        assert c.shape == want.shape == (T, S) and L.shape == (1,)
+        assert np.abs(c - want).max() <= 1e-10 * np.abs(want).max(), i
+
+
+def _kind(c_type):
+    c_type = c_type.strip()
+    if "*" in c_type:
+        return "ptr"
+    return {"int": "i4", "int32_t": "i4"}[c_type]
+
+
+def _ctypes_kind(t):
+    if issubclass(t, (ctypes._Pointer, ctypes.c_void_p)):
+        return "ptr"
+    return "i%d" % ctypes.sizeof(t)
+
+
+def _header():
+    return open(os.path.join(ROOT, "include", "nnk_gmm_traj.h")).read()
+
+
+def test_binding_matches_header():
+    """Every nnk_gmm_traj.h prototype is bound with the header's arity and argument kinds, takes the stream
+    last and is exported by the library; the struct's fields and the constants agree."""
+    from nnmnkwii_b200 import _lib
+    h = _header()
+    body = re.sub(r"/\*.*?\*/|//[^\n]*", "", h, flags=re.S)
+    protos = re.findall(r"([A-Za-z_][\w ]*\**)\s*\b(nnk_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", body)
+    assert sorted(name for _, name, _ in protos) == sorted(_lib.GMM_TRAJ_SIGNATURES)
+    L = ctypes.CDLL(_lib.LIB_PATH)
+    for ret, name, params in protos:
+        restype, argtypes = _lib.GMM_TRAJ_SIGNATURES[name]
+        assert _kind(ret) == _ctypes_kind(restype), name
+        assert [_ctypes_kind(t) for t in argtypes] == [_kind(p.rsplit(None, 1)[0]) for p in params.split(",")], name
+        assert argtypes[-1] is ctypes.c_void_p and params.split(",")[-1].split()[-1] == "stream", name
+        assert hasattr(L, name)
+        assert name not in _lib.SIGNATURES
+    fields = re.search(r"typedef struct nnk_gmm_traj_args \{(.*?)\} nnk_gmm_traj_args_t;", body, re.S).group(1)
+    names = [re.findall(r"[A-Za-z_]\w*", d)[-1] for d in fields.split(";") if d.strip()]
+    assert names == [f[0] for f in _lib.NnkGmmTrajArgs._fields_]
+    for c in ("EM", "OBJECTIVE", "TILE"):
+        assert int(re.search(r"#define NNK_GMM_TRAJ_%s (\d+)" % c, h).group(1)) == getattr(_lib, "NNK_GMM_TRAJ_" + c)
+
+
+def _valid_args(_lib):
+    """A filled argument block with distinct non-NULL dummy pointers; nothing behind them is ever read."""
+    g = _lib.NnkGmm()
+    g.src_means = g.tgt_means = g.prec_chol = g.log_const = g.A_t = g.Dm = 0x1000
+    g.M, g.D = 4, 4
+    a = _lib.NnkGmmTrajArgs()
+    for k, name in enumerate(("x", "lp", "c", "utt_off", "tile_off", "inv_Dm", "log_norm", "E_bar", "V", "ll_part")):
+        setattr(a, name, 0x2000 + 0x100 * k)
+    a.x_ld, a.c_ld, a.T, a.n_utt, a.n_tiles, a.static_dim = 4, 2, 0, 1, 0, 2
+    a.win = _lib.make_windows([(0, 0, np.array([1.0])), (1, 1, np.array([-0.5, 0.0, 0.5]))])
+    a.mode = _lib.NNK_GMM_TRAJ_EM
+    return g, a
+
+
+def test_c_argument_checks():
+    """Each bad argument gets NNK_ERR_ARG / NNK_ERR_UNSUPPORTED from the C entry point; T = 0 is a no-op."""
+    from nnmnkwii_b200 import _lib
+    fn = _lib.lib.nnk_gmm_traj_em
+    g, a = _valid_args(_lib)
+    assert fn(ctypes.byref(g), ctypes.byref(a), None) == _lib.NNK_OK
+    assert fn(None, ctypes.byref(a), None) == _lib.NNK_ERR_ARG
+    assert fn(ctypes.byref(g), None, None) == _lib.NNK_ERR_ARG
+
+    def rc(**changes):
+        g, a = _valid_args(_lib)
+        for k, v in changes.items():
+            if k.startswith("g_"):
+                setattr(g, k[2:], v)
+            elif k == "half":
+                a.win.u[1] = v
+            else:
+                setattr(a, k, v)
+        return fn(ctypes.byref(g), ctypes.byref(a), None)
+
+    for bad in (dict(mode=2), dict(mode=-1), dict(T=-1), dict(n_utt=0), dict(n_tiles=-1), dict(static_dim=0),
+                dict(static_dim=3), dict(g_D=5), dict(g_M=0), dict(x_ld=3), dict(c_ld=1), dict(x=None), dict(lp=None),
+                dict(c=None), dict(utt_off=None), dict(tile_off=None), dict(inv_Dm=None), dict(log_norm=None),
+                dict(E_bar=None), dict(V=None), dict(g_A_t=None), dict(g_src_means=None), dict(g_tgt_means=None),
+                dict(mode=_lib.NNK_GMM_TRAJ_OBJECTIVE, ll_part=None), dict(half=_lib.NNK_MAX_HALF + 1)):
+        assert rc(**bad) == _lib.NNK_ERR_ARG, bad
+    # the objective mode needs no E_bar / V, the EM mode no ll_part
+    assert rc(mode=_lib.NNK_GMM_TRAJ_OBJECTIVE, E_bar=None, V=None) == _lib.NNK_OK
+    assert rc(ll_part=None) == _lib.NNK_OK
+    # more than 96 features, more than 65535 mixtures
+    assert rc(g_D=98, static_dim=49, x_ld=98, c_ld=49) == _lib.NNK_ERR_UNSUPPORTED
+    assert rc(g_M=65536) == _lib.NNK_ERR_UNSUPPORTED
+    assert "96" in _lib.last_error() or "65535" in _lib.last_error()
