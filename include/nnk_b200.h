@@ -312,6 +312,59 @@ int nnk_gmm_logprob(const nnk_gmm_t* gmm, const double* x, int64_t x_ld, int32_t
 int nnk_gmm_map(const nnk_gmm_t* gmm, const double* x, int64_t x_ld, int32_t T, const double* lp, int32_t mode, double* E,
                 double* Dv, int32_t* mix, void* stream);
 
+/* ---- trajectory EM of GMM voice conversion (baseline.gmm.MLPG.transform_em; csrc/nnk_gmm_traj.cu) --------------
+ * float64.  The model (Toda, Black & Tokuda 2007, Sec. III, with the diagonal Eq. 23 variances of baseline.gmm.MLPG):
+ * source frames x_t (D = nw * static_dim columns), static trajectory c (static_dim columns) and its
+ * static + dynamic sequence Y_t[w * static_dim + s] = sum_{k = -l_w}^{u_w} coef[w][l_w + k] c_{t+k}[s], where
+ * frames outside the utterance of t are zero.  Per mixture m:
+ *   E_{m,t} = nu_m + A_m (x_t - mu_m)                    (gmm->tgt_means, gmm->A_t, gmm->src_means; Eq. 22)
+ *   lw_{t,m} = lp[t][m] + log_norm[m][e_t] - 1/2 sum_{d in K_t} (Y_t - E_{m,t})_d^2 inv_Dm[m][d]
+ * with lp from nnk_gmm_logprob and inv_Dm = 1 / D_m.  Like nnk_mlpg_fwd, which gives the dynamic windows zero
+ * precision on the first and last H frames of an utterance (H = max_w max(l_w, u_w)), the columns K_t of frame t
+ * are all D columns (e_t = 0) except on those edge frames, where they are the static_dim columns of window 0
+ * (e_t = 1); log_norm[m][e] = -1/2 (sum_{d in K} log D_m,d + |K| log 2 pi) over the same columns.
+ *
+ * nnk_gmm_traj_em, one CTA per tile of NNK_GMM_TRAJ_TILE frames of one utterance:
+ *   mode NNK_GMM_TRAJ_EM (E-step): gamma_{t,m} = softmax_m lw_{t,m};
+ *     V[t][d] = 1 / P_t,d with P_t,d = sum_m gamma_{t,m} inv_Dm[m][d];
+ *     E_bar[t][d] = (sum_m gamma_{t,m} E_{m,t,d} inv_Dm[m][d]) / P_t,d;
+ *     both (T, D) row-major, the layout nnk_mlpg_fwd reads as means / variances.
+ *   mode NNK_GMM_TRAJ_OBJECTIVE: E_bar and V are not touched (may be NULL).
+ *   Both modes: ll_part[tile] = sum over the tile's frames, in frame order, of log sum_m exp lw_{t,m}
+ *     (ll_part may be NULL in mode EM).  Utterance u owns the tiles tile_off[u] .. tile_off[u+1] - 1, in frame
+ *     order; the per-utterance objective is their sum.
+ * Tables (device int32, n_utt + 1 entries each): utterance u is frames utt_off[u] .. utt_off[u+1] - 1 with
+ * utt_off[0] = 0, utt_off[n_utt] = T; tile_off[0] = 0, tile_off[u+1] - tile_off[u] =
+ * ceil(len_u / NNK_GMM_TRAJ_TILE), tile_off[n_utt] = n_tiles.
+ * Errors: NNK_ERR_ARG for NULL pointers, bad sizes or strides, D != win.nw * static_dim, a bad window set or
+ * mode; NNK_ERR_UNSUPPORTED for D > 96 or more than 65535 mixtures; all before anything touches the device. */
+#define NNK_GMM_TRAJ_EM 0
+#define NNK_GMM_TRAJ_OBJECTIVE 1
+#define NNK_GMM_TRAJ_TILE 32
+
+typedef struct nnk_gmm_traj_args {
+  const double* x;            /* device (T, x_ld) source frames, D = gmm->D columns                         */
+  int64_t x_ld;
+  const double* lp;           /* device (T, M) from nnk_gmm_logprob                                         */
+  const double* c;            /* device (T, c_ld) current static trajectory, static_dim columns              */
+  int64_t c_ld;
+  int32_t T;
+  int32_t n_utt;
+  const int32_t* utt_off;     /* device (n_utt + 1)                                                         */
+  const int32_t* tile_off;    /* device (n_utt + 1)                                                         */
+  int32_t n_tiles;
+  int32_t static_dim;
+  nnk_windows_t win;
+  int32_t mode;               /* NNK_GMM_TRAJ_EM / NNK_GMM_TRAJ_OBJECTIVE                                    */
+  const double* inv_Dm;       /* device (M, D) 1 / D_m                                                      */
+  const double* log_norm;     /* device (M, 2): all columns, static columns only                            */
+  double* E_bar;              /* device (T, D), mode EM                                                     */
+  double* V;                  /* device (T, D), mode EM                                                     */
+  double* ll_part;            /* device (n_tiles), or NULL in mode EM                                       */
+} nnk_gmm_traj_args_t;
+
+int nnk_gmm_traj_em(const nnk_gmm_t* gmm, const nnk_gmm_traj_args_t* args, void* stream);
+
 /* ---- GMM training: EM for full-covariance mixtures (sklearn.mixture.GaussianMixture.fit) ----------------
  * N frames of D features (D <= 128), K components (K <= 128); all parameters are float64 device arrays,
  * X is float32 (widened on load) or float64.  One EM iteration is
@@ -466,6 +519,38 @@ int nnk_preemphasis(const void* x, void* out, int32_t dtype, int64_t rows, int64
                     unsigned long long* counters, void* stream);
 int nnk_mulaw(const void* x, int32_t in_type, void* out, int32_t mode, int32_t variant, int64_t n, double mu,
               void* stream);
+
+/* ---- modulation spectrum (preprocessing/modspec.py; csrc/nnk_modspec.cu; DESIGN.md 3.16) -----------------------
+ * nnk_modspec: one CTA per (utterance b, feature column d).  The column's first len_b frames (lengths[b], or
+ * T_in when lengths is NULL; later frames are never read) are zero-padded to n and transformed with an n-point
+ * real FFT in shared memory (n / 2-point complex FFT and split); Y = fwd_scale * X is the spectrum in the
+ * norm's scaling.  K = n / 2 + 1 bins; all arrays are row-major (B, rows, D).
+ *   mode 0 (power):   out  = |Y_k|^2, (B, K, D); out2 = Y_k / |Y_k| as interleaved (re, im), (B, K, D, 2),
+ *                     or NULL.  A zero bin has phase (+1, 0), or (-1, 0) when its real part is -0.
+ *   mode 1 (smooth):  bins k >= limit_bin become Y_k / |Y_k| (log_domain) or 0, then
+ *                     out = inv_scale * irfft_unnormalised(Y)[:len_b], (B, T_out, D).
+ *   mode 2 (inverse): in = |Y|^2 (B, K, D), in2 = phase (B, K, D, 2); Y = sqrt(in) * in2;
+ *                     out = inv_scale * irfft_unnormalised(Y)[:len_b], (B, T_out, D).  The imaginary parts of
+ *                     bins 0 and n / 2 are ignored, as numpy.fft.irfft does.
+ *   mode 3 (grad):    in2 = dL/d|Y|^2 (B, K, D); out = dL/dx = 2 fwd_scale Re(sum_k G_k conj(Y_k) e^{-2 pi i k t / n})
+ *                     for t < len_b, (B, T_out, D).
+ *   mode 4 (log power): out = log(max(|Y_k|^2, tiny)), (B, K, D), tiny the smallest normal number of the dtype
+ *                     (FLT_MIN, DBL_MIN); out2 must be NULL.  No inverse FFT, like mode 0.
+ *   mode 5 (post-filter): in2 = (a, c) interleaved, (K, D, 2), shared by every utterance.  Bin 0 is kept; a bin
+ *                     k >= 1 of zero power stays 0, any other becomes Y_k / |Y_k| exp(s' / 2) with
+ *                     s' = a s + c, s = log(max(|Y_k|^2, tiny)); then, as mode 1,
+ *                     out = inv_scale * irfft_unnormalised(Y)[:len_b], (B, T_out, D).  out2 must be NULL.
+ * Frames len_b <= t < T_out of out are written as 0.  n is 256, 512, 1024, 2048 or 4096 (else NNK_ERR_ARG);
+ * every len_b must be <= n and <= T_out (<= T_in for the modes that read x). */
+#define NNK_MS_POWER 0
+#define NNK_MS_SMOOTH 1
+#define NNK_MS_INVERSE 2
+#define NNK_MS_GRAD 3
+#define NNK_MS_LOGPOWER 4
+#define NNK_MS_POSTFILTER 5
+int nnk_modspec(int32_t mode, int32_t dtype, int32_t n, const void* in, const void* in2, void* out, void* out2,
+                int32_t B, int32_t T_in, int32_t T_out, int32_t D, const int32_t* lengths, double fwd_scale,
+                double inv_scale, int32_t limit_bin, int32_t log_domain, void* stream);
 
 /* ---- sharded batches (SURVEY.md 8e; the reference has no multi-device path) ------------------------
  * Copies n_seg row segments (whole utterances) between two row-major device matrices:

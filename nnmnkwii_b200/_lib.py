@@ -77,6 +77,32 @@ class NnkGmm(ctypes.Structure):
     ]
 
 
+NNK_GMM_TRAJ_EM, NNK_GMM_TRAJ_OBJECTIVE, NNK_GMM_TRAJ_TILE = 0, 1, 32
+
+
+class NnkGmmTrajArgs(ctypes.Structure):
+    _fields_ = [
+        ("x", ctypes.c_void_p),
+        ("x_ld", ctypes.c_int64),
+        ("lp", ctypes.c_void_p),
+        ("c", ctypes.c_void_p),
+        ("c_ld", ctypes.c_int64),
+        ("T", ctypes.c_int32),
+        ("n_utt", ctypes.c_int32),
+        ("utt_off", ctypes.c_void_p),
+        ("tile_off", ctypes.c_void_p),
+        ("n_tiles", ctypes.c_int32),
+        ("static_dim", ctypes.c_int32),
+        ("win", NnkWindows),
+        ("mode", ctypes.c_int32),
+        ("inv_Dm", ctypes.c_void_p),
+        ("log_norm", ctypes.c_void_p),
+        ("E_bar", ctypes.c_void_p),
+        ("V", ctypes.c_void_p),
+        ("ll_part", ctypes.c_void_p),
+    ]
+
+
 class NnkGmmEmArgs(ctypes.Structure):
     _fields_ = [
         ("X", ctypes.c_void_p),
@@ -102,6 +128,7 @@ class NnkGmmEmArgs(ctypes.Structure):
 
 NNK_KM_CHANGED, NNK_KM_EMPTY, NNK_KM_SHIFT, NNK_KM_INERTIA, NNK_KM_DISTINCT, NNK_KM_VAR_MEAN = 0, 1, 2, 3, 4, 5
 NNK_KM_STATUS_LEN = 8
+NNK_MS_POWER, NNK_MS_SMOOTH, NNK_MS_INVERSE, NNK_MS_GRAD, NNK_MS_LOGPOWER, NNK_MS_POSTFILTER = 0, 1, 2, 3, 4, 5
 
 
 class NnkKmeansArgs(ctypes.Structure):
@@ -199,6 +226,7 @@ SIGNATURES = {
     "nnk_segment_copy": (ctypes.c_int, [vp, vp, i32, i64, i64, i64, vp, vp, vp, i32, i32, vp]),
     "nnk_gmm_logprob": (ctypes.c_int, [P(NnkGmm), vp, i64, i32, vp, vp]),
     "nnk_gmm_map": (ctypes.c_int, [P(NnkGmm), vp, i64, i32, vp, i32, vp, vp, vp, vp]),
+    "nnk_gmm_traj_em": (ctypes.c_int, [P(NnkGmm), P(NnkGmmTrajArgs), vp]),
     "nnk_gmm_em_workspace_bytes": (size_t, [i64, i32, i32]),
     "nnk_gmm_em_estep": (ctypes.c_int, _GMM_EM),
     "nnk_gmm_em_mstep": (ctypes.c_int, _GMM_EM),
@@ -221,6 +249,7 @@ SIGNATURES = {
     "nnk_preemphasis_workspace_bytes": (i64, [i32, i64, i64, f64, i32]),
     "nnk_preemphasis": (ctypes.c_int, [vp, vp, i32, i64, i64, vp, f64, i32, vp, i64, vp, vp]),
     "nnk_mulaw": (ctypes.c_int, [vp, i32, vp, i32, i32, i64, f64, vp]),
+    "nnk_modspec": (ctypes.c_int, [i32, i32, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp, f64, f64, i32, i32, vp]),
     "nnk_peer_alloc": (ctypes.c_int, [size_t, P(vp)]),
     "nnk_peer_free": (ctypes.c_int, [vp]),
     "nnk_peer_export": (ctypes.c_int, [vp, vp]),
@@ -229,44 +258,6 @@ SIGNATURES = {
     "nnk_peer_copy": (ctypes.c_int, [vp, vp, size_t, vp]),
 }
 EXPORTS = list(SIGNATURES)
-
-# the modulation-spectrum kernels (include/nnk_modspec.h), in the same library
-NNK_MS_POWER, NNK_MS_SMOOTH, NNK_MS_INVERSE, NNK_MS_GRAD, NNK_MS_LOGPOWER, NNK_MS_POSTFILTER = 0, 1, 2, 3, 4, 5
-MODSPEC_SIGNATURES = {
-    "nnk_modspec": (ctypes.c_int, [i32, i32, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp, f64, f64, i32, i32, vp]),
-}
-
-# the trajectory EM of GMM voice conversion (include/nnk_gmm_traj.h), in the same library
-NNK_GMM_TRAJ_EM, NNK_GMM_TRAJ_OBJECTIVE, NNK_GMM_TRAJ_TILE = 0, 1, 32
-
-
-class NnkGmmTrajArgs(ctypes.Structure):
-    _fields_ = [
-        ("x", ctypes.c_void_p),
-        ("x_ld", ctypes.c_int64),
-        ("lp", ctypes.c_void_p),
-        ("c", ctypes.c_void_p),
-        ("c_ld", ctypes.c_int64),
-        ("T", ctypes.c_int32),
-        ("n_utt", ctypes.c_int32),
-        ("utt_off", ctypes.c_void_p),
-        ("tile_off", ctypes.c_void_p),
-        ("n_tiles", ctypes.c_int32),
-        ("static_dim", ctypes.c_int32),
-        ("win", NnkWindows),
-        ("mode", ctypes.c_int32),
-        ("inv_Dm", ctypes.c_void_p),
-        ("log_norm", ctypes.c_void_p),
-        ("E_bar", ctypes.c_void_p),
-        ("V", ctypes.c_void_p),
-        ("ll_part", ctypes.c_void_p),
-    ]
-
-
-GMM_TRAJ_SIGNATURES = {
-    "nnk_gmm_traj_em": (ctypes.c_int, [P(NnkGmm), P(NnkGmmTrajArgs), vp]),
-}
-
 
 class NnkError(RuntimeError):
     pass
@@ -281,8 +272,7 @@ def _load():
     L.nnk_abi_version.restype = ctypes.c_int
     if L.nnk_abi_version() != ABI_VERSION:
         raise ImportError("libnnk_b200.so ABI %d != binding ABI %d: rebuild" % (L.nnk_abi_version(), ABI_VERSION))
-    for name, (restype, argtypes) in (list(SIGNATURES.items()) + list(MODSPEC_SIGNATURES.items())
-                                  + list(GMM_TRAJ_SIGNATURES.items())):
+    for name, (restype, argtypes) in SIGNATURES.items():
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, argtypes
     return L

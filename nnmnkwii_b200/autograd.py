@@ -10,9 +10,7 @@ Differences that are additions, not signature changes:
     (csrc/nnk_uvmlpg.cu) instead of two dense GEMMs that multiply ~95 % zeros.
 
 The modulation-spectrum part (nnmnkwii/autograd/_impl/modspec.py): ``ModSpec`` and ``modspec``, plus the batched
-``ModSpecBatch`` / ``modspec_batch``, on csrc/nnk_modspec.cu.  Like ``preprocessing.modspec`` their names are not
-in ``__all__``, which names the entry points of the buffers-and-streams catalogue; tests/test_modspec_gpu.py runs
-the same checks on them.
+``ModSpecBatch`` / ``modspec_batch``, on csrc/nnk_modspec.cu.
 """
 import numpy as np
 import torch
@@ -226,5 +224,6 @@ def unit_variance_mlpg(R, means):
     return UnitVarianceMLPG.apply(means, R)
 
 
-__all__ = ["MLPG", "MLPGBatch", "UnitVarianceMLPG", "mlpg", "mlpg_batch", "unit_variance_mlpg"]
+__all__ = ["MLPG", "MLPGBatch", "UnitVarianceMLPG", "mlpg", "mlpg_batch", "unit_variance_mlpg", "ModSpec",
+           "ModSpecBatch", "modspec", "modspec_batch"]
 _ = np  # numpy is part of the reference module's namespace

@@ -348,7 +348,7 @@ class MLPG(MLPGBase):
 
     def _em_constants(self, c):
         """1 / D_m and -1/2 (sum_d log D_m,d + n log 2 pi) over all n = D columns and over the static ones (the
-        columns an utterance's edge frames keep, see include/nnk_gmm_traj.h) on the device, cached with the
+        columns an utterance's edge frames keep, see include/nnk_b200.h) on the device, cached with the
         other tables."""
         if "em" not in c:
             import torch

@@ -1,10 +1,10 @@
 // nnk_gmm_traj.cu -- trajectory EM of GMM-based voice conversion (baseline.gmm.MLPG.transform_em) on sm_90a,
-// float64 (C ABI: include/nnk_gmm_traj.h).
+// float64 (C ABI: include/nnk_b200.h).
 //
 // The E-step of the EM of Toda, Black & Tokuda 2007, Sec. III, with the diagonal Eq. 23 variances: for every
 // frame t and mixture m the log-weight
 //   lw_{t,m} = lp[t][m] + log_norm[m] - 1/2 |Y_t - E_{m,t}|^2_{1 / D_m},   E_{m,t} = nu_m + A_m (x_t - mu_m),
-// (on an utterance's edge frames over the static columns only, see include/nnk_gmm_traj.h), its softmax over m, and the precision-weighted statistics the M-step (one MLPG solve) needs.  One kernel,
+// (on an utterance's edge frames over the static columns only, see include/nnk_b200.h), its softmax over m, and the precision-weighted statistics the M-step (one MLPG solve) needs.  One kernel,
 // gmm_traj_em_kernel<EPL, EM>: a CTA owns a tile of TRAJ_FT frames of one utterance; the tile's x rows and the
 // c rows of the tile plus the window halo (zero outside the utterance) are staged once, Y_t is formed from the
 // window taps into registers, then the mixtures stream through shared memory (A_m^T, mu_m, nu_m, 1 / D_m).
@@ -16,7 +16,6 @@
 #include <math_constants.h>
 
 #include "nnk_common.cuh"
-#include "../../include/nnk_gmm_traj.h"
 
 namespace nnk {
 

@@ -1,5 +1,5 @@
 // nnk_modspec.cu -- modulation spectrum: preprocessing.modspec / inv_modspec / modspec_smoothing and the
-// gradient of autograd.ModSpec (C ABI: include/nnk_modspec.h).
+// gradient of autograd.ModSpec (C ABI: include/nnk_b200.h).
 //
 // modspec_kernel<T, LOGN>: one CTA per (utterance, feature column).  The n real frames are packed as
 // z_t = x_{2t} + i x_{2t+1} (M = n / 2 complex points) into shared memory in bit-reversed order, and an
@@ -17,7 +17,6 @@
 #include <cfloat>
 
 #include "nnk_common.cuh"
-#include "../../include/nnk_modspec.h"
 
 namespace nnk {
 

@@ -2,9 +2,7 @@
 pysptk) and the modulation-spectrum post-filter with its statistics (additive)."""
 import numpy as np
 
-# ``__all__`` names the entry points of the buffers-and-streams catalogue (tests/stream_catalogue.py); the
-# modulation-spectrum post-filter has the same checks in tests/test_ms_postfilter_gpu.py, so it is not listed
-__all__ = ["merlin_post_filter"]
+__all__ = ["merlin_post_filter", "modspec_post_filter", "modspec_statistics"]
 
 _basis_cache = {}
 

@@ -114,11 +114,10 @@ from .normalize import (inv_minmax_scale, inv_scale, meanstd, meanvar, minmax, m
 from .f0 import interp1d  # noqa: E402
 from .waveform import (inv_mulaw, inv_mulaw_quantize, inv_preemphasis, mulaw, mulaw_quantize,  # noqa: E402
                        preemphasis)
-# ``__all__`` names the entry points of the buffers-and-streams catalogue (tests/stream_catalogue.py); the
-# modulation spectrum has the same checks in tests/test_modspec_gpu.py, so its names are imported, not listed
 from .modspec import inv_modspec, modphase, modspec, modspec_smoothing  # noqa: E402,F401
 
 __all__ = ["trim_zeros_frames", "delta_features", "meanvar", "meanstd", "minmax", "scale", "inv_scale",
            "minmax_scale_params", "minmax_scale", "inv_minmax_scale", "remove_zeros_frames", "interp1d",
            "preemphasis", "inv_preemphasis", "mulaw", "inv_mulaw", "mulaw_quantize", "inv_mulaw_quantize",
-           "adjust_frame_length", "adjust_frame_lengths", "adjast_frame_length", "adjast_frame_lengths"]
+           "adjust_frame_length", "adjust_frame_lengths", "adjast_frame_length", "adjast_frame_lengths", "modspec",
+           "modphase", "inv_modspec", "modspec_smoothing"]

@@ -1,7 +1,7 @@
 """Modulation spectrum (MS) -- drop-in for ``nnmnkwii.preprocessing.modspec``, ``modphase``, ``inv_modspec`` and
 ``modspec_smoothing`` (nnmnkwii/preprocessing/modspec.py).
 
-Runs on the GPU (C ABI ``nnk_modspec``, include/nnk_modspec.h, csrc/nnk_modspec.cu): one CTA per (utterance,
+Runs on the GPU (C ABI ``nnk_modspec``, include/nnk_b200.h, csrc/nnk_modspec.cu): one CTA per (utterance,
 feature column) zero-pads the column to ``n`` frames and runs the real FFT in shared memory.  Smoothing runs the
 forward FFT, the band removal and the inverse FFT in the same CTA, so the spectrum never reaches global memory;
 the gradient of ``autograd.ModSpec`` is the same kernel in its gradient mode.

@@ -15,6 +15,8 @@ HOST_ONLY = {
     ("autograd", "mlpg"): "calls MLPG.apply, which the MLPG case runs",
     ("autograd", "mlpg_batch"): "calls MLPGBatch.apply, which the MLPGBatch case runs",
     ("autograd", "unit_variance_mlpg"): "calls UnitVarianceMLPG.apply, which the UnitVarianceMLPG cases run",
+    ("autograd", "modspec"): "calls ModSpec.apply, which the ModSpec case runs",
+    ("autograd", "modspec_batch"): "calls ModSpecBatch.apply, which the ModSpecBatch case runs",
     ("preprocessing", "trim_zeros_frames"): "NumPy on the host; the device trim runs inside DTWAligner and "
                                             "apply_each2d_trim",
     ("preprocessing", "remove_zeros_frames"): "NumPy on the host, the reference's semantics",
@@ -42,7 +44,8 @@ COVERED = {
     ("paramgen", "mlpg"), ("paramgen", "mlpg_batch"), ("paramgen", "mlpg_grad"), ("paramgen", "mlpg_grad_batch"),
     ("paramgen", "unit_variance_mlpg_matrix"), ("paramgen", "mlpg_gv"), ("paramgen", "mlpg_gv_batch"),
     ("paramgen", "global_variance"), ("paramgen", "gv_statistics"),
-    ("autograd", "MLPG"), ("autograd", "MLPGBatch"), ("autograd", "UnitVarianceMLPG"),
+    ("autograd", "MLPG"), ("autograd", "MLPGBatch"), ("autograd", "UnitVarianceMLPG"), ("autograd", "ModSpec"),
+    ("autograd", "ModSpecBatch"),
     ("metrics", "melcd"), ("metrics", "mean_squared_error"), ("metrics", "lf0_mean_squared_error"),
     ("metrics", "vuv_error"),
     ("preprocessing", "delta_features"), ("preprocessing", "meanvar"), ("preprocessing", "meanstd"),
@@ -50,8 +53,10 @@ COVERED = {
     ("preprocessing", "minmax_scale"), ("preprocessing", "inv_minmax_scale"), ("preprocessing", "interp1d"),
     ("preprocessing", "preemphasis"), ("preprocessing", "inv_preemphasis"), ("preprocessing", "mulaw"),
     ("preprocessing", "inv_mulaw"), ("preprocessing", "mulaw_quantize"), ("preprocessing", "inv_mulaw_quantize"),
+    ("preprocessing", "modspec"), ("preprocessing", "modphase"), ("preprocessing", "inv_modspec"),
+    ("preprocessing", "modspec_smoothing"),
     ("preprocessing.alignment", "DTWAligner"),
-    ("postfilters", "merlin_post_filter"),
+    ("postfilters", "merlin_post_filter"), ("postfilters", "modspec_post_filter"), ("postfilters", "modspec_statistics"),
     ("baseline.gmm", "MLPG"), ("baseline.gmm", "MLPGBase"), ("baseline.gmm", "GaussianMixture"),
     ("util", "apply_each2d_trim"), ("util", "apply_each2d_padded"),
     ("util.linalg", "cholesky_inv"), ("util.linalg", "cholesky_inv_banded"),

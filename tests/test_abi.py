@@ -1,5 +1,6 @@
-"""CPU: the C-ABI library builds, loads, exports every symbol include/nnk_b200.h declares, and the
-product never routes through the oracle or any CPU fallback.  No compute calls (no GPU here)."""
+"""CPU: the C-ABI library builds, loads and exports every symbol include/nnk_b200.h declares; the binding
+(nnmnkwii_b200/_lib.py) matches every prototype, struct and integer constant of that header; and the product
+never routes through the oracle or any CPU fallback.  No compute calls (no GPU here)."""
 import ctypes
 import os
 import re
@@ -24,12 +25,27 @@ def test_library_exports_every_declared_symbol():
     assert _lib.lib.nnk_abi_version() == int(re.search(r"#define NNK_ABI_VERSION (\d+)", _header()).group(1))
 
 
+def _code():
+    """The header without its comments."""
+    return re.sub(r"/\*.*?\*/|//[^\n]*", "", _header(), flags=re.S)
+
+
+def prototypes():
+    """(return type, name, [parameter declarations]) of every function the header declares."""
+    protos = re.findall(r"([A-Za-z_][\w ]*\**)\s*\b(nnk_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", _code())
+    return [(ret, name, [] if params.strip() in ("", "void") else [p.strip() for p in params.split(",")])
+            for ret, name, params in protos]
+
+
 def _c_kind(c_type):
-    """'ptr', 'i4', 'i8', 'f8' or None (void) of a C type."""
+    """'ptr', 'i4', 'i8', 'f8', 'struct nnk_<x>' or None (void) of a C type."""
     if "*" in c_type:
         return "ptr"
+    c_type = c_type.replace("const", "").strip()
+    if re.fullmatch(r"nnk_\w+_t", c_type):
+        return "struct " + c_type[:-2]
     return {"void": None, "int": "i4", "int32_t": "i4", "int64_t": "i8", "uint64_t": "i8", "size_t": "i8",
-            "double": "f8"}[c_type.strip()]
+            "double": "f8"}[c_type]
 
 
 def _ctypes_kind(t):
@@ -37,6 +53,10 @@ def _ctypes_kind(t):
         return None
     if issubclass(t, (ctypes._Pointer, ctypes.c_void_p, ctypes.c_char_p)):
         return "ptr"
+    if issubclass(t, ctypes.Array):
+        return ("array", t._length_, _ctypes_kind(t._type_))
+    if issubclass(t, ctypes.Structure):
+        return "struct " + re.sub(r"(?<!^)([A-Z])", r"_\1", t.__name__).lower()
     if t is ctypes.c_double:
         return "f8"
     return "i%d" % ctypes.sizeof(t)
@@ -46,34 +66,66 @@ def test_signature_table_matches_header_prototypes():
     """Every binding has the header's arity and, per argument and result, the same kind: an int32_t bound
     as an int64_t (or back) would silently truncate or misread the argument."""
     from nnmnkwii_b200 import _lib
-    h = re.sub(r"/\*.*?\*/|//[^\n]*", "", _header(), flags=re.S)
-    protos = re.findall(r"([A-Za-z_][\w ]*\**)\s*\b(nnk_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", h)
+    protos = prototypes()
     assert sorted(name for _, name, _ in protos) == sorted(_lib.SIGNATURES)
     for ret, name, params in protos:
         restype, argtypes = _lib.SIGNATURES[name]
-        params = [] if params.strip() in ("", "void") else params.split(",")
         assert _ctypes_kind(restype) == _c_kind(ret), name
         assert [_ctypes_kind(t) for t in argtypes] == [_c_kind(p.rsplit(None, 1)[0]) for p in params], name
 
 
+def _struct_fields(body, _lib):
+    """[(name, kind)] of the fields of a C struct body; an array's kind is ('array', length, element kind)."""
+    fields = []
+    for decl in (d.strip() for d in body.split(";")):
+        if not decl:
+            continue
+        c_type, declarators = re.match(r"((?:const\s+)?[A-Za-z_]\w*\s*\**)\s*(.*)", decl, re.S).groups()
+        for d in declarators.split(","):
+            name = re.match(r"\s*(\**)\s*([A-Za-z_]\w*)", d).group(2)
+            kind = _c_kind(c_type + ("*" if d.strip().startswith("*") else ""))
+            for dim in reversed(re.findall(r"\[\s*(\w+)\s*\]", d)):
+                kind = ("array", int(dim) if dim.isdigit() else getattr(_lib, dim), kind)
+            fields.append((name, kind))
+    return fields
+
+
+def test_every_struct_matches_its_binding():
+    """Each ``typedef struct nnk_<x> { ... } nnk_<x>_t`` has the fields of its ctypes class ``_lib.Nnk<X>`` (of
+    ``CHAIN_DTYPE`` for nnk_chain) in the same order and of the same kinds, so both sides lay it out alike; and
+    every ctypes structure of the binding is one of them."""
+    from nnmnkwii_b200 import _lib
+    structs = re.findall(r"typedef struct (nnk_\w+) \{(.*?)\} (\w+);", _code(), re.S)
+    assert len(structs) >= 10
+    bound = set()
+    for name, body, alias in structs:
+        assert alias == name + "_t", alias
+        want = _struct_fields(body, _lib)
+        if name == "nnk_chain":
+            dt = _lib.CHAIN_DTYPE
+            got = [(f, "i%d" % dt.fields[f][0].itemsize) for f in dt.names if dt.fields[f][0].kind == "i"]
+        else:
+            cls = getattr(_lib, "".join(p.capitalize() for p in name.split("_")))
+            bound.add(cls.__name__)
+            got = [(f, _ctypes_kind(t)) for f, t in cls._fields_]
+        assert got == want, (name, got, want)
+    structures = {n for n, v in vars(_lib).items() if isinstance(v, type) and issubclass(v, ctypes.Structure)}
+    assert structures == bound, sorted(structures ^ bound)
+
+
+def test_every_integer_constant_matches_its_binding():
+    from nnmnkwii_b200 import _lib
+    defines = re.findall(r"^#define (NNK_[A-Z0-9_]+)\s+(-?\d+)\b", _code(), re.M)
+    assert len(defines) >= 25
+    for name, value in defines:
+        assert getattr(_lib, "ABI_VERSION" if name == "NNK_ABI_VERSION" else name) == int(value), name
+
+
 def test_struct_layouts_match_header():
     from nnmnkwii_b200 import _lib
-    h = _header()
-    assert int(re.search(r"#define NNK_MAX_WIN (\d+)", h).group(1)) == _lib.NNK_MAX_WIN
-    assert int(re.search(r"#define NNK_MAX_HALF (\d+)", h).group(1)) == _lib.NNK_MAX_HALF
     assert ctypes.sizeof(_lib.NnkWindows) == 4 + 4 * _lib.NNK_MAX_WIN * 2 + 4 + 8 * _lib.NNK_MAX_WIN * _lib.NNK_MAX_TAPS
     assert ctypes.sizeof(_lib.NnkStatus) == 16
     assert _lib.CHAIN_DTYPE.itemsize == 16
-    # field order of nnk_mlpg_args_t
-    body = re.search(r"typedef struct nnk_mlpg_args \{(.*?)\} nnk_mlpg_args_t;", h, re.S).group(1)
-    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
-    names = []
-    for decl in body.split(";"):
-        decl = decl.strip()
-        if decl:
-            for part in decl.split(","):
-                names.append(re.findall(r"[A-Za-z_][A-Za-z0-9_]*", part)[-1])
-    assert names == [f[0] for f in _lib.NnkMlpgArgs._fields_]
 
 
 def test_status_decode_roundtrip():

@@ -34,7 +34,8 @@ def test_every_export_is_sorted():
     launching = C.launching_exports(exports)
     # the symbols the kernel families launch through, by header name
     for name in ("nnk_mlpg_fwd", "nnk_mlpg_grad", "nnk_mlpg_solve", "nnk_mlpg_gv", "nnk_dtw_align",
-                 "nnk_postfilter_apply", "nnk_gmm_em_estep", "nnk_kmeans_seed", "nnk_mlpg_host"):
+                 "nnk_postfilter_apply", "nnk_gmm_em_estep", "nnk_kmeans_seed", "nnk_mlpg_host", "nnk_modspec",
+                 "nnk_gmm_traj_em"):
         assert name in launching, name
     assert not any(n.endswith("_workspace_bytes") for n in launching)
 
@@ -43,9 +44,13 @@ def test_every_launching_export_takes_the_stream_last():
     """The GPU module reads a launching call's stream from its last argument; the exceptions run their own."""
     import ctypes
 
+    from test_abi import prototypes
+
     from nnmnkwii_b200 import _lib
     launching = C.launching_exports(_lib.EXPORTS)
     assert C.EXPORTS_OWN_STREAMS <= set(launching)
+    params = {name: p for _, name, p in prototypes()}
     for name in launching:
         if name not in C.EXPORTS_OWN_STREAMS:
             assert _lib.SIGNATURES[name][1][-1] is ctypes.c_void_p, name
+            assert params[name][-1] == "void* stream", name

@@ -6,9 +6,10 @@ family's own reference at its usual bar, and the outputs to compare.  Each case 
 must give outputs bit-identical (NaN positions included) to the plain run:
 
 1. plain, as users call it (and checked against the reference);
-2. with every floating-point CUDA tensor from ``torch.empty`` / ``empty_like`` / ``Tensor.new_empty`` filled
-   with 0xFF bytes (NaN), then with 0x7F bytes (a huge finite value).  Integer and uint8 allocations carry
-   indices and workspace tables: they are zero-filled in all three runs, never filled with arbitrary bytes;
+2. with every floating-point (real or complex) CUDA tensor from ``torch.empty`` / ``empty_like`` /
+   ``Tensor.new_empty`` filled with 0xFF bytes (NaN), then with 0x7F bytes (a huge finite value).  Integer and
+   uint8 allocations carry indices and workspace tables: they are zero-filled in all three runs, never filled with
+   arbitrary bytes;
 3. with every workspace request served by the block a larger valid call of the same entry point (other data,
    other lengths) just used, as that call left it (a spy on ``_device.workspace`` hands the blocks over and
    asserts that every request was served), compared with the case run straight after
@@ -79,8 +80,9 @@ def _record_exports():
 # ---- allocation poison and the workspace spy ------------------------------------------------------------------------
 @contextlib.contextmanager
 def allocations(fill=None):
-    """Patch torch.empty / empty_like / Tensor.new_empty (and _device.workspace): floating-point CUDA results
-    get every byte set to ``fill`` (None: left as they are); integer, bool and uint8 results are zeroed."""
+    """Patch torch.empty / empty_like / Tensor.new_empty (and _device.workspace): floating-point (real or complex)
+    CUDA results get every byte set to ``fill`` (None: left as they are); integer, bool and uint8 results are
+    zeroed."""
     import torch
 
     from nnmnkwii_b200 import _device as dev
@@ -88,7 +90,7 @@ def allocations(fill=None):
 
     def treat(t):
         if isinstance(t, torch.Tensor) and t.is_cuda and t.numel():
-            if t.is_floating_point():
+            if t.is_floating_point() or t.is_complex():
                 if fill is not None:
                     t.reshape(-1).view(torch.uint8).fill_(fill)
             else:
@@ -157,6 +159,8 @@ def same(a, b):
     for k, (x, y) in enumerate(zip(a, b)):
         x, y = _as_tensor(x), _as_tensor(y)
         assert x.dtype == y.dtype and x.shape == y.shape, (k, x.dtype, y.dtype, x.shape, y.shape)
+        if x.is_complex():
+            x, y = torch.view_as_real(x), torch.view_as_real(y)
         if x.is_floating_point():
             nx, ny = torch.isnan(x), torch.isnan(y)
             assert torch.equal(nx, ny), "output %d: NaN positions differ (%d vs %d NaN)" % (k, int(nx.sum()), int(ny.sum()))
@@ -212,6 +216,24 @@ def _mv(rng, T, D, dt, var_global=False):
 
 def _lens(rng, n, lo, hi):
     return rng.integers(lo, hi, n).astype(np.int64)
+
+
+MS_N = 512  # DFT length of the modulation-spectrum cases
+
+
+def _nan_padded(rng, lens, T, D, dt):
+    """(B, T, D): utterance b is lens[b] frames of noise through 1 + 0.7 z^-1, then NaN padding."""
+    x = np.full((len(lens), T, D), np.nan, dt)
+    for b, L in enumerate(lens):
+        w = rng.standard_normal((L + 1, D))
+        x[b, :L] = w[1:] + 0.7 * w[:-1]
+    return x
+
+
+def _crel(a, b):
+    """max |a - b| / max |b| of complex arrays."""
+    a, b = np.asarray(a, np.complex128), np.asarray(b, np.complex128)
+    return float(np.abs(a - b).max() / max(1e-300, np.abs(b).max()))
 
 
 # ---- paramgen ----
@@ -507,6 +529,46 @@ for _kind in ("table", "toeplitz", "factored"):
                           *_uv_case(_kind)))
 
 
+@case("autograd_ModSpec_and_ModSpecBatch_f64", [("autograd", "ModSpec"), ("autograd", "ModSpecBatch")])
+def _c():
+    K = MS_N // 2 + 1
+
+    def make(rng, big):
+        T, D = (200, 5) if big else (150, 4)
+        lens = np.array([T, 1, 0, T // 3])
+        return {"x": _cuda(_nan_padded(rng, [T], T, D, np.float64)[0]), "go": _cuda(rng.standard_normal((K, D))),
+                "xb": _cuda(_nan_padded(rng, lens, T, D, np.float64)), "lens": lens,
+                "gob": _cuda(rng.standard_normal((len(lens), K, D)))}
+
+    def call(i):
+        y = i["x"].clone().requires_grad_(True)
+        ms = _AF().ModSpec.apply(y, MS_N, None)
+        ms.backward(i["go"])
+        yb = i["xb"].clone().requires_grad_(True)
+        msb = _AF().ModSpecBatch.apply(yb, MS_N, "ortho", i["lens"])
+        msb.backward(i["gob"])
+        return [ms.detach(), y.grad, msb.detach(), yb.grad]
+
+    def reference(x, G, scale):
+        """scale |X|^2 and the reference's dense gradient scale * 2 G (R cos + I sin), kt = -2 pi k t / n."""
+        X = np.fft.rfft(x, MS_N, axis=0)
+        kt = -2 * np.pi / MS_N * np.arange(K)[:, None] * np.arange(len(x))
+        grad = np.stack([G[:, d] @ (2 * (X.real[:, d, None] * np.cos(kt) + X.imag[:, d, None] * np.sin(kt)))
+                         for d in range(x.shape[1])], axis=1)
+        return scale * (X.real ** 2 + X.imag ** 2), scale * grad
+
+    def check(i, o):
+        o = [_h(t) for t in o]
+        pw, g = reference(_h(i["x"]), _h(i["go"]), 1.0)
+        _bar(rel_err(o[0], pw) < 1e-10 and rel_err(o[1], g) < 1e-10)
+        xb, gob = _h(i["xb"]), _h(i["gob"])
+        for b, L in enumerate(i["lens"]):
+            pw, g = reference(xb[b, :L], gob[b], 1.0 / MS_N)  # norm "ortho": |X|^2 / n
+            _bar(rel_err(o[2][b], pw) < 1e-10 and not o[3][b, L:].any())
+            _bar(L == 0 or rel_err(o[3][b, :L], g) < 1e-10)
+    return make, call, check
+
+
 # ---- metrics ----
 def _metric_inputs(rng, big):
     B, T = (4, 50) if big else (3, 30)
@@ -689,6 +751,50 @@ def _c():
     return make, call, check
 
 
+def _modspec_case(dt, n):
+    K, tol = n // 2 + 1, 1e-4 if dt == np.float32 else 1e-10
+
+    def make(rng, big):
+        T, D = (min(n, 300), 6) if big else (240, 5)
+        lens = np.array([T, 1, 0, T // 2 + 1])
+        ph = np.exp(1j * rng.uniform(-np.pi, np.pi, (len(lens), K, D)))
+        return {"x": _cuda(_nan_padded(rng, lens, T, D, dt)), "lens": lens,
+                "ms": _cuda((rng.random((len(lens), K, D)) ** 2).astype(dt)),
+                "ph": _cuda(ph.astype(np.complex64 if dt == np.float32 else np.complex128))}
+
+    def call(i):
+        P = _P()
+        x, lens = i["x"], i["lens"]
+        ms, ph = P.modspec(x, n=n, return_phase=True, lengths=lens)
+        return [ms, ph, P.modphase(x, n=n, norm="ortho", lengths=lens),
+                P.inv_modspec(i["ms"], i["ph"], lengths=lens), P.inv_modspec(i["ms"], i["ph"]),
+                P.modspec_smoothing(x, 200, n=n, cutoff=40, lengths=lens),
+                P.modspec_smoothing(x, 200, n=n, cutoff=40, log_domain=False, lengths=lens)]
+
+    def check(i, o):
+        x, o = _h(i["x"]).astype(np.float64), [_h(t) for t in o]
+        Y = np.sqrt(_h(i["ms"]).astype(np.float64)) * _h(i["ph"])
+        cut = np.arange(K)[:, None] >= int(n * 40 / 200) + 1
+        for b, L in enumerate(i["lens"]):
+            X = np.fft.rfft(x[b, :L], n, axis=0)
+            pw = X.real ** 2 + X.imag ** 2
+            _bar(rel_err(o[0][b], pw) <= tol)
+            for ph in (o[1], o[2]):  # the phase is judged where it matters, weighted by the amplitude
+                _bar(_crel(np.sqrt(pw) * ph[b], X) <= tol)
+            _bar(rel_err(o[4][b], np.fft.irfft(Y[b], n, axis=0)) <= tol)
+            refs = (np.fft.irfft(Y[b], n, axis=0), np.fft.irfft(np.where(cut, np.exp(1j * np.angle(X)), X), n, axis=0),
+                    np.fft.irfft(np.where(cut, 0, X), n, axis=0))
+            for got, ref in zip((o[3], o[5], o[6]), refs):  # inv_modspec with lengths, smoothing log / linear
+                _bar(not got[b, L:].any() and (L == 0 or rel_err(got[b, :L], ref[:L]) <= tol))
+    return make, call, check
+
+
+for _dt, _n in ((np.float32, 512), (np.float64, 256)):
+    CATALOGUE.append(Case("modspec_family_padded_%s_n%d" % (np.dtype(_dt).name, _n),
+                          [("preprocessing", f) for f in ("modspec", "modphase", "inv_modspec", "modspec_smoothing")],
+                          *_modspec_case(_dt, _n)))
+
+
 def _dtw_case(radius):
     def make(rng, big):
         N, Tx, Ty, D = (3, 60, 70, 5) if big else (2, 40, 48, 5)
@@ -741,6 +847,37 @@ def _c():
     return make, lambda i: [__import__("nnmnkwii_b200.postfilters", fromlist=["x"]).merlin_post_filter(i["mgc"], **PF)], check
 
 
+@case("modspec_statistics_and_post_filter_f64", [("postfilters", "modspec_statistics"),
+                                                 ("postfilters", "modspec_post_filter")])
+def _c():
+    import oracle.ms_postfilter as OM
+
+    def make(rng, big):
+        T, D = (260, 5) if big else (200, 4)
+        glens, lens = np.array([T, T // 2, 1, 37]), np.array([T, 1, 0, T // 4 + 1])
+        return {"gen": _cuda(_nan_padded(rng, glens, T, D, np.float64)), "glens": glens,
+                "nat": _cuda(rng.standard_normal((5, T, D))), "x": _cuda(_nan_padded(rng, lens, T, D, np.float64)),
+                "lens": lens}
+
+    def call(i):
+        from nnmnkwii_b200.postfilters import modspec_post_filter, modspec_statistics
+        G = modspec_statistics(i["gen"], n=MS_N, lengths=i["glens"])
+        N = modspec_statistics(i["nat"], n=MS_N)
+        return list(G) + list(N) + [modspec_post_filter(i["x"], N, G, k=0.8, n=MS_N, lengths=i["lens"])]
+
+    def check(i, o):
+        gen, x, o = _h(i["gen"]), _h(i["x"]), [_h(t) for t in o]
+        want = (OM.statistics([gen[b, :L] for b, L in enumerate(i["glens"])], MS_N)
+                + OM.statistics(list(_h(i["nat"])), MS_N))
+        for got, w in zip(o[:4], want):
+            _bar(rel_err(got, w) < 1e-10)
+        for b, L in enumerate(i["lens"]):  # the filter against the restatement given the device's statistics
+            y = o[4][b]
+            _bar(not y[L:].any() and (L == 0 or rel_err(y[:L], OM.post_filter(x[b, :L], o[2:4], o[0:2], 0.8, MS_N))
+                                      < 1e-10))
+    return make, call, check
+
+
 # ---- baseline.gmm ----
 def _joint_gmm(rng, Mx, dim):
     import types
@@ -767,6 +904,30 @@ def _c():
         mix = lp.argmax(1)
         _bar(rel_err(o[0], oracle.mlpg(Em[np.arange(len(mix)), mix], Dm[mix], W2)) < 1e-9)
         _bar(rel_err(o[1], post) < 1e-9)
+    return make, call, check
+
+
+@case("gmm_MLPG_transform_em", [("baseline.gmm", "MLPG")], ws=True)
+def _c():
+    import oracle.gmm_traj_em as OT
+
+    # one workspace request per MLPG solve: ``big`` keeps n_iter and the number of utterances, only the lengths grow
+    def make(rng, big):
+        return {"gmm": _joint_gmm(np.random.default_rng(11), 6, 24),
+                "srcs": [rng.standard_normal((T, 24)) for T in ((150, 20, 90) if big else (120, 7, 65))]}
+
+    def call(i):
+        from nnmnkwii_b200.baseline.gmm import MLPG
+        m = MLPG(i["gmm"], windows=W3, diff=True)
+        ys, L = m.transform_em_batch(i["srcs"], n_iter=3, return_log_likelihood=True)
+        return [np.concatenate(ys), L, m.transform_em(i["srcs"][0], n_iter=2)]
+
+    def check(i, o):
+        off = np.concatenate([[0], np.cumsum([len(s) for s in i["srcs"]])])
+        for u, src in enumerate(i["srcs"]):
+            want, Lw = OT.transform_em(i["gmm"], W3, src, 3, diff=True)
+            _bar(rel_err(o[0][off[u]:off[u + 1]], want) <= 1e-9 and np.all(np.abs(o[1][u] - Lw) <= 1e-10 * np.abs(Lw)))
+        _bar(rel_err(o[2], OT.transform_em(i["gmm"], W3, i["srcs"][0], 2, diff=True)[0]) <= 1e-9)
     return make, call, check
 
 
@@ -1003,7 +1164,8 @@ def _map_tensors(inp, fn):
 
 
 def _side_stream(c, inp):
-    """The case on a fresh stream S behind a sleep; inputs NaN (integers 0) until S copies them in.
+    """The case on a fresh stream S behind a sleep; inputs NaN (complex: NaN in both parts; integers 0) until S
+    copies them in.
 
     Most calls synchronise S on a host-to-device upload before their launch, so by then S's sleep is over.
     Two things make the arm independent of that timing.  Every launching C call must pass S as its stream
@@ -1013,6 +1175,7 @@ def _side_stream(c, inp):
     the call."""
     import torch
     holders = _map_tensors(inp, lambda t: torch.full_like(t, float("nan")) if t.is_floating_point()
+                           else torch.full_like(t, complex(math.nan, math.nan)) if t.is_complex()
                            else torch.zeros_like(t))
     _cold_caches()
     with allocations(fill=0xFF):

@@ -1,10 +1,9 @@
 """Without a GPU: the float64 restatement of the trajectory EM (oracle/gmm_traj_em.py) never lowers its
-objective and starts from the reference's MLPG.transform; the binding of include/nnk_gmm_traj.h matches the
-header; the C entry point refuses bad arguments before touching the device."""
+objective and starts from the reference's MLPG.transform; the C entry point refuses bad arguments before touching
+the device."""
 import ctypes
 import importlib.util
 import os
-import re
 
 import numpy as np
 import pytest
@@ -41,46 +40,6 @@ def test_oracle_starts_from_the_reference_transform():
         want = golden["y_%d" % i]
         assert c.shape == want.shape == (T, S) and L.shape == (1,)
         assert np.abs(c - want).max() <= 1e-10 * np.abs(want).max(), i
-
-
-def _kind(c_type):
-    c_type = c_type.strip()
-    if "*" in c_type:
-        return "ptr"
-    return {"int": "i4", "int32_t": "i4"}[c_type]
-
-
-def _ctypes_kind(t):
-    if issubclass(t, (ctypes._Pointer, ctypes.c_void_p)):
-        return "ptr"
-    return "i%d" % ctypes.sizeof(t)
-
-
-def _header():
-    return open(os.path.join(ROOT, "include", "nnk_gmm_traj.h")).read()
-
-
-def test_binding_matches_header():
-    """Every nnk_gmm_traj.h prototype is bound with the header's arity and argument kinds, takes the stream
-    last and is exported by the library; the struct's fields and the constants agree."""
-    from nnmnkwii_b200 import _lib
-    h = _header()
-    body = re.sub(r"/\*.*?\*/|//[^\n]*", "", h, flags=re.S)
-    protos = re.findall(r"([A-Za-z_][\w ]*\**)\s*\b(nnk_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", body)
-    assert sorted(name for _, name, _ in protos) == sorted(_lib.GMM_TRAJ_SIGNATURES)
-    L = ctypes.CDLL(_lib.LIB_PATH)
-    for ret, name, params in protos:
-        restype, argtypes = _lib.GMM_TRAJ_SIGNATURES[name]
-        assert _kind(ret) == _ctypes_kind(restype), name
-        assert [_ctypes_kind(t) for t in argtypes] == [_kind(p.rsplit(None, 1)[0]) for p in params.split(",")], name
-        assert argtypes[-1] is ctypes.c_void_p and params.split(",")[-1].split()[-1] == "stream", name
-        assert hasattr(L, name)
-        assert name not in _lib.SIGNATURES
-    fields = re.search(r"typedef struct nnk_gmm_traj_args \{(.*?)\} nnk_gmm_traj_args_t;", body, re.S).group(1)
-    names = [re.findall(r"[A-Za-z_]\w*", d)[-1] for d in fields.split(";") if d.strip()]
-    assert names == [f[0] for f in _lib.NnkGmmTrajArgs._fields_]
-    for c in ("EM", "OBJECTIVE", "TILE"):
-        assert int(re.search(r"#define NNK_GMM_TRAJ_%s (\d+)" % c, h).group(1)) == getattr(_lib, "NNK_GMM_TRAJ_" + c)
 
 
 def _valid_args(_lib):

@@ -5,10 +5,11 @@
   within 1e-10 relative, for every EPL instance of gmm_traj_em_kernel, diff / swap, T off the tile and T < the
   window; the device objective never decreases;
 * a batch equals its utterances one by one, two calls are bit-identical, the errors come before any launch
-  and the launch count depends on n_iter only;
-* dirty allocations (NaN and huge values, device tables built under them) and a delayed side stream with every
-  launch on it, as tests/test_buffers_and_streams_gpu.py runs them for the catalogued entry points.  A call
-  returns only after its work has finished, so no table it reads can be evicted while that work is pending."""
+  and the launch count depends on n_iter only.
+
+Dirty allocations, workspace reuse and a delayed side stream are checked for these entry points by the
+buffers-and-streams catalogue (tests/test_buffers_and_streams_gpu.py), as for every other one.  A call returns
+only after its work has finished, so no table it reads can be evicted while that work is pending."""
 import importlib.util
 import os
 
@@ -18,7 +19,6 @@ import pytest
 from conftest import ROOT
 
 import oracle.gmm_traj_em as OT
-from test_buffers_and_streams_gpu import LEGACY_HOLD_CYCLES, SLEEP_CYCLES, allocations, same
 
 pytestmark = pytest.mark.gpu
 
@@ -128,54 +128,3 @@ def test_errors_come_before_any_launch_and_launches_depend_on_n_iter_only():
             assert len(counts) == 1, (n_iter, ll, counts)
     assert launches(50, 3, False) - launches(50, 2, False) == launches(50, 2, False) - launches(50, 1, False)
     assert launches(50, 2, True) == launches(50, 2, False) + 1
-
-
-# ---- dirty memory and a delayed side stream ---------------------------------------------------------------------
-def _call(m, srcs):
-    ys, L = m.transform_em_batch(srcs, n_iter=3, return_log_likelihood=True)
-    return [np.concatenate(ys), L, m.transform_em(srcs[0], n_iter=2)]
-
-
-def _inputs():
-    g, m = _model(8, 3, 6, 11, diff=True)
-    return g, m, [_src(T, 24, T) for T in (120, 7, 65)]
-
-
-def test_dirty_allocations_and_a_delayed_side_stream():
-    import torch
-
-    from nnmnkwii_b200 import _lib
-    from nnmnkwii_b200.baseline.gmm import MLPG
-    g, m, srcs = _inputs()
-    plain = _call(m, srcs)
-    for fill in (0xFF, 0x7F):
-        with allocations(fill=fill):
-            got = _call(MLPG(g, windows=W[:3], diff=True), srcs)  # tables built under the poison too
-        same(got, plain)
-    # every launching call names the side stream; the legacy default stream is held for the whole call
-    names = list(_lib.GMM_TRAJ_SIGNATURES) + ["nnk_gmm_logprob", "nnk_gmm_map", "nnk_mlpg_fwd"]
-    saved, bad, seen = {n: getattr(_lib.lib, n) for n in names}, [], set()
-    for n, fn in saved.items():
-        def proxy(*a, _fn=fn, _n=n):
-            seen.add(_n)
-            if int(getattr(a[-1], "value", a[-1]) or 0) != torch.cuda.current_stream().cuda_stream:
-                bad.append(_n)
-            return _fn(*a)
-        setattr(_lib.lib, n, proxy)
-    try:
-        torch.cuda.synchronize()
-        S = torch.cuda.Stream()
-        torch.cuda._sleep(LEGACY_HOLD_CYCLES)
-        held = torch.cuda.Event()
-        held.record(torch.cuda.default_stream())
-        with torch.cuda.stream(S), allocations(fill=0xFF):
-            torch.cuda._sleep(SLEEP_CYCLES)
-            got = _call(MLPG(g, windows=W[:3], diff=True), srcs)
-        still_held = not held.query()
-    finally:
-        for n, fn in saved.items():
-            setattr(_lib.lib, n, fn)
-    torch.cuda.synchronize()
-    assert not bad and seen == set(names), (bad, seen)
-    assert still_held, "the legacy default stream's hold ended during the call"
-    same(got, plain)

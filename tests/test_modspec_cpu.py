@@ -1,13 +1,7 @@
 """Without a GPU: the modulation-spectrum entry points refuse bad input with a clear error before touching the
-device, and the binding of nnk_modspec matches include/nnk_modspec.h."""
-import ctypes
-import os
-import re
-
+device."""
 import numpy as np
 import pytest
-
-from conftest import ROOT
 
 
 def test_input_errors():
@@ -58,35 +52,3 @@ def test_input_errors():
     with pytest.raises(ValueError, match=r"\(T, D\) or \(B, T, D\)"):
         P.modspec(np.zeros(10), n=256)
 
-
-def _kind(c_type):
-    c_type = c_type.strip()
-    if "*" in c_type:
-        return "ptr"
-    return {"int": "i4", "int32_t": "i4", "double": "f8"}[c_type]
-
-
-def _ctypes_kind(t):
-    if issubclass(t, (ctypes._Pointer, ctypes.c_void_p)):
-        return "ptr"
-    return "f8" if t is ctypes.c_double else "i%d" % ctypes.sizeof(t)
-
-
-def test_binding_matches_header():
-    """Every nnk_modspec.h prototype is bound with the header's arity and argument kinds, takes the stream last,
-    and is exported by the library; the mode codes agree."""
-    from nnmnkwii_b200 import _lib
-    h = open(os.path.join(ROOT, "include", "nnk_modspec.h")).read()
-    body = re.sub(r"/\*.*?\*/|//[^\n]*", "", h, flags=re.S)
-    protos = re.findall(r"([A-Za-z_][\w ]*\**)\s*\b(nnk_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", body)
-    assert sorted(name for _, name, _ in protos) == sorted(_lib.MODSPEC_SIGNATURES)
-    L = ctypes.CDLL(_lib.LIB_PATH)
-    for ret, name, params in protos:
-        restype, argtypes = _lib.MODSPEC_SIGNATURES[name]
-        assert _kind(ret) == _ctypes_kind(restype), name
-        assert [_ctypes_kind(t) for t in argtypes] == [_kind(p.rsplit(None, 1)[0]) for p in params.split(",")], name
-        assert argtypes[-1] is ctypes.c_void_p and params.split(",")[-1].split()[-1] == "stream", name
-        assert hasattr(L, name)
-        assert name not in _lib.SIGNATURES
-    for mode in ("POWER", "SMOOTH", "INVERSE", "GRAD"):
-        assert int(re.search(r"#define NNK_MS_%s (\d+)" % mode, h).group(1)) == getattr(_lib, "NNK_MS_" + mode)

@@ -5,11 +5,11 @@ autograd.ModSpec / ModSpecBatch.
   DFT length, T = 1, odd, n - 1 and n, norm None and "ortho": float64 within 1e-10, float32 within 1e-4;
 * torch.fft as a second oracle on whole outputs, D = 1 and 37, every norm;
 * the round trip, smoothing above the Nyquist frequency (the identity) and smoothing twice (idempotent);
-* a padded batch with NaN in its padding equals per-utterance calls bit for bit, with every float result
-  allocation poisoned, on a side stream held back by a sleep while the inputs are still NaN on the default
-  stream;
-* gradcheck of the float64 gradient, and the float32 gradient against it."""
-import contextlib
+* a padded batch with NaN in its padding equals per-utterance calls bit for bit;
+* gradcheck of the float64 gradient, and the float32 gradient against it.
+
+Dirty allocations, workspace reuse and a delayed side stream are checked for these entry points by the
+buffers-and-streams catalogue (tests/test_buffers_and_streams_gpu.py), as for every other one."""
 import importlib.util
 import os
 
@@ -25,7 +25,6 @@ _spec = importlib.util.spec_from_file_location("make_modspec_golden",
 MG = importlib.util.module_from_spec(_spec)
 _spec.loader.exec_module(MG)
 TOL = {np.float64: 1e-10, np.float32: 1e-4}
-SLEEP_CYCLES = 40_000_000  # about 20 ms on an H100
 
 
 @pytest.fixture(scope="module")
@@ -163,26 +162,7 @@ def test_smoothing_invariants(dtype):
                 assert rel_err(_np(once), _np(x)) > 1e-2  # the smoothing did remove something
 
 
-# ---- batched == per utterance, whatever the padding, the allocations and the stream hold ---------------------------
-@contextlib.contextmanager
-def _poisoned_allocations():
-    """Every floating-point (real or complex) CUDA tensor from torch.empty / empty_like comes filled with NaN."""
-    import torch
-    orig = (torch.empty, torch.empty_like)
-
-    def treat(t):
-        if t.is_cuda and (t.is_floating_point() or t.is_complex()) and t.numel():
-            t.view(torch.uint8).fill_(0xFF) if t.is_contiguous() else t.fill_(float("nan"))
-        return t
-
-    torch.empty = lambda *a, **k: treat(orig[0](*a, **k))
-    torch.empty_like = lambda *a, **k: treat(orig[1](*a, **k))
-    try:
-        yield
-    finally:
-        torch.empty, torch.empty_like = orig
-
-
+# ---- batched == per utterance, whatever the padding ------------------------------------------------------------------
 def _all_outputs(xb, lens, n, norm, grad_ms):
     """Every entry point on a padded batch: the list of its results."""
     from nnmnkwii_b200 import preprocessing as P
@@ -226,7 +206,6 @@ def test_batched_equals_per_utterance(n, dtype):
     padded = torch.full((len(lens), T, D), float("nan"), dtype=tdt, device="cuda")
     for b, u in enumerate(utts):
         padded[b, :len(u)] = u
-    torch.cuda.synchronize()
 
     def check(got):
         for b, L in enumerate(lens):
@@ -236,21 +215,7 @@ def test_batched_equals_per_utterance(n, dtype):
                 else:
                     assert _same(g[b], w), (b, i)
 
-    with _poisoned_allocations():
-        check(_all_outputs(padded, lens, n, norm, G))
-    # on a side stream held back by a sleep, with the inputs still NaN on the default stream until it has slept
-    xin = torch.full_like(padded, float("nan"))
-    gin = torch.full_like(G, float("nan"))
-    torch.cuda.synchronize()
-    S = torch.cuda.Stream()
-    with _poisoned_allocations(), torch.cuda.stream(S):
-        torch.cuda._sleep(SLEEP_CYCLES)
-        xin.copy_(padded)
-        gin.copy_(G)
-        got = [t.clone() for t in _all_outputs(xin, lens, n, norm, gin)]
-    S.synchronize()
-    check(got)
-    torch.cuda.synchronize()
+    check(_all_outputs(padded, lens, n, norm, G))
 
 
 # ---- gradients ---------------------------------------------------------------------------------------------------------
