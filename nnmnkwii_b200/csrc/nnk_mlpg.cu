@@ -515,11 +515,11 @@ static int launch_mlpg(const nnk_mlpg_args_t& a, const nnk_mlpg_gv_t* gv, cudaSt
   if constexpr (CAN_AS) {
     staged = (a.win.nw == NW) && !(GRAD && a.go_f64) &&
              as_geometry<AS_TT, AS_NA, AS_NSA1, AS_ND, AS_TTB, NSB>(GRAD ? a.go_ld * 4 : a.in_ld * ES, a.var_ld * ES, GRAD,
-                                                                    L, NT, geom, smem);
+                                                                    L, NT, ES, geom, smem);
     if constexpr (CAN_G2)
       grouped = staged && p.n_groups >= 2 &&
-                as_geometry<AS_TT, AS_NA, AS_NSA2, AS_ND, AS_TTB, NSB, 2>(a.in_ld * ES, a.var_ld * ES, false, L, NT, geom2,
-                                                                          smem2);
+                as_geometry<AS_TT, AS_NA, AS_NSA2, AS_ND, AS_TTB, NSB, 2>(a.in_ld * ES, a.var_ld * ES, false, L, NT, ES,
+                                                                          geom2, smem2);
   }
   const bool stdw = (NW == 3 && L == 1 && U == 1) && is_std_windows(a.win);
   const bool varg = (a.var_ld == 0);

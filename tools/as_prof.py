@@ -59,8 +59,11 @@ def t1000(mode, rhs, o, out_ld):
 
 cases = (("configs[1]", cfg2), ("T1000 forward", lambda: t1000("fwd", None, y2, sd2)),
          ("T1000 gradient", lambda: t1000("grad", go2, g2, 3 * sd2)))
-A_PH = ["wait pb_empty", "wait input TMA", "convert+assemble+publish"]
-S_PH = ["wait pb_full", "eliminate", "wait scratch TMA", "backward"]
+# forward pass phases, then the whole backward pass (forward solves: the segment replay; assemblers
+# >= AS_NA_B only wait at the pass boundary).  Solver: forward pass, then backward: forward solves wait for
+# replayed band rows / replay + back-substitute (waits included); gradients wait for scratch TMA / backward
+A_PH = ["wait pb_empty", "wait input TMA", "convert+assemble+publish", "replay pass (fwd solves)"]
+S_PH = ["wait pb_full", "eliminate", "wait replay rows | scratch TMA", "replay+backward | backward"]
 SLOTS = 40  # NNK_AS_PROF_SLOTS: [role * 4 + phase], [32] CTAs, [33] G, [34] NA
 buf = (ctypes.c_ulonglong * SLOTS)()
 print("%s, per-CTA average cycles of each warp (assembler q.h: tile ownership q of chain group h of the CTA)"
