@@ -320,8 +320,9 @@ int nnk_gmm_map(const nnk_gmm_t* gmm, const double* x, int64_t x_ld, int32_t T, 
  *   E_{m,t} = nu_m + A_m (x_t - mu_m)                    (gmm->tgt_means, gmm->A_t, gmm->src_means; Eq. 22)
  *   lw_{t,m} = lp[t][m] + log_norm[m][e_t] - 1/2 sum_{d in K_t} (Y_t - E_{m,t})_d^2 inv_Dm[m][d]
  * with lp from nnk_gmm_logprob and inv_Dm = 1 / D_m.  Like nnk_mlpg_fwd, which gives the dynamic windows zero
- * precision on the first and last H frames of an utterance (H = max_w max(l_w, u_w)), the columns K_t of frame t
- * are all D columns (e_t = 0) except on those edge frames, where they are the static_dim columns of window 0
+ * precision on the first and last H frames of an utterance (H = max_w max(l_w, u_w)) and on every frame when H = 0
+ * (the reference's precisions[-0:] is the whole column), the columns K_t of frame t are all D columns (e_t = 0)
+ * except on those edge frames, where they are the static_dim columns of window 0
  * (e_t = 1); log_norm[m][e] = -1/2 (sum_{d in K} log D_m,d + |K| log 2 pi) over the same columns.
  *
  * nnk_gmm_traj_em, one CTA per tile of NNK_GMM_TRAJ_TILE frames of one utterance:

@@ -230,7 +230,9 @@ class MLPG(MLPGBase):
         maximum-likelihood conversion over all mixture sequences (Toda, Black & Tokuda 2007, Sec. III).
 
         The trajectory ``c`` maximises ``L(c) = sum_t log sum_m exp(lp[t, m] + log N(Y_t; E_{m,t}, diag D_m))``
-        with ``Y = W c`` its static + dynamic sequence (windows never cross the utterance), ``E_{m,t}`` the
+        with ``Y = W c`` its static + dynamic sequence (windows never cross the utterance; on the first and last
+        ``H = max(l, u)`` frames, and on every frame of a window set with ``H = 0``, only the static columns count,
+        as :func:`~nnmnkwii_b200.paramgen.mlpg` gives the dynamic windows zero precision there), ``E_{m,t}`` the
         Eq. 22 mean, ``D_m`` the diagonal Eq. 23 variances :meth:`transform` uses and
         ``lp[t, m] = log w_m + log N(x_t; mu_m, Sigma_xx,m)``.  EM from ``c_0 = transform(src)``: the E-step
         gives the mixture posteriors ``gamma[t, m]`` of the current trajectory, the M-step is one MLPG solve with

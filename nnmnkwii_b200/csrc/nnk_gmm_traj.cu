@@ -89,14 +89,15 @@ __global__ void __launch_bounds__(TRAJ_WARPS * 32) gmm_traj_em_kernel(const Traj
   }
 
   // mlpg gives the dynamic windows (w >= 1) zero precision on the first and last H frames of an utterance
-  // (H the widest half-width of the set); the model leaves those columns out there as well
+  // (H the widest half-width of the set), and on every frame when H = 0 (the reference's [-0:] slice is the
+  // whole column, as m_edge == 0 in nnk_mlpg.cu); the model leaves those columns out there as well
   int H = 0;
   for (int w = 0; w < a.win.nw; ++w) H = max(H, max(a.win.l[w], a.win.u[w]));
   bool edge[TRAJ_FPW];
 #pragma unroll
   for (int f = 0; f < TRAJ_FPW; ++f) {
     const int t = t0 + warp * TRAJ_FPW + f;
-    edge[f] = (t - ub < H) || (ue - 1 - t < H);
+    edge[f] = (H == 0) || (t - ub < H) || (ue - 1 - t < H);
   }
 
   double mx[TRAJ_FPW], sum[TRAJ_FPW];

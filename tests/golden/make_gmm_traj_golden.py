@@ -18,6 +18,30 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 WINDOWS = [(0, 0, np.array([1.0])), (1, 1, np.array([-0.5, 0.0, 0.5])), (1, 1, np.array([1.0, -2.0, 1.0]))]
 
 
+def em_window_sets():
+    """name -> window set the trajectory-EM tests cover: the reference's test sets with a dynamic window
+    (tests/conftest.py ``windows_set()[1:4]``: half-width 1 with two and three windows, half-width 2), an
+    asymmetric set whose H = 2 comes from ``l`` alone, half-widths 3 and 4, four windows, and a set whose widest
+    half-width is 0 (``mlpg`` then drops the dynamic window on every frame)."""
+    from conftest import windows_set
+    std = windows_set()
+    static = (0, 0, np.array([1.0]))
+    return {
+        "nw2": std[1], "nw3": std[2], "hw2": std[3],
+        "asym": [static, (2, 0, np.array([1.0, -4.0, 3.0]) / 2.0), (0, 1, np.array([-1.0, 1.0]))],
+        "hw3": [static, (3, 3, np.array([-1.0, 9.0, -45.0, 0.0, 45.0, -9.0, 1.0]) / 60.0)],
+        "hw4": [static, (4, 4, np.array([3.0, -32.0, 168.0, -672.0, 0.0, 672.0, -168.0, 32.0, -3.0]) / 840.0),
+                (1, 1, np.array([1.0, -2.0, 1.0]))],
+        "nw4": std[2] + [(2, 2, np.array([1.0, -8.0, 0.0, 8.0, -1.0]) / 12.0)],
+        "h0": [static, (0, 0, np.array([0.5]))],
+    }
+
+
+def half_width(windows):
+    """H = max_w max(l_w, u_w): the number of edge frames at each end of an utterance."""
+    return max(max(int(l), int(u)) for l, u, _ in windows)
+
+
 def cases():
     """(T, static_dim, nw, M, swap, diff) of every stored conversion."""
     return [(60, 2, 2, 4, False, False), (45, 3, 3, 3, True, False), (37, 2, 2, 5, False, True),

@@ -1,6 +1,7 @@
 """Without a GPU: the float64 restatement of the trajectory EM (oracle/gmm_traj_em.py) never lowers its
-objective and starts from the reference's MLPG.transform; the C entry point refuses bad arguments before touching
-the device."""
+objective, starts from the reference's MLPG.transform and, on every window set the GPU tests use, from the C
+restatement of mlpg; its banded path equals its dense one; the C entry point refuses bad arguments before
+touching the device."""
 import ctypes
 import importlib.util
 import os
@@ -40,6 +41,44 @@ def test_oracle_starts_from_the_reference_transform():
         want = golden["y_%d" % i]
         assert c.shape == want.shape == (T, S) and L.shape == (1,)
         assert np.abs(c - want).max() <= 1e-10 * np.abs(want).max(), i
+
+
+SETS = MG.em_window_sets()
+
+
+@pytest.mark.parametrize("name", list(SETS))
+def test_oracle_starts_from_mlpg_and_climbs_on_every_window_set(name):
+    """c_0 is the C restatement's mlpg of the arg-max mixture's E and D_m on every window set (the edge rule is
+    mlpg's, [-0:] included), and the objective never decreases over 20 iterations."""
+    import oracle
+    w = SETS[name]
+    S, M = 3, 6
+    rng = np.random.default_rng(sum(map(ord, name)))
+    g = MG.joint_gmm(rng, M, S * len(w))
+    model = OT.Model(g, w)
+    for T in sorted({1, 2, MG.half_width(w), 2 * MG.half_width(w) + 1, 40} - {0}):
+        src = rng.standard_normal((T, S * len(w)))
+        lp, E = model.frame_terms(src)
+        mix = np.argmax(lp, axis=1)
+        want = oracle.mlpg(E[mix, np.arange(T)], model.Dm[mix], w)
+        c, L = OT.transform_em(g, w, src, 20)
+        assert np.abs(OT.transform_em(g, w, src, 0)[0] - want).max() <= 1e-12 * np.abs(want).max(), T
+        assert L.shape == (21,) and np.all(np.isfinite(L))
+        assert np.all(np.diff(L) >= -1e-12 * np.abs(L[:-1])), (T, np.diff(L).min())
+
+
+@pytest.mark.parametrize("name", ["nw3", "asym", "hw4", "h0"])
+def test_banded_restatement_equals_the_dense_one(name):
+    """The banded path the long-utterance GPU tests use against the dense one, T around the window and beyond."""
+    w = SETS[name]
+    rng = np.random.default_rng(3)
+    g = MG.joint_gmm(rng, 5, 2 * len(w))
+    for T in (1, 2, 5, 150):
+        src = rng.standard_normal((T, 2 * len(w)))
+        cd, Ld = OT.transform_em(g, w, src, 3)
+        cb, Lb = OT.transform_em(g, w, src, 3, banded=True)
+        assert np.abs(cb - cd).max() <= 1e-11 * np.abs(cd).max(), T
+        assert np.all(np.abs(Lb - Ld) <= 1e-12 * np.abs(Ld)), T
 
 
 def _valid_args(_lib):

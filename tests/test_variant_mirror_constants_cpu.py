@@ -1,8 +1,8 @@
 """The constants that tests/variant_mirror.py restates, read out of the CUDA sources (no GPU needed).
 
-The metric, statistics, affine and segment-copy variant tests pick their shapes from the mirror; if one of
-these constants is retuned in a .cu file without the mirror, this test fails instead of the GPU tests
-quietly covering other instances than they say."""
+The metric, statistics, affine, segment-copy and trajectory-EM variant tests pick their shapes from the
+mirror; if one of these constants is retuned in a .cu file without the mirror, this test fails instead of the
+GPU tests quietly covering other instances than they say."""
 import os
 import re
 
@@ -72,3 +72,15 @@ def test_segment_copy_constants():
     src = _function(_source("nnk_shard.cu"), 'extern "C" int nnk_segment_copy(')
     assert re.findall(r"p\.rows_per_block = (\d+);", src) == [str(M.SEG_ROWS_PER_BLOCK)]
     assert M.segment_copy_vec(4, 4, 4, 4, 0, 0) and not M.segment_copy_vec(4, 4, 4, 4, 4, 0)
+
+
+def test_gmm_traj_constants_and_dispatch_rule():
+    src = _source("nnk_gmm_traj.cu")
+    assert _constexpr(src, "TRAJ_MAX_EPL") == M.TRAJ_MAX_EPL
+    with open(os.path.join(os.path.dirname(os.path.dirname(CSRC)), "include", "nnk_b200.h")) as f:
+        assert re.findall(r"#define NNK_GMM_TRAJ_TILE (\d+)", f.read()) == [str(M.NNK_GMM_TRAJ_TILE)]
+    body = _function(src, "static int traj_dispatch(")
+    assert "const int epl = (p.g.D + 31) / 32;" in body
+    assert re.findall(r"if \(epl == (\d)\) return traj_launch<(\d), EM>", body) == [("1", "1"), ("2", "2")]
+    assert "return traj_launch<3, EM>(p, st);" in body
+    assert [M.traj_epl(D) for D in (1, 32, 33, 64, 65, 96)] == [1, 1, 2, 2, 3, 3]

@@ -4,8 +4,8 @@ affine and segment-copy launchers, and a profiler helper that names the CUDA ker
 The mirrors restate, in Python, the size thresholds of the launchers (`pick_instance`, `as_geometry`
 in csrc/nnk_mlpg*.cu*, `dtw_fused_smem` / `dtw_smem_bytes` / `dtw_fast_cells_bound` /
 `dtw_exact_chunk` in csrc/nnk_dtw.cu, `em_layout` / `estep_d` / `mstep_d` in csrc/nnk_gmm_em.cu, the
-launch sizes of csrc/nnk_gmm.cu, `dispatch_frame` in csrc/nnk_metrics.cu, `stats_shape` and
-`launch_affine` in csrc/nnk_stats.cu and the vector test of `nnk_segment_copy` in csrc/nnk_shard.cu).
+launch sizes of csrc/nnk_gmm.cu, `traj_dispatch` in csrc/nnk_gmm_traj.cu, `dispatch_frame` in
+csrc/nnk_metrics.cu, `stats_shape` and `launch_affine` in csrc/nnk_stats.cu and the vector test of `nnk_segment_copy` in csrc/nnk_shard.cu).
 The tests of tests/test_kernel_variants_*_gpu.py and tests/test_variants_*_gpu.py pick their shapes from them and then assert, with the
 profiler, that the kernel the mirror predicts is the one that ran: a later change to a geometry function
 makes those tests fail instead of silently moving their coverage.  tests/test_variant_mirror_constants_cpu.py
@@ -302,6 +302,17 @@ def gmm_logprob_smem(D):
 
 def gmm_posterior_smem(D):
     return 8 * (D * D + GMM_FT * D + 2 * GMM_FT)
+
+
+# ---- GMM trajectory EM (csrc/nnk_gmm_traj.cu) ------------------------------------------------------------------
+TRAJ_MAX_EPL = 3       # D <= 96
+NNK_GMM_TRAJ_TILE = 32  # frames per CTA, one utterance per tile
+
+
+def traj_epl(D):
+    """EPL of the `gmm_traj_em_kernel<EPL, EM>` that `traj_dispatch` launches (output dimensions per lane)."""
+    assert 1 <= D <= 32 * TRAJ_MAX_EPL
+    return (D + 31) // 32
 
 
 # ---- kernel names in a child process -----------------------------------------------------------------------------
