@@ -1,8 +1,8 @@
 """The constants that tests/variant_mirror.py restates, read out of the CUDA sources (no GPU needed).
 
-The metric, statistics, affine, segment-copy and trajectory-EM variant tests pick their shapes from the
-mirror; if one of these constants is retuned in a .cu file without the mirror, this test fails instead of the
-GPU tests quietly covering other instances than they say."""
+The metric, statistics, affine, segment-copy, trajectory-EM and modulation-spectrum variant tests pick their
+shapes from the mirror; if one of these constants is retuned in a .cu file without the mirror, this test fails
+instead of the GPU tests quietly covering other instances than they say."""
 import os
 import re
 
@@ -84,3 +84,37 @@ def test_gmm_traj_constants_and_dispatch_rule():
     assert re.findall(r"if \(epl == (\d)\) return traj_launch<(\d), EM>", body) == [("1", "1"), ("2", "2")]
     assert "return traj_launch<3, EM>(p, st);" in body
     assert [M.traj_epl(D) for D in (1, 32, 33, 64, 65, 96)] == [1, 1, 2, 2, 3, 3]
+
+
+def _declared(src, name):
+    """Value of `name = <int>` in a constexpr declaration that may declare several names."""
+    m = re.findall(r"constexpr\s+int\s+(?:\w+\s*=\s*\d+\s*,\s*)*%s\s*=\s*(\d+)\s*[,;]" % name, src)
+    assert len(m) == 1, (name, m)
+    return int(m[0])
+
+
+def test_modspec_constants_and_dispatch_rule():
+    from nnmnkwii_b200.preprocessing.modspec import NS
+    src = _source("nnk_modspec.cu")
+    assert _constexpr(src, "MS_MAX_THREADS") == M.MS_MAX_THREADS
+    assert (_declared(src, "MS_LOGN_MIN"), _declared(src, "MS_LOGN_MAX")) == (M.MS_LOGN_MIN, M.MS_LOGN_MAX)
+    assert "(1 << (LOGN - 2)) < MS_MAX_THREADS ? (1 << (LOGN - 2)) : MS_MAX_THREADS" in src
+    # every LOGN but the largest has a case of its own; the largest is the default
+    body = _function(src, "static int dispatch_modspec(")
+    cases = re.findall(r"case (\d+): return launch_modspec<T, (\d+), PF>\(a, st\);", body)
+    assert [(int(c), int(l)) for c, l in cases] == [(l, l) for l in range(M.MS_LOGN_MIN, M.MS_LOGN_MAX)]
+    assert re.findall(r"default: return launch_modspec<T, (\d+), PF>\(a, st\);", body) == [str(M.MS_LOGN_MAX)]
+    assert len(re.findall(r"\breturn\b", body)) == len(cases) + 1
+    # the C ABI refuses every other n, and the PF instance takes the modes from NNK_MS_LOGPOWER on
+    entry = _function(src, 'extern "C" int nnk_modspec(')
+    assert "(1 << logn) == n && logn >= MS_LOGN_MIN && logn <= MS_LOGN_MAX" in entry
+    pf = r"if \(mode >= NNK_MS_(\w+)\)\s*return dtype == NNK_F32 \? dispatch_modspec<float, true>"
+    assert re.findall(pf, entry) == ["LOGPOWER"]
+    assert "mode >= NNK_MS_POWER && mode <= NNK_MS_POSTFILTER" in entry
+    with open(os.path.join(os.path.dirname(os.path.dirname(CSRC)), "include", "nnk_b200.h")) as f:
+        modes = {k: int(v) for k, v in re.findall(r"#define NNK_MS_(\w+) (\d+)", f.read())}
+    assert tuple(v for v in sorted(modes.values()) if v >= modes["LOGPOWER"]) == M.MS_PF_MODES
+    assert modes["POSTFILTER"] == max(modes.values())
+    # the Python layer offers exactly the lengths of the instances
+    assert tuple(NS) == tuple(2 ** l for l in range(M.MS_LOGN_MIN, M.MS_LOGN_MAX + 1))
+    assert [M.ms_threads(n) for n in NS] == [64, 128, 256, 256, 256]

@@ -1,11 +1,13 @@
 """Host-side mirrors of the kernel-selection rules of the MLPG, UnitVarianceMLPG, DTW, GMM, metric, statistics,
-affine and segment-copy launchers, and a profiler helper that names the CUDA kernels a call launched.
+affine, segment-copy and modulation-spectrum launchers, and a profiler helper that names the CUDA kernels a call
+launched.
 
 The mirrors restate, in Python, the size thresholds of the launchers (`pick_instance`, `as_geometry`
 in csrc/nnk_mlpg*.cu*, `dtw_fused_smem` / `dtw_smem_bytes` / `dtw_fast_cells_bound` /
 `dtw_exact_chunk` in csrc/nnk_dtw.cu, `em_layout` / `estep_d` / `mstep_d` in csrc/nnk_gmm_em.cu, the
 launch sizes of csrc/nnk_gmm.cu, `traj_dispatch` in csrc/nnk_gmm_traj.cu, `dispatch_frame` in
-csrc/nnk_metrics.cu, `stats_shape` and `launch_affine` in csrc/nnk_stats.cu and the vector test of `nnk_segment_copy` in csrc/nnk_shard.cu).
+csrc/nnk_metrics.cu, `stats_shape` and `launch_affine` in csrc/nnk_stats.cu, the vector test of
+`nnk_segment_copy` in csrc/nnk_shard.cu and `dispatch_modspec` / `ms_threads` in csrc/nnk_modspec.cu).
 The tests of tests/test_kernel_variants_*_gpu.py and tests/test_variants_*_gpu.py pick their shapes from them and then assert, with the
 profiler, that the kernel the mirror predicts is the one that ran: a later change to a geometry function
 makes those tests fail instead of silently moving their coverage.  tests/test_variant_mirror_constants_cpu.py
@@ -422,3 +424,28 @@ def segment_copy_vec(cols, es, src_ld, dst_ld, src_ptr, dst_ptr):
     `segment_copy_kernel<uint32_t>`."""
     row, sp, dp = cols * es, src_ld * es, dst_ld * es
     return row % 16 == 0 and sp % 16 == 0 and dp % 16 == 0 and src_ptr % 16 == 0 and dst_ptr % 16 == 0
+
+
+# ---- modulation spectrum (csrc/nnk_modspec.cu) -------------------------------------------------------------------
+MS_MAX_THREADS = 256
+MS_LOGN_MIN, MS_LOGN_MAX = 8, 12        # n = 256 .. 4096
+MS_PF_MODES = (4, 5)                    # NNK_MS_LOGPOWER, NNK_MS_POSTFILTER: the PF instance
+
+
+def ms_logn(n):
+    """LOGN of the instance `dispatch_modspec` launches for DFT length n (the C ABI refuses every other n)."""
+    logn = int(n).bit_length() - 1
+    assert n == 1 << logn and MS_LOGN_MIN <= logn <= MS_LOGN_MAX, n
+    return logn
+
+
+def ms_threads(n):
+    """Threads per CTA of `modspec_kernel` (`ms_threads<LOGN>`): n / 4, at most MS_MAX_THREADS."""
+    return min(1 << (ms_logn(n) - 2), MS_MAX_THREADS)
+
+
+def modspec_kernel_for(n, dtype, mode):
+    """`modspec_kernel<T, LOGN, PF>` that `nnk_modspec` launches: LOGN = log2 n, PF exactly for the log-power
+    and post-filter modes."""
+    return "modspec_kernel<%s, %d, %s>" % ("float" if _itemsize(dtype) == 4 else "double", ms_logn(n),
+                                           "true" if mode in MS_PF_MODES else "false")
