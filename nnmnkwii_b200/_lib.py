@@ -259,6 +259,12 @@ SIGNATURES = {
 }
 EXPORTS = list(SIGNATURES)
 
+# the segment-level modulation-spectrum kernels (include/nnk_ms_segment.h), in the same library
+NNK_MSSEG_LOGPOWER, NNK_MSSEG_POSTFILTER = 0, 1
+MS_SEGMENT_SIGNATURES = {
+    "nnk_ms_segment": (ctypes.c_int, [i32, i32, i32, i32, vp, vp, vp, i32, i32, i32, vp, vp, vp]),
+}
+
 class NnkError(RuntimeError):
     pass
 
@@ -272,7 +278,7 @@ def _load():
     L.nnk_abi_version.restype = ctypes.c_int
     if L.nnk_abi_version() != ABI_VERSION:
         raise ImportError("libnnk_b200.so ABI %d != binding ABI %d: rebuild" % (L.nnk_abi_version(), ABI_VERSION))
-    for name, (restype, argtypes) in SIGNATURES.items():
+    for name, (restype, argtypes) in list(SIGNATURES.items()) + list(MS_SEGMENT_SIGNATURES.items()):
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, argtypes
     return L

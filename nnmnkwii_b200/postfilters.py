@@ -113,7 +113,7 @@ def _ms_input(x, n, lengths):
     return B, T, D, lens
 
 
-def modspec_statistics(x, n=4096, lengths=None):
+def modspec_statistics(x, n=4096, lengths=None, segment=None):
     """Statistics of the log modulation spectrum over a set of utterances, for :func:`modspec_post_filter`.
 
     For each utterance and feature column, ``s_j = log(max(|rfft(x[:, d], n)_j|^2, tiny))`` (natural log; ``tiny``
@@ -128,14 +128,27 @@ def modspec_statistics(x, n=4096, lengths=None):
 
     Pass the columns you will filter, typically ``mgc[:, 1:]``: the power coefficient (column 0) is usually left
     alone.  Compute the natural statistics on natural speech and the generated ones on the model's output for
-    the same kind of utterances, with the same ``n``.
+    the same kind of utterances, with the same ``n`` (and the same ``segment``).
+
+    **Segment level** (``segment=L``, the paper's other variant).  Each utterance of ``T`` frames is cut into
+    ``J = ceil(T / H) + 1`` overlapping segments (none when ``T = 0``) with the hop ``H = L / 2``: segment ``j``
+    starts at frame ``(j - 1) H`` and frames outside ``[0, T)`` are 0, so every frame lies in exactly two
+    segments, and the first and last segments lie half outside the utterance (they count like any other).  Each
+    segment is windowed with the periodic Hann window ``w_m = 0.5 - 0.5 cos(2 pi m / L)``, and ``s_j`` is the log
+    power of ``rfft(w * segment, n)``.  ``mean`` and ``var`` are taken over all segments of all utterances, so
+    utterances of any length count, and a corpus gives many more samples per bin than at the utterance level.
+    The statistics have the same shape as utterance-level statistics of the same ``n``: nothing tells the two
+    apart, so keep track of which kind you computed.  The temporary holds every segment's log power,
+    ``S * (n // 2 + 1) * D`` elements for ``S`` segments in all.
 
     Args:
         x: ``(T, D)`` trajectory (one utterance) or a padded ``(B, T, D)`` batch; float32 / float64 CUDA tensor or
             NumPy array (a CPU tensor is refused).
-        n (int): DFT length, 256, 512, 1024, 2048 or 4096, at least every utterance's length.
+        n (int): DFT length, 256, 512, 1024, 2048 or 4096, at least every utterance's length; with ``segment``,
+            the per-segment DFT length, 32, 64, 128, 256 or 512.
         lengths: with a ``(B, T, D)`` ``x``, frames of each utterance (default: ``T``); frames past a length are
             never read.
+        segment (int): ``None`` for the utterance level, or the segment length ``L``, even, ``4 <= L <= n``.
 
     Returns:
         ``(mean, var)``, each float64 of shape ``(n // 2 + 1, D)``: NumPy arrays for NumPy ``x``, tensors on
@@ -143,13 +156,17 @@ def modspec_statistics(x, n=4096, lengths=None):
 
     Raises:
         ValueError: ``n`` not supported, an utterance longer than ``n``, no utterance, or an utterance of no
-            frames (it has no modulation spectrum), all before any device work.
+            frames (it has no modulation spectrum), all before any device work.  With ``segment``: an ``n`` or
+            ``L`` not supported, or a set without a segment (zero-length utterances are skipped); a ``segment``
+            that is not an int is a TypeError.
     """
     import torch
 
     from . import _device as dev
     from . import _lib
     from .preprocessing.modspec import _device_input, _launch
+    if segment is not None:
+        return _segment_statistics(x, n, lengths, segment)
     B, T, D, lens = _ms_input(x, n, lengths)
     if B == 0:
         raise ValueError("modspec_statistics needs at least one utterance")
@@ -202,7 +219,7 @@ def _ms_table(natural, generated, k, K, D, dtype):
     return np.stack([(1.0 - k) + k * g, k * (mu_n - g * mu_g)], axis=-1).astype(dtype)
 
 
-def modspec_post_filter(x, natural, generated, k=1.0, n=4096, lengths=None):
+def modspec_post_filter(x, natural, generated, k=1.0, n=4096, lengths=None, segment=None):
     """Modulation-spectrum (MS) post-filter of Takamichi et al., "A postfilter to modify the modulation spectrum
     in HMM-based speech synthesis", ICASSP 2014, at the utterance level, on the GPU.
 
@@ -220,8 +237,8 @@ def modspec_post_filter(x, natural, generated, k=1.0, n=4096, lengths=None):
     back to rounding.
 
     Deliberate choices:
-      * utterance level only: the filter sees each utterance's whole MS; the segment-level variant of the paper
-        is not offered;
+      * utterance level by default: the filter sees each utterance's whole MS; ``segment=L`` selects the
+        segment-level variant below;
       * bin 0 is not filtered (``C_0 = Y_0``): it is ``T`` times the column's mean, which the acoustic model sets,
         not modulation, so each column keeps its level.  A bin of zero power stays 0, so an all-zero column comes
         out all zero;
@@ -239,6 +256,21 @@ def modspec_post_filter(x, natural, generated, k=1.0, n=4096, lengths=None):
     Pass the columns the statistics were computed on, typically ``mgc[:, 1:]`` (leave the power coefficient
     alone).
 
+    **Segment level** (``segment=L``).  The utterance is cut into the windowed segments of
+    :func:`modspec_statistics` (hop ``H = L / 2``, periodic Hann window ``w``, segment ``j`` from frame
+    ``(j - 1) H``, ``J = ceil(T / H) + 1`` of them), each segment's spectrum ``Y_j = rfft(w * segment, n)`` is
+    filtered bin by bin as above, and the result is overlap-added without a synthesis window::
+
+        y_t = sum_j irfft(C_j, n)[t - (j - 1) H]     over the j with 0 <= t - (j - 1) H < L
+
+    For this window ``w_m + w_{m + H} = 1``, so ``k = 0`` or equal statistics give ``x`` back to rounding.
+    There is no limit on the utterance's length, and the cost grows with its frames, not with the longest
+    utterance of the batch.  The first and last segments lie half outside the utterance and are filtered like
+    the others.  Use statistics computed with the same ``n`` and ``segment``: segment-level and utterance-level
+    statistics of one ``n`` have the same shape, so the shape check cannot tell them apart.  Runs on the GPU
+    (``nnk_ms_segment``, csrc/nnk_ms_segment.cu): one CTA per (utterance, tile of frames, group of columns)
+    filters every segment of its tile, one warp per (segment, column), and overlap-adds them in shared memory.
+
     Args:
         x: ``(T, D)`` trajectory or a padded ``(B, T, D)`` batch; float32 / float64 CUDA tensor or NumPy array (a
             CPU tensor is refused).
@@ -247,23 +279,27 @@ def modspec_post_filter(x, natural, generated, k=1.0, n=4096, lengths=None):
         generated: ``(mean, var)`` of generated speech, likewise.
         k (float): emphasis weight in ``[0, 1]``; 1 replaces the MS statistics completely.
         n (int): DFT length, 256, 512, 1024, 2048 or 4096, at least every utterance's length; the ``n`` of the
-            statistics.
+            statistics.  With ``segment``: the per-segment DFT length, 32, 64, 128, 256 or 512.
         lengths: with a ``(B, T, D)`` ``x``, frames of each utterance (default: ``T``).
+        segment (int): ``None`` for the utterance level, or the segment length ``L``, even, ``4 <= L <= n``.
 
     Returns:
         The filtered trajectories: ``x``'s shape and dtype, NumPy for NumPy ``x``, a tensor on ``x``'s device
         otherwise.
 
     Raises:
-        ValueError: for any of the range checks above, an ``n`` not supported, an utterance longer than ``n``, or
-            statistics of the wrong shape; TypeError for inputs that are not float arrays.  Argument errors are
-            raised before any device work.
+        ValueError: for any of the range checks above, an ``n`` not supported, an utterance longer than ``n``
+            (utterance level only), a ``segment`` length not supported, or statistics of the wrong shape;
+            TypeError for inputs that are not float arrays or a ``segment`` that is not an int.  Argument errors
+            are raised before any device work.
     """
     import torch
 
     from . import _device as dev
     from . import _lib
     from .preprocessing.modspec import _device_input, _launch, _out
+    if segment is not None:
+        return _segment_post_filter(x, natural, generated, k, n, lengths, segment)
     B, T, D, lens = _ms_input(x, n, lengths)
     k = float(k)
     if not 0.0 <= k <= 1.0:
@@ -273,4 +309,85 @@ def modspec_post_filter(x, natural, generated, k=1.0, n=4096, lengths=None):
     out = torch.empty_like(xt)
     _launch(_lib.NNK_MS_POSTFILTER, n, xt, dev.to_device(table, xt.device), out, None, B, T, T, D, lens, 1.0,
             1.0 / n)
+    return _out(out, x, x.ndim == 2)
+
+
+# ---- segment level (csrc/nnk_ms_segment.cu) ------------------------------------------------------------------------
+SEGMENT_NS = (32, 64, 128, 256, 512)
+
+
+def _segment_input(x, n, lengths, segment):
+    """(B, T, D, host lengths or None, L) of a segment-level call; argument errors only."""
+    from .preprocessing.modspec import _batch, _checked
+    _checked(x, "x")
+    if n not in SEGMENT_NS:
+        raise ValueError("with segment, n must be one of %s, got %r" % (", ".join(map(str, SEGMENT_NS)), n))
+    if isinstance(segment, bool) or not isinstance(segment, (int, np.integer)):
+        raise TypeError("segment must be an int (the segment length L) or None, got %s" % type(segment).__name__)
+    L = int(segment)
+    if L % 2 or not 4 <= L <= n:
+        raise ValueError("segment length must be even with 4 <= L <= n = %d, got %d" % (n, L))
+    B, T, D, lens, _ = _batch(x, lengths)
+    return B, T, D, lens, L
+
+
+def _segment_counts(lengths, L):
+    """Segments ``ceil(T / (L / 2)) + 1`` of each length ``T`` (0 for ``T = 0``), int64."""
+    lens = np.asarray(lengths, np.int64)
+    H = L // 2
+    return np.where(lens > 0, -(-lens // H) + 1, 0)
+
+
+def _segment_launch(mode, n, L, xt, table, out, B, T, D, lens, seg_off=None):
+    """Enqueue nnk_ms_segment on the current stream of ``out``'s device."""
+    from . import _device as dev
+    from . import _lib
+    lt = dev.lengths_on(lens, out.device)
+    _lib.check(_lib.lib.nnk_ms_segment(mode, dev.torch_dtype_code(xt.dtype), n, L, xt.data_ptr(),
+                                       table.data_ptr() if table is not None else None, out.data_ptr(), B, T, D,
+                                       lt.data_ptr() if lt is not None else None, seg_off.data_ptr() if seg_off is not None else None,
+                                       dev.current_stream_ptr(out.device)), "nnk_ms_segment")
+
+
+def _segment_statistics(x, n, lengths, segment):
+    import torch
+
+    from . import _device as dev
+    from . import _lib
+    from .preprocessing.modspec import _device_input
+    B, T, D, lens, L = _segment_input(x, n, lengths, segment)
+    J = _segment_counts(np.full(B, T) if lens is None else lens, L)
+    S = int(J.sum())
+    if S == 0:
+        raise ValueError("modspec_statistics needs at least one segment (every utterance has zero frames)")
+    K = n // 2 + 1
+    xt = _device_input(x, B, T, D)
+    device = xt.device
+    mean = torch.empty((D, K), dtype=torch.float64, device=device)
+    var = torch.empty((D, K), dtype=torch.float64, device=device)
+    if D:
+        logms = torch.empty((S, D, K), dtype=xt.dtype, device=device)
+        seg_off = torch.as_tensor(np.concatenate([[0], np.cumsum(J)[:-1]]).astype(np.int64), device=device)
+        _segment_launch(_lib.NNK_MSSEG_LOGPOWER, n, L, xt, None, logms, B, T, D, lens, seg_off)
+        off = torch.tensor([0, S], dtype=torch.int64, device=device)  # one segment of S rows and D * K columns
+        _lib.check(_lib.lib.nnk_segment_moments(logms.data_ptr(), dev.torch_dtype_code(logms.dtype), D * K, D * K,
+                                                off.data_ptr(), None, 1, mean.data_ptr(), var.data_ptr(),
+                                                dev.current_stream_ptr(device)), "nnk_segment_moments")
+    return dev.like_input(mean.t().contiguous(), x), dev.like_input(var.t().contiguous(), x)
+
+
+def _segment_post_filter(x, natural, generated, k, n, lengths, segment):
+    import torch
+
+    from . import _device as dev
+    from . import _lib
+    from .preprocessing.modspec import _device_input, _out
+    B, T, D, lens, L = _segment_input(x, n, lengths, segment)
+    k = float(k)
+    if not 0.0 <= k <= 1.0:
+        raise ValueError("k must be in [0, 1], got %r" % k)
+    table = _ms_table(natural, generated, k, n // 2 + 1, D, dev.np_dtype(x))
+    xt = _device_input(x, B, T, D)
+    out = torch.empty_like(xt)
+    _segment_launch(_lib.NNK_MSSEG_POSTFILTER, n, L, xt, dev.to_device(table, xt.device), out, B, T, D, lens)
     return _out(out, x, x.ndim == 2)
