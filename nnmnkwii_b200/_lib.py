@@ -265,6 +265,13 @@ MS_SEGMENT_SIGNATURES = {
     "nnk_ms_segment": (ctypes.c_int, [i32, i32, i32, i32, vp, vp, vp, i32, i32, i32, vp, vp, vp]),
 }
 
+# parameter generation considering the modulation spectrum (include/nnk_ms_gen.h), in the same library; the
+# nnk_mlpg_ms_t argument is passed by reference to paramgen's ctypes mirror of it
+MS_GEN_SIGNATURES = {
+    "nnk_mlpg_ms": (ctypes.c_int, [P(NnkMlpgArgs), vp, vp]),
+    "nnk_mlpg_ms_workspace_bytes": (size_t, [i32, i32, i32, i64, i64, P(NnkWindows)]),
+}
+
 class NnkError(RuntimeError):
     pass
 
@@ -278,7 +285,8 @@ def _load():
     L.nnk_abi_version.restype = ctypes.c_int
     if L.nnk_abi_version() != ABI_VERSION:
         raise ImportError("libnnk_b200.so ABI %d != binding ABI %d: rebuild" % (L.nnk_abi_version(), ABI_VERSION))
-    for name, (restype, argtypes) in list(SIGNATURES.items()) + list(MS_SEGMENT_SIGNATURES.items()):
+    for name, (restype, argtypes) in (list(SIGNATURES.items()) + list(MS_SEGMENT_SIGNATURES.items()) +
+                                      list(MS_GEN_SIGNATURES.items())):
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, argtypes
     return L

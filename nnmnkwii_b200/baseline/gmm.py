@@ -22,7 +22,7 @@ import numpy as np
 from scipy import linalg
 from sklearn.mixture import GaussianMixture as _SkGaussianMixture
 
-from ..paramgen import mlpg_batch, mlpg_gv_batch
+from ..paramgen import mlpg_batch, mlpg_gv_batch, mlpg_ms_batch
 
 
 def _compute_precision_cholesky_full(covariances):
@@ -171,9 +171,15 @@ class MLPG(MLPGBase):
             :func:`nnmnkwii_b200.paramgen.mlpg_gv_batch` (Toda, Black & Tokuda 2007, Sec. IV) instead of
             plain MLPG.  Not defined for ``diff=True`` (``ValueError``), and not applied on the
             posterior-mean path (source features of ``static_dim`` columns), which runs no MLPG.
+        ms (tuple): additive: ``(ms_mean, ms_var)``, statistics of the log modulation spectrum of the target's
+            static features, each ``(n // 2 + 1, static_dim)`` (e.g.
+            :func:`nnmnkwii_b200.postfilters.modspec_statistics` of natural static trajectories).  When given,
+            :meth:`transform` and :meth:`transform_batch` generate with
+            :func:`nnmnkwii_b200.paramgen.mlpg_ms_batch` instead of plain MLPG.  ``ValueError`` together with
+            ``gv``, with ``diff=True`` and for :meth:`transform_em`; not applied on the posterior-mean path.
     """
 
-    def __init__(self, gmm, windows=None, swap=False, diff=False, gv=None):
+    def __init__(self, gmm, windows=None, swap=False, diff=False, gv=None, ms=None):
         super(MLPG, self).__init__(gmm, swap, diff)
         if windows is None:
             windows = [(0, 0, np.array([1.0])), (1, 1, np.array([-0.5, 0.0, 0.5]))]
@@ -187,8 +193,20 @@ class MLPG(MLPGBase):
             from ..paramgen import StreamLayout, _gv_args
             _gv_args(gv_mean, gv_var, StreamLayout.single(self.static_dim * len(windows), len(windows)), 0, 1.0, None)
             self.gv = (gv_mean, gv_var)
+        self.ms = None
+        if ms is not None:
+            if gv is not None:
+                raise ValueError("ms and gv cannot be combined")
+            if diff:
+                raise ValueError("ms is not defined for difference features (diff=True)")
+            from ..paramgen import StreamLayout, _ms_args
+            ms_mean, ms_var = _ms_args(ms[0], ms[1], StreamLayout.single(self.static_dim * len(windows), len(windows)),
+                                       0, 1.0, None)[:2]
+            self.ms = (ms_mean, ms_var)
 
     def _generate(self, E, Dv, lengths):
+        if self.ms is not None:
+            return mlpg_ms_batch(E, Dv, self.windows, self.ms[0], self.ms[1], lengths=lengths)
         if self.gv is None:
             return mlpg_batch(E, Dv, self.windows, lengths=lengths)
         return mlpg_gv_batch(E, Dv, self.windows, self.gv[0], self.gv[1], lengths=lengths)
@@ -330,6 +348,8 @@ class MLPG(MLPGBase):
         """The arguments :meth:`transform_em_batch` refuses, before anything is launched; returns ``n_iter``."""
         if self.gv is not None:
             raise ValueError("transform_em does not combine EM with global variance (gv is set)")
+        if self.ms is not None:
+            raise ValueError("transform_em does not combine EM with the modulation spectrum (ms is set)")
         D = self.src_means.shape[1]
         for s in srcs:
             if s.ndim != 2:

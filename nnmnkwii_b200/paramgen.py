@@ -21,6 +21,9 @@ streams in Python): :class:`StreamLayout`, :func:`merlin_layout`, :func:`mlpg_ba
 Additive, parameter generation considering global variance (Toda, Black & Tokuda 2007, Sec. IV):
 :func:`mlpg_gv`, :func:`mlpg_gv_batch` and the GV statistics :func:`global_variance`,
 :func:`gv_statistics` (csrc/nnk_mlpg.cu ``nnk_mlpg_gv``, csrc/nnk_stats.cu ``nnk_segment_moments``).
+
+Additive, parameter generation considering the modulation spectrum (DESIGN.md 3.18): :func:`mlpg_ms`,
+:func:`mlpg_ms_batch` (csrc/nnk_ms_gen.cu ``nnk_mlpg_ms``, C ABI include/nnk_ms_gen.h).  Not in ``__all__``.
 """
 import ctypes
 
@@ -431,6 +434,223 @@ def gv_statistics(x, lengths=None, offsets=None):
     _, gv = _moments(x, lengths, offsets, False)
     mean, var = _moments(gv, None, None, True)
     return dev.like_input(mean[0], x), dev.like_input(var[0], x)
+
+
+# ---------------------------------------------------------------------------------------------------
+# modulation spectrum (additive)
+# ---------------------------------------------------------------------------------------------------
+class _NnkMlpgMs(ctypes.Structure):
+    """ctypes mirror of ``nnk_mlpg_ms_t`` (include/nnk_ms_gen.h)."""
+    _fields_ = [
+        ("ms_mean", ctypes.c_void_p),
+        ("ms_var", ctypes.c_void_p),
+        ("n", ctypes.c_int32),
+        ("n_iter", ctypes.c_int32),
+        ("step", ctypes.c_double),
+        ("weight", ctypes.c_double),
+        ("n_rows", ctypes.c_int64),
+    ]
+
+
+_MS_GEN_N = (256, 512, 1024, 2048, 4096)
+
+
+def _ms_args(ms_mean, ms_var, layout, n_iter, step, weight):
+    """Checked MS parameters ``(ms_mean, ms_var, n, n_iter, step, weight)``: float64 host ``(K, layout.D_out)``
+    arrays (``weight`` 0 = the default ``1 / (nw T)``).  Columns of copied chains are not used and not checked;
+    they are set to ``(0, inf)``."""
+    from ._device import is_tensor
+    arrs = []
+    for name, a in (("ms_mean", ms_mean), ("ms_var", ms_var)):
+        if is_tensor(a):
+            a = a.detach().cpu().numpy()
+        try:
+            a = np.array(a, dtype=np.float64)
+        except (TypeError, ValueError):
+            raise ValueError("%s must be an array of numbers" % name)
+        if a.ndim != 2 or a.shape[1] != layout.D_out:
+            raise ValueError("%s must be (n // 2 + 1, %d), got shape %s" % (name, layout.D_out, a.shape))
+        arrs.append(a)
+    mm, mv = arrs
+    if mm.shape != mv.shape:
+        raise ValueError("ms_mean and ms_var differ in shape: %s, %s" % (mm.shape, mv.shape))
+    n = 2 * (mm.shape[0] - 1)
+    if n not in _MS_GEN_N:
+        raise ValueError("ms_mean / ms_var have %d bins: n = 2 (K - 1) = %d must be one of 256, 512, 1024, 2048, "
+                         "4096" % (mm.shape[0], n))
+    used = np.unique(layout.chains["out_col"][layout.chains["flags"] == 0])
+    unused = np.setdiff1d(np.arange(layout.D_out), used)
+    v, m = mv[:, used], mm[:, used]
+    if np.any(np.isnan(v)) or np.any(v <= 0):
+        raise ValueError("ms_var must be > 0 (inf exempts a bin), not NaN")
+    if not np.all(np.isfinite(m[np.isfinite(v)])):
+        raise ValueError("ms_mean must be finite where ms_var is finite")
+    if isinstance(n_iter, bool) or int(n_iter) != n_iter or n_iter < 0:
+        raise ValueError("n_iter must be an integer >= 0, got %r" % (n_iter,))
+    if not (np.isfinite(step) and step > 0):
+        raise ValueError("step must be finite and > 0, got %r" % (step,))
+    if weight is not None and not (np.isfinite(weight) and weight > 0):
+        raise ValueError("weight must be finite and > 0 (or None), got %r" % (weight,))
+    mm[:, unused] = 0.0
+    mv[:, unused] = np.inf
+    return mm, mv, n, int(n_iter), float(step), 0.0 if weight is None else float(weight)
+
+
+def _ms_lengths(means, lengths, offsets, padded):
+    """Host frame counts of the utterances of a batch (argument errors as ``ValueError``)."""
+    from . import _device as dev
+    if padded:
+        lens = dev.check_lengths(lengths, means.shape[0])
+        if lens.size and int(lens.max()) > means.shape[1]:
+            raise ValueError("lengths exceed Tmax = %d" % means.shape[1])
+        return lens
+    n_rows = means.shape[0]
+    if offsets is not None:
+        off = np.asarray(offsets.cpu().numpy() if dev.is_tensor(offsets) else offsets, dtype=np.int64)
+        if off.ndim != 1 or len(off) < 1 or off[0] != 0 or off[-1] != n_rows or np.any(np.diff(off) < 0):
+            raise ValueError("offsets must rise from 0 to %d" % n_rows)
+        return np.diff(off)
+    if lengths is not None:
+        lens = dev.check_lengths(lengths, len(lengths))
+        if int(lens.sum()) != n_rows:
+            raise ValueError("lengths sum to %d, means have %d rows" % (lens.sum(), n_rows))
+        return lens
+    return np.array([n_rows], dtype=np.int64)
+
+
+def mlpg_ms_batch(means, variances, windows, ms_mean, ms_var, lengths=None, offsets=None, layout=None, n_iter=20,
+                  step=1.0, weight=None, check=True, out=None):
+    r"""Batched parameter generation considering the modulation spectrum (additive API).
+
+    Per utterance and smoothed output column ``s``, with ``Y = rfft(c, n)`` and
+    :math:`s_k(c) = \log \max(|Y_k|^2, \mathrm{tiny})` (what :func:`~nnmnkwii_b200.postfilters.modspec_statistics`
+    averages), maximises
+
+    .. math:: F(c) = \omega (b^T c - \tfrac12 c^T P c) - \tfrac12 \sum_{k=1}^{n/2} q_k (s_k(c) - \nu_k)^2,
+              \quad \nu_k = \mathrm{ms\_mean}[k, s], \; q_k = 1 / \mathrm{ms\_var}[k, s]
+
+    from the :func:`mlpg_batch` trajectory :math:`c_m = P^{-1} b`.  Each of the ``n_iter`` trials takes the
+    step ``alpha * ((c_m - c) + P^-1 g / omega)`` (``g`` the gradient of the MS term) and keeps it when
+    :math:`F` does not decrease, otherwise halves ``alpha`` (which starts at ``step``), so ``F`` never falls
+    below :math:`F(c_m)` and ``n_iter = 0`` is plain MLPG.  Bin 0 has no term (the model sets the level); a bin
+    with ``ms_var = inf`` has none either, which is how a column (e.g. the power coefficient) is left alone.
+    This follows the idea of Takamichi et al. (ICASSP 2015) with the project's own step rule (DESIGN.md 3.18);
+    nobody has measured the output quality at the default ``n_iter`` and ``step``.
+
+    Args:
+        means, variances, windows, lengths, offsets, layout, check: as :func:`mlpg_batch` (flat or padded,
+            per-frame or global ``(D,)`` variances, NumPy arrays or torch CUDA tensors).
+        ms_mean, ms_var: ``(K, layout.D_out)`` statistics of the log modulation spectrum, e.g.
+            :func:`~nnmnkwii_b200.postfilters.modspec_statistics` of natural static trajectories; the DFT length
+            ``n = 2 (K - 1)`` is 256, 512, 1024, 2048 or 4096 and at least every utterance's length.
+            ``ms_var > 0`` (``inf`` exempts the bin); ``ms_mean`` finite where ``ms_var`` is.  Copied columns
+            (Merlin's vuv) ignore theirs.
+        n_iter: trials (``>= 0``).
+        step: initial step ``alpha`` (``> 0``).
+        weight: :math:`\omega` (``> 0``); default ``1 / (num_windows * T)`` per utterance.
+        out: optional ``(sum_T, D_out)`` NumPy buffer of the working dtype (flat host form only).
+
+    Returns:
+        Trajectories shaped and typed like :func:`mlpg_batch`'s.  Arithmetic is float64 (float32 inputs are
+        widened once on the device).  Every argument error is a ``ValueError`` raised before any launch.
+    """
+    import torch
+
+    from . import _device as dev
+    if means.ndim not in (2, 3):
+        raise ValueError("means must be (sum_T, D) or (B, Tmax, D)")
+    padded = means.ndim == 3
+    D = means.shape[-1]
+    if layout is None:
+        layout = StreamLayout.single(D, len(windows))
+    if layout.D_in != D:
+        raise ValueError("layout covers %d input columns, means have %d" % (layout.D_in, D))
+    if padded and lengths is None:
+        raise ValueError("padded (B, Tmax, D) input needs lengths")
+    ms = _ms_args(ms_mean, ms_var, layout, n_iter, step, weight)
+    lens = _ms_lengths(means, lengths, offsets, padded)
+    if lens.size and int(lens.max()) > ms[2]:
+        raise ValueError("an utterance of %d frames is longer than the DFT length n = %d" % (lens.max(), ms[2]))
+    if dev.is_tensor(means):
+        return _mlpg_ms_device(means, variances, windows, lengths, offsets, layout, padded, check, ms)
+    dtype = np.asarray(means).dtype
+    v_np = np.asarray(variances)
+    work = dtype if (dtype in (np.float32, np.float64) and v_np.dtype == dtype) else np.dtype(np.float64)
+    dev.require_cuda()
+    device = dev.cuda_device()
+    m = torch.from_numpy(np.ascontiguousarray(means, dtype=work)).to(device)
+    v = torch.from_numpy(np.ascontiguousarray(v_np, dtype=work)).to(device)
+    y = _mlpg_ms_device(m, v, windows, lengths, offsets, layout, padded, check, ms).cpu().numpy()
+    if out is not None:
+        if padded or out.shape != y.shape or out.dtype != work or not out.flags.c_contiguous:
+            raise ValueError("out must be a C-contiguous %s array of dtype %s" % (y.shape, work))
+        out[...] = y
+        y = out
+    return y if y.dtype == dtype else y.astype(dtype)
+
+
+def _mlpg_ms_device(means, variances, windows, lengths, offsets, layout, padded, check, ms):
+    import torch
+
+    from . import _device as dev
+
+    dev.require_cuda()
+    assert means.is_cuda, "torch inputs must be CUDA tensors (no CPU fallback)"
+    dev.poll_errors()
+    n_rows = means.shape[0] * means.shape[1] if padded else means.shape[0]
+    off, lens, order, max_T, n_utt = _utterance_table(lengths, offsets, n_rows, means.shape[:2] if padded else None)
+    device = means.device
+    dtype = means.dtype
+    m = means.to(torch.float64).contiguous()  # float32 inputs are widened once; all arithmetic is float64
+    v = variances.to(device=device, dtype=torch.float64)
+    var1d = v.dim() == 1
+    D = m.shape[-1]
+    v = v.contiguous() if var1d else (v.expand_as(m).contiguous() if v.shape != m.shape else v.contiguous())
+    out = torch.zeros((n_rows, layout.D_out), dtype=torch.float64, device=device)
+    if n_utt and max_T and layout.n_chain:
+        wc = _lib.make_windows(windows)
+        need = _lib.lib.nnk_mlpg_ms_workspace_bytes(n_utt, layout.n_chain, max_T, n_rows, layout.D_out,
+                                                    ctypes.byref(wc))
+        if need == 0:
+            raise NotImplementedError("window set not supported by the CUDA kernels")
+        ws = dev.workspace(device, need)
+        status = torch.zeros(1, dtype=torch.int64, device=device)
+        offsets_d = torch.from_numpy(off).to(device)
+        lengths_d = dev.lengths_on(lens, device) if padded else None
+        order_d = torch.from_numpy(order).to(device)
+        chains_d = dev.chains_on_device(layout.chains, device)
+        mean_d = torch.from_numpy(np.ascontiguousarray(ms[0])).to(device)
+        var_d = torch.from_numpy(np.ascontiguousarray(ms[1])).to(device)
+        a = _lib.NnkMlpgArgs()
+        a.means, a.vars, a.grad_out, a.out = m.data_ptr(), v.data_ptr(), None, out.data_ptr()
+        a.dtype, a.n_utt = _lib.NNK_F64, n_utt
+        a.in_ld, a.var_ld, a.go_ld, a.out_ld = D, 0 if var1d else D, 0, layout.D_out
+        a.utt_off, a.utt_len, a.order = offsets_d.data_ptr(), lengths_d.data_ptr() if padded else None, order_d.data_ptr()
+        a.chains, a.n_chain, a.max_T, a.go_f64, a.win = chains_d.data_ptr(), layout.n_chain, max_T, 0, wc
+        a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
+        a.status_word, a.out_off = status.data_ptr(), None
+        p = _NnkMlpgMs()
+        p.ms_mean, p.ms_var, p.n, p.n_iter, p.step, p.weight = (mean_d.data_ptr(), var_d.data_ptr(), ms[2], ms[3],
+                                                                ms[4], ms[5])
+        p.n_rows = n_rows
+        _lib.check(_lib.lib.nnk_mlpg_ms(ctypes.byref(a), ctypes.byref(p), dev.current_stream_ptr(device)),
+                   "nnk_mlpg_ms")
+        if check == "deferred":
+            dev._defer_check(status, device)
+        elif check:
+            dev.raise_if_failed(status)
+    if padded:
+        out = out.reshape(m.shape[0], m.shape[1], layout.D_out)
+    return out if dtype == torch.float64 else out.to(dtype)
+
+
+def mlpg_ms(mean_frames, variance_frames, windows, ms_mean, ms_var, n_iter=20, step=1.0, weight=None):
+    """Parameter generation considering the modulation spectrum for one utterance, ``(T, D) -> (T, static_dim)``:
+    :func:`mlpg`'s arguments plus the MS parameters of :func:`mlpg_ms_batch` (``ms_mean`` / ``ms_var`` of shape
+    ``(n // 2 + 1, static_dim)``).  NumPy in, NumPy out (a CUDA tensor stays a CUDA tensor)."""
+    T, D = mean_frames.shape
+    return mlpg_ms_batch(mean_frames, variance_frames, windows, ms_mean, ms_var, lengths=[T], n_iter=n_iter,
+                         step=step, weight=weight)
 
 
 # ---------------------------------------------------------------------------------------------------
