@@ -259,10 +259,12 @@ SIGNATURES = {
 }
 EXPORTS = list(SIGNATURES)
 
-# the segment-level modulation-spectrum kernels (include/nnk_ms_segment.h), in the same library
+# the segment-level modulation-spectrum kernels (include/nnk_ms_segment.h), in the same library; the
+# nnk_mlpg_ms_t argument of nnk_mlpg_ms_segment is passed by reference to paramgen's ctypes mirror of it
 NNK_MSSEG_LOGPOWER, NNK_MSSEG_POSTFILTER = 0, 1
 MS_SEGMENT_SIGNATURES = {
     "nnk_ms_segment": (ctypes.c_int, [i32, i32, i32, i32, vp, vp, vp, i32, i32, i32, vp, vp, vp]),
+    "nnk_mlpg_ms_segment": (ctypes.c_int, [P(NnkMlpgArgs), vp, i32, vp]),
 }
 
 # parameter generation considering the modulation spectrum (include/nnk_ms_gen.h), in the same library; the

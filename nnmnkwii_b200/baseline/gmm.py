@@ -177,9 +177,12 @@ class MLPG(MLPGBase):
             :meth:`transform` and :meth:`transform_batch` generate with
             :func:`nnmnkwii_b200.paramgen.mlpg_ms_batch` instead of plain MLPG.  ``ValueError`` together with
             ``gv``, with ``diff=True`` and for :meth:`transform_em`; not applied on the posterior-mean path.
+        ms_segment (int): additive: the segment length ``L`` of a segment-level ``ms``
+            (``mlpg_ms_batch(..., segment=L)``, statistics from ``modspec_statistics(..., segment=L)`` with
+            ``n`` 32 .. 512), for utterances of any length.  ``ValueError`` without ``ms``.
     """
 
-    def __init__(self, gmm, windows=None, swap=False, diff=False, gv=None, ms=None):
+    def __init__(self, gmm, windows=None, swap=False, diff=False, gv=None, ms=None, ms_segment=None):
         super(MLPG, self).__init__(gmm, swap, diff)
         if windows is None:
             windows = [(0, 0, np.array([1.0])), (1, 1, np.array([-0.5, 0.0, 0.5]))]
@@ -194,6 +197,9 @@ class MLPG(MLPGBase):
             _gv_args(gv_mean, gv_var, StreamLayout.single(self.static_dim * len(windows), len(windows)), 0, 1.0, None)
             self.gv = (gv_mean, gv_var)
         self.ms = None
+        self.ms_segment = None
+        if ms_segment is not None and ms is None:
+            raise ValueError("ms_segment needs ms (segment-level MS statistics)")
         if ms is not None:
             if gv is not None:
                 raise ValueError("ms and gv cannot be combined")
@@ -201,12 +207,14 @@ class MLPG(MLPGBase):
                 raise ValueError("ms is not defined for difference features (diff=True)")
             from ..paramgen import StreamLayout, _ms_args
             ms_mean, ms_var = _ms_args(ms[0], ms[1], StreamLayout.single(self.static_dim * len(windows), len(windows)),
-                                       0, 1.0, None)[:2]
+                                       0, 1.0, None, ms_segment)[:2]
             self.ms = (ms_mean, ms_var)
+            self.ms_segment = None if ms_segment is None else int(ms_segment)
 
     def _generate(self, E, Dv, lengths):
         if self.ms is not None:
-            return mlpg_ms_batch(E, Dv, self.windows, self.ms[0], self.ms[1], lengths=lengths)
+            return mlpg_ms_batch(E, Dv, self.windows, self.ms[0], self.ms[1], lengths=lengths,
+                                 segment=self.ms_segment)
         if self.gv is None:
             return mlpg_batch(E, Dv, self.windows, lengths=lengths)
         return mlpg_gv_batch(E, Dv, self.windows, self.gv[0], self.gv[1], lengths=lengths)

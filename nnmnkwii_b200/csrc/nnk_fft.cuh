@@ -1,5 +1,6 @@
 // nnk_fft.cuh -- complex arithmetic and the per-bin operations of the modulation-spectrum kernels, shared by
-// csrc/nnk_modspec.cu (utterance level) and csrc/nnk_ms_segment.cu (segment level).
+// csrc/nnk_modspec.cu (utterance level), csrc/nnk_ms_segment.cu (segment level) and csrc/nnk_ms_gen.cu
+// (generation, both levels).
 #pragma once
 #include <cfloat>
 
@@ -78,6 +79,40 @@ __device__ __forceinline__ void block_ifft_dif(V* z, const V* tw, int tid) {
       z[i1] = cmul(csub(u, v), conj_(tw[p << (LOGN - s)]));
     }
     __syncthreads();
+  }
+}
+
+// the same two transforms run by the 32 lanes of one warp on the warp's own z, with __syncwarp between stages
+// (csrc/nnk_ms_gen.cu's segment-level trial kernel; nnk_ms_segment.cu keeps its own copy for now)
+template <int LOGN, typename V>
+__device__ __forceinline__ void warp_fft_dit(V* z, const V* tw, int lane) {
+  constexpr int LOGM = LOGN - 1, M = 1 << LOGM;
+#pragma unroll
+  for (int s = 1; s <= LOGM; ++s) {
+    const int half = 1 << (s - 1);
+    for (int j = lane; j < M / 2; j += 32) {
+      const int p = j & (half - 1), i0 = ((j >> (s - 1)) << s) + p, i1 = i0 + half;
+      const V u = z[i0], v = cmul(z[i1], tw[p << (LOGN - s)]);
+      z[i0] = cadd(u, v);
+      z[i1] = csub(u, v);
+    }
+    __syncwarp();
+  }
+}
+
+template <int LOGN, typename V>
+__device__ __forceinline__ void warp_ifft_dif(V* z, const V* tw, int lane) {
+  constexpr int LOGM = LOGN - 1, M = 1 << LOGM;
+#pragma unroll
+  for (int s = LOGM; s >= 1; --s) {
+    const int half = 1 << (s - 1);
+    for (int j = lane; j < M / 2; j += 32) {
+      const int p = j & (half - 1), i0 = ((j >> (s - 1)) << s) + p, i1 = i0 + half;
+      const V u = z[i0], v = z[i1];
+      z[i0] = cadd(u, v);
+      z[i1] = cmul(csub(u, v), conj_(tw[p << (LOGN - s)]));
+    }
+    __syncwarp();
   }
 }
 

@@ -23,7 +23,8 @@ Additive, parameter generation considering global variance (Toda, Black & Tokuda
 :func:`gv_statistics` (csrc/nnk_mlpg.cu ``nnk_mlpg_gv``, csrc/nnk_stats.cu ``nnk_segment_moments``).
 
 Additive, parameter generation considering the modulation spectrum (DESIGN.md 3.18): :func:`mlpg_ms`,
-:func:`mlpg_ms_batch` (csrc/nnk_ms_gen.cu ``nnk_mlpg_ms``, C ABI include/nnk_ms_gen.h).  Not in ``__all__``.
+:func:`mlpg_ms_batch` (csrc/nnk_ms_gen.cu ``nnk_mlpg_ms``, C ABI include/nnk_ms_gen.h; with ``segment=L``
+``nnk_mlpg_ms_segment``, include/nnk_ms_segment.h).  Not in ``__all__``.
 """
 import ctypes
 
@@ -453,13 +454,16 @@ class _NnkMlpgMs(ctypes.Structure):
 
 
 _MS_GEN_N = (256, 512, 1024, 2048, 4096)
+_MS_SEG_N = (32, 64, 128, 256, 512)  # the segment level's DFT lengths (postfilters.SEGMENT_NS)
 
 
-def _ms_args(ms_mean, ms_var, layout, n_iter, step, weight):
+def _ms_args(ms_mean, ms_var, layout, n_iter, step, weight, segment=None):
     """Checked MS parameters ``(ms_mean, ms_var, n, n_iter, step, weight)``: float64 host ``(K, layout.D_out)``
     arrays (``weight`` 0 = the default ``1 / (nw T)``).  Columns of copied chains are not used and not checked;
-    they are set to ``(0, inf)``."""
+    they are set to ``(0, inf)``.  With ``segment`` (the segment length L), n is one of the segment level's."""
     from ._device import is_tensor
+    if segment is not None and (isinstance(segment, bool) or not isinstance(segment, (int, np.integer))):
+        raise TypeError("segment must be an int (the segment length L) or None, got %s" % type(segment).__name__)
     arrs = []
     for name, a in (("ms_mean", ms_mean), ("ms_var", ms_var)):
         if is_tensor(a):
@@ -475,7 +479,13 @@ def _ms_args(ms_mean, ms_var, layout, n_iter, step, weight):
     if mm.shape != mv.shape:
         raise ValueError("ms_mean and ms_var differ in shape: %s, %s" % (mm.shape, mv.shape))
     n = 2 * (mm.shape[0] - 1)
-    if n not in _MS_GEN_N:
+    if segment is not None:
+        if n not in _MS_SEG_N:
+            raise ValueError("ms_mean / ms_var have %d bins: with segment, n = 2 (K - 1) = %d must be one of 32, 64, "
+                             "128, 256, 512" % (mm.shape[0], n))
+        if int(segment) % 2 or not 4 <= int(segment) <= n:
+            raise ValueError("segment length must be even with 4 <= L <= n = %d, got %d" % (n, int(segment)))
+    elif n not in _MS_GEN_N:
         raise ValueError("ms_mean / ms_var have %d bins: n = 2 (K - 1) = %d must be one of 256, 512, 1024, 2048, "
                          "4096" % (mm.shape[0], n))
     used = np.unique(layout.chains["out_col"][layout.chains["flags"] == 0])
@@ -519,7 +529,7 @@ def _ms_lengths(means, lengths, offsets, padded):
 
 
 def mlpg_ms_batch(means, variances, windows, ms_mean, ms_var, lengths=None, offsets=None, layout=None, n_iter=20,
-                  step=1.0, weight=None, check=True, out=None):
+                  step=1.0, weight=None, check=True, out=None, segment=None):
     r"""Batched parameter generation considering the modulation spectrum (additive API).
 
     Per utterance and smoothed output column ``s``, with ``Y = rfft(c, n)`` and
@@ -549,10 +559,21 @@ def mlpg_ms_batch(means, variances, windows, ms_mean, ms_var, lengths=None, offs
         step: initial step ``alpha`` (``> 0``).
         weight: :math:`\omega` (``> 0``); default ``1 / (num_windows * T)`` per utterance.
         out: optional ``(sum_T, D_out)`` NumPy buffer of the working dtype (flat host form only).
+        segment: ``None`` (the utterance level above) or the segment length ``L`` of the segment-level term:
+            with hop ``H = L / 2``, a periodic Hann window ``w`` and the ``J = ceil(T / H) + 1`` segments of
+            :func:`~nnmnkwii_b200.postfilters.modspec_statistics` ``(segment=L)`` (segment ``j`` starts at frame
+            ``(j - 1) H``, frames outside the utterance are 0), the MS term becomes the mean over the segments,
+            :math:`-\tfrac{1}{2J} \sum_j \sum_{k=1}^{n/2} q_k (s_{j,k}(c) - \nu_k)^2` with
+            :math:`s_{j,k}` the log power of ``rfft(w * c[segment j], n)``.  ``ms_mean`` / ``ms_var`` are then
+            ``(n // 2 + 1, D_out)`` statistics with ``n`` 32, 64, 128, 256 or 512, e.g.
+            ``modspec_statistics(natural_static, n=n, segment=L)``; ``L`` is even with ``4 <= L <= n``, and
+            utterances may have any length.  Nobody has measured the output quality of this variant at the
+            default ``n_iter`` and ``step`` either.
 
     Returns:
         Trajectories shaped and typed like :func:`mlpg_batch`'s.  Arithmetic is float64 (float32 inputs are
-        widened once on the device).  Every argument error is a ``ValueError`` raised before any launch.
+        widened once on the device).  Every argument error is raised before any launch: a ``segment`` that is
+        not an int is a ``TypeError``, every other one a ``ValueError``.
     """
     import torch
 
@@ -567,12 +588,13 @@ def mlpg_ms_batch(means, variances, windows, ms_mean, ms_var, lengths=None, offs
         raise ValueError("layout covers %d input columns, means have %d" % (layout.D_in, D))
     if padded and lengths is None:
         raise ValueError("padded (B, Tmax, D) input needs lengths")
-    ms = _ms_args(ms_mean, ms_var, layout, n_iter, step, weight)
+    ms = _ms_args(ms_mean, ms_var, layout, n_iter, step, weight, segment)
     lens = _ms_lengths(means, lengths, offsets, padded)
-    if lens.size and int(lens.max()) > ms[2]:
+    if segment is None and lens.size and int(lens.max()) > ms[2]:
         raise ValueError("an utterance of %d frames is longer than the DFT length n = %d" % (lens.max(), ms[2]))
+    L = None if segment is None else int(segment)
     if dev.is_tensor(means):
-        return _mlpg_ms_device(means, variances, windows, lengths, offsets, layout, padded, check, ms)
+        return _mlpg_ms_device(means, variances, windows, lengths, offsets, layout, padded, check, ms, L)
     dtype = np.asarray(means).dtype
     v_np = np.asarray(variances)
     work = dtype if (dtype in (np.float32, np.float64) and v_np.dtype == dtype) else np.dtype(np.float64)
@@ -580,7 +602,7 @@ def mlpg_ms_batch(means, variances, windows, ms_mean, ms_var, lengths=None, offs
     device = dev.cuda_device()
     m = torch.from_numpy(np.ascontiguousarray(means, dtype=work)).to(device)
     v = torch.from_numpy(np.ascontiguousarray(v_np, dtype=work)).to(device)
-    y = _mlpg_ms_device(m, v, windows, lengths, offsets, layout, padded, check, ms).cpu().numpy()
+    y = _mlpg_ms_device(m, v, windows, lengths, offsets, layout, padded, check, ms, L).cpu().numpy()
     if out is not None:
         if padded or out.shape != y.shape or out.dtype != work or not out.flags.c_contiguous:
             raise ValueError("out must be a C-contiguous %s array of dtype %s" % (y.shape, work))
@@ -589,7 +611,7 @@ def mlpg_ms_batch(means, variances, windows, ms_mean, ms_var, lengths=None, offs
     return y if y.dtype == dtype else y.astype(dtype)
 
 
-def _mlpg_ms_device(means, variances, windows, lengths, offsets, layout, padded, check, ms):
+def _mlpg_ms_device(means, variances, windows, lengths, offsets, layout, padded, check, ms, L=None):
     import torch
 
     from . import _device as dev
@@ -633,8 +655,12 @@ def _mlpg_ms_device(means, variances, windows, lengths, offsets, layout, padded,
         p.ms_mean, p.ms_var, p.n, p.n_iter, p.step, p.weight = (mean_d.data_ptr(), var_d.data_ptr(), ms[2], ms[3],
                                                                 ms[4], ms[5])
         p.n_rows = n_rows
-        _lib.check(_lib.lib.nnk_mlpg_ms(ctypes.byref(a), ctypes.byref(p), dev.current_stream_ptr(device)),
-                   "nnk_mlpg_ms")
+        if L is None:
+            _lib.check(_lib.lib.nnk_mlpg_ms(ctypes.byref(a), ctypes.byref(p), dev.current_stream_ptr(device)),
+                       "nnk_mlpg_ms")
+        else:
+            _lib.check(_lib.lib.nnk_mlpg_ms_segment(ctypes.byref(a), ctypes.byref(p), L,
+                                                    dev.current_stream_ptr(device)), "nnk_mlpg_ms_segment")
         if check == "deferred":
             dev._defer_check(status, device)
         elif check:
@@ -644,13 +670,15 @@ def _mlpg_ms_device(means, variances, windows, lengths, offsets, layout, padded,
     return out if dtype == torch.float64 else out.to(dtype)
 
 
-def mlpg_ms(mean_frames, variance_frames, windows, ms_mean, ms_var, n_iter=20, step=1.0, weight=None):
+def mlpg_ms(mean_frames, variance_frames, windows, ms_mean, ms_var, n_iter=20, step=1.0, weight=None,
+            segment=None):
     """Parameter generation considering the modulation spectrum for one utterance, ``(T, D) -> (T, static_dim)``:
     :func:`mlpg`'s arguments plus the MS parameters of :func:`mlpg_ms_batch` (``ms_mean`` / ``ms_var`` of shape
-    ``(n // 2 + 1, static_dim)``).  NumPy in, NumPy out (a CUDA tensor stays a CUDA tensor)."""
+    ``(n // 2 + 1, static_dim)``; ``segment=L`` for the segment-level term).  NumPy in, NumPy out (a CUDA tensor
+    stays a CUDA tensor)."""
     T, D = mean_frames.shape
     return mlpg_ms_batch(mean_frames, variance_frames, windows, ms_mean, ms_var, lengths=[T], n_iter=n_iter,
-                         step=step, weight=weight)
+                         step=step, weight=weight, segment=segment)
 
 
 # ---------------------------------------------------------------------------------------------------
