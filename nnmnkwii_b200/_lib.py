@@ -274,6 +274,15 @@ MS_GEN_SIGNATURES = {
     "nnk_mlpg_ms_workspace_bytes": (size_t, [i32, i32, i32, i64, i64, P(NnkWindows)]),
 }
 
+# parameter generation from mixture outputs (include/nnk_mix_gen.h), in the same library; the nnk_mix_gen_args_t
+# argument is passed by reference to paramgen's ctypes mirror of it
+NNK_MIX_GEN_SELECT, NNK_MIX_GEN_ESTEP, NNK_MIX_GEN_OBJECTIVE = 0, 1, 2
+NNK_MIX_GEN_TILE, NNK_MIX_GEN_MAX_D, NNK_MIX_GEN_MAX_M = 32, 256, 64
+
+MIX_GEN_SIGNATURES = {
+    "nnk_mix_gen": (ctypes.c_int, [vp, vp]),
+}
+
 class NnkError(RuntimeError):
     pass
 
@@ -288,7 +297,7 @@ def _load():
     if L.nnk_abi_version() != ABI_VERSION:
         raise ImportError("libnnk_b200.so ABI %d != binding ABI %d: rebuild" % (L.nnk_abi_version(), ABI_VERSION))
     for name, (restype, argtypes) in (list(SIGNATURES.items()) + list(MS_SEGMENT_SIGNATURES.items()) +
-                                      list(MS_GEN_SIGNATURES.items())):
+                                      list(MS_GEN_SIGNATURES.items()) + list(MIX_GEN_SIGNATURES.items())):
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, argtypes
     return L

@@ -16,7 +16,7 @@ OBJ = os.path.join(HERE, "csrc", "_obj")
 LIB = os.environ.get("NNK_LIB_OUT") or os.path.join(HERE, "libnnk_b200.so")  # NNK_LIB_OUT: A/B builds
 SOURCES = ["nnk_core.cu", "nnk_mlpg.cu", "nnk_host.cu", "nnk_uvmlpg.cu", "nnk_dtw.cu", "nnk_delta.cu", "nnk_metrics.cu", "nnk_shard.cu", "nnk_gmm.cu",
            "nnk_gmm_em.cu", "nnk_kmeans.cu", "nnk_postfilter.cu", "nnk_stats.cu", "nnk_wave.cu", "nnk_linalg.cu",
-           "nnk_modspec.cu", "nnk_gmm_traj.cu", "nnk_ms_segment.cu", "nnk_ms_gen.cu"]
+           "nnk_modspec.cu", "nnk_gmm_traj.cu", "nnk_ms_segment.cu", "nnk_ms_gen.cu", "nnk_mix_gen.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",

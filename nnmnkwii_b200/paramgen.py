@@ -25,6 +25,10 @@ Additive, parameter generation considering global variance (Toda, Black & Tokuda
 Additive, parameter generation considering the modulation spectrum (DESIGN.md 3.18): :func:`mlpg_ms`,
 :func:`mlpg_ms_batch` (csrc/nnk_ms_gen.cu ``nnk_mlpg_ms``, C ABI include/nnk_ms_gen.h; with ``segment=L``
 ``nnk_mlpg_ms_segment``, include/nnk_ms_segment.h).  Not in ``__all__``.
+
+Additive, parameter generation from per-frame mixture outputs over all components (DESIGN.md 3.19):
+:func:`mlpg_mixture`, :func:`mlpg_mixture_batch` (csrc/nnk_mix_gen.cu ``nnk_mix_gen``, C ABI
+include/nnk_mix_gen.h).  Not in ``__all__``.
 """
 import ctypes
 
@@ -679,6 +683,264 @@ def mlpg_ms(mean_frames, variance_frames, windows, ms_mean, ms_var, n_iter=20, s
     T, D = mean_frames.shape
     return mlpg_ms_batch(mean_frames, variance_frames, windows, ms_mean, ms_var, lengths=[T], n_iter=n_iter,
                          step=step, weight=weight, segment=segment)
+
+
+# ---------------------------------------------------------------------------------------------------
+# mixture outputs (additive)
+# ---------------------------------------------------------------------------------------------------
+class _NnkMixGenArgs(ctypes.Structure):
+    """ctypes mirror of ``nnk_mix_gen_args_t`` (include/nnk_mix_gen.h)."""
+    _fields_ = [
+        ("log_weights", ctypes.c_void_p),
+        ("means", ctypes.c_void_p),
+        ("vars", ctypes.c_void_p),
+        ("dtype", ctypes.c_int32),
+        ("M", ctypes.c_int32),
+        ("D", ctypes.c_int32),
+        ("n_utt", ctypes.c_int32),
+        ("utt_off", ctypes.c_void_p),
+        ("utt_len", ctypes.c_void_p),
+        ("tile_off", ctypes.c_void_p),
+        ("n_tiles", ctypes.c_int32),
+        ("col_map", ctypes.c_void_p),
+        ("win", _lib.NnkWindows),
+        ("mode", ctypes.c_int32),
+        ("c", ctypes.c_void_p),
+        ("c_ld", ctypes.c_int64),
+        ("c_cols", ctypes.c_int32),
+        ("lnorm", ctypes.c_void_p),
+        ("E", ctypes.c_void_p),
+        ("V", ctypes.c_void_p),
+        ("ll_part", ctypes.c_void_p),
+        ("status_word", ctypes.c_void_p),
+    ]
+
+
+_MIX_DATA_ERRORS = {1: "a NaN or +inf log-weight", 2: "every log-weight is -inf",
+                    3: "a variance that is not positive and finite"}
+
+
+def _mix_column_map(layout, nw):
+    """int32 ``(D_in,)`` column map of nnk_mix_gen (include/nnk_mix_gen.h): ``-1`` for a column no chain reads,
+    ``out_col << 3`` for a copied column, ``(out_col << 3) | (w + 1)`` for window ``w`` of a smoothed one."""
+    cmap = np.full(layout.D_in, -1, dtype=np.int32)
+    for in_col, stride, out_col, flags in layout.chains.tolist():
+        for w in range(1 if flags & 1 else nw):
+            col = in_col + w * stride
+            if not 0 <= col < layout.D_in or cmap[col] != -1:
+                raise ValueError("layout: column %d is outside the %d input columns or read by two chains"
+                                 % (col, layout.D_in))
+            cmap[col] = (out_col << 3) | (0 if flags & 1 else w + 1)
+    return cmap
+
+
+def _mix_check(log_weights, means, variances, windows, lengths, offsets, layout, n_iter):
+    """Checked arguments of :func:`mlpg_mixture_batch`, all raised before any launch:
+    ``(padded, lens, layout, column map, n_iter, arrays)``."""
+    from . import _device as dev
+    if isinstance(n_iter, (bool, np.bool_)) or not isinstance(n_iter, (int, np.integer)) or n_iter < 0:
+        raise ValueError("n_iter must be an integer >= 0, got %r" % (n_iter,))
+    arrs = (log_weights, means, variances)
+    tensors = [dev.is_tensor(a) for a in arrs]
+    if any(tensors) and not all(tensors):
+        raise ValueError("log_weights, means and variances must all be CUDA tensors or all NumPy arrays")
+    if all(tensors):
+        if not all(a.is_cuda for a in arrs):
+            raise ValueError("torch inputs must be CUDA tensors (no CPU fallback)")
+    else:
+        arrs = tuple(np.asarray(a) for a in arrs)
+    for name, a in zip(("log_weights", "means", "variances"), arrs):
+        if dev.np_dtype(a) not in (np.float32, np.float64):
+            raise ValueError("%s must be float32 or float64, got %s" % (name, dev.np_dtype(a)))
+    means = arrs[1]
+    if means.ndim not in (3, 4):
+        raise ValueError("means must be (sum_T, M, D) or (B, Tmax, M, D), got shape %s" % (tuple(means.shape),))
+    if tuple(arrs[2].shape) != tuple(means.shape):
+        raise ValueError("variances must have the shape of means %s, got %s" % (tuple(means.shape),
+                                                                                 tuple(arrs[2].shape)))
+    if tuple(arrs[0].shape) != tuple(means.shape[:-1]):
+        raise ValueError("log_weights must be %s, got %s" % (tuple(means.shape[:-1]), tuple(arrs[0].shape)))
+    padded = means.ndim == 4
+    M, D = int(means.shape[-2]), int(means.shape[-1])
+    if not 1 <= M <= _lib.NNK_MIX_GEN_MAX_M:
+        raise ValueError("mlpg_mixture supports 1 .. %d components, got %d" % (_lib.NNK_MIX_GEN_MAX_M, M))
+    if not 1 <= D <= _lib.NNK_MIX_GEN_MAX_D:
+        raise ValueError("mlpg_mixture supports 1 .. %d columns, got %d" % (_lib.NNK_MIX_GEN_MAX_D, D))
+    if not windows:
+        raise ValueError("windows must not be empty")
+    _lib.make_windows(windows)
+    if layout is None:
+        layout = StreamLayout.single(D, len(windows))
+    if layout.D_in != D:
+        raise ValueError("layout covers %d input columns, means have %d" % (layout.D_in, D))
+    if padded and lengths is None:
+        raise ValueError("padded (B, Tmax, M, D) input needs lengths")
+    lens = _ms_lengths(means, lengths, offsets, padded)
+    return padded, lens, layout, _mix_column_map(layout, len(windows)), int(n_iter), arrs
+
+
+def mlpg_mixture_batch(log_weights, means, variances, windows, lengths=None, offsets=None, layout=None, n_iter=5,
+                       return_log_likelihood=False):
+    r"""Batched parameter generation from per-frame Gaussian mixtures, over all components (additive API).
+
+    Frame ``t`` has ``M`` diagonal Gaussian components with log-weights ``lw[t, m]``, means ``mu[t, m]`` and
+    variances ``s2[t, m]`` in the column layout of :func:`mlpg_batch`'s ``(T, D)`` rows, e.g. the output of a
+    mixture density network.  With ``Y = W c`` the static and dynamic sequence of trajectory ``c`` (windows
+    never cross an utterance), the trajectory maximises
+
+    .. math:: L(c) = \sum_t \log \sum_m \exp(lw_{t,m} + \log N(Y_t; \mu_{t,m}, \mathrm{diag}\,\sigma^2_{t,m}))
+
+    over the columns that count at ``t``: on the first and last ``H = max(l, u)`` frames of an utterance (every
+    frame when ``H = 0``) only the static and copied columns, as :func:`mlpg` gives the dynamic windows zero
+    precision there; elsewhere every column a chain reads.  EM (Tokuda et al., ICASSP 2000): ``c_0`` is
+    :func:`mlpg_batch` of each frame's most probable component (the lowest index on ties, as ``np.argmax``); each
+    iteration takes the posteriors ``gamma[t, m]`` of the current trajectory and solves with precisions
+    ``P_t = sum_m gamma / s2`` and means ``(sum_m gamma mu / s2) / P_t``, so ``L`` never decreases.  See
+    DESIGN.md 3.19.  Nobody has measured whether the result sounds better than the most-probable collapse.
+
+    Args:
+        log_weights: flat ``(sum_T, M)`` or padded ``(B, Tmax, M)``; need not be normalised, may be ``-inf``
+            (a log-softmax output goes in as it is).
+        means, variances: flat ``(sum_T, M, D)`` or padded ``(B, Tmax, M, D)``; ``variances`` positive and
+            finite wherever a chain reads.  The three are CUDA tensors or NumPy arrays, float32 or float64.
+        windows, lengths, offsets, layout: as :func:`mlpg_batch` (``merlin_layout()`` included: a copied column
+            counts like a static one).
+        n_iter: EM iterations (``>= 0``); 0 returns :func:`mlpg_batch` of the most probable components.
+        return_log_likelihood: also return ``L(c_0) .. L(c_n_iter)`` per utterance.
+
+    Returns:
+        The trajectories, flat ``(sum_T, D_out)`` or padded ``(B, Tmax, D_out)`` with zero rows beyond each
+        length, of the form and dtype of ``means`` (computed in float64; a float32 result is the float64 result of
+        the widened inputs, rounded); with ``return_log_likelihood`` also an ``(n_utt, n_iter + 1)`` float64 NumPy
+        array.  Argument errors (shapes, dtypes, more than 64 components or 256 columns, ``n_iter``) raise
+        ``ValueError`` before any launch.  A data error (a NaN or ``+inf`` log-weight, a frame whose log-weights
+        are all ``-inf``, a variance that is not positive and finite) is found on the device and raises
+        ``ValueError`` when the result comes back.
+    """
+    import torch
+
+    from . import _device as dev
+    padded, lens, layout, cmap, n_iter, arrs = _mix_check(log_weights, means, variances, windows, lengths, offsets,
+                                                          layout, n_iter)
+    on_device = dev.is_tensor(arrs[1])
+    if not on_device:
+        dev.require_cuda()
+        device = dev.cuda_device()
+        arrs = tuple(torch.from_numpy(np.ascontiguousarray(a)).to(device) for a in arrs)
+    y, L = _mlpg_mixture_device(*arrs, windows, lens, layout, cmap, padded, n_iter, return_log_likelihood)
+    if y.dtype != arrs[1].dtype:
+        y = y.to(arrs[1].dtype)
+    if not on_device:
+        y = y.cpu().numpy()
+    return (y, L) if return_log_likelihood else y
+
+
+def _mlpg_mixture_device(lw, mu, s2, windows, lens, layout, cmap, padded, n_iter, want_ll):
+    """The device part of :func:`mlpg_mixture_batch` on checked CUDA tensors: float64 ``(y, L or None)``."""
+    import math
+
+    import torch
+
+    from . import _device as dev
+    device = mu.device
+    dev.poll_errors()
+    if not (lw.dtype == mu.dtype == s2.dtype):
+        lw, mu, s2 = (a.to(torch.float64) for a in (lw, mu, s2))
+    lw, mu, s2 = (a.contiguous() for a in (lw, mu, s2))
+    M, D = mu.shape[-2], mu.shape[-1]
+    n_rows = mu.shape[0] * mu.shape[1] if padded else mu.shape[0]
+    n_utt = len(lens)
+    off = (np.arange(n_utt + 1, dtype=np.int64) * mu.shape[1] if padded
+           else np.concatenate([[0], np.cumsum(lens)]).astype(np.int64))
+    y = torch.zeros((n_rows, layout.D_out), dtype=torch.float64, device=device)
+    L = np.zeros((n_utt, n_iter + 1)) if want_ll else None
+    if not (n_utt and int(lens.max(initial=0)) and layout.n_chain):
+        return (y.reshape(mu.shape[0], mu.shape[1], layout.D_out) if padded else y), L
+    order = np.argsort(-lens, kind="stable").astype(np.int32)
+    max_T = int(lens.max())
+    tiles = -(-lens // _lib.NNK_MIX_GEN_TILE)
+    tile_off = np.concatenate([[0], np.cumsum(tiles)]).astype(np.int32)
+    n_tiles = int(tile_off[-1])
+
+    def up(a):  # asynchronous upload: nothing below waits for the device until the results come back
+        return torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(device, non_blocking=True)
+    tables = up(np.concatenate([off[:-1].astype(np.int32), lens.astype(np.int32), tile_off, order, cmap]))
+    utt_off_d, len_d = tables[:n_utt], tables[n_utt:2 * n_utt]
+    tile_d, order_d = tables[2 * n_utt:3 * n_utt + 1], tables[3 * n_utt + 1:4 * n_utt + 1]
+    cmap_d = tables[4 * n_utt + 1:]
+    offsets_d = up(off)
+    chains = dev.chains_on_device(layout.chains, device)
+    win = _lib.make_windows(windows)
+    status = torch.zeros(2, dtype=torch.int64, device=device)  # [0] the solves' pivots, [1] the data errors
+
+    def solve(E, V):  # the kernels and arguments of mlpg_batch(E, V, windows, lengths, layout=layout)
+        out = torch.zeros((n_rows, layout.D_out), dtype=torch.float64, device=device)
+        dev.run_mlpg("fwd", means=E, variances=V, rhs=None, out=out, offsets=offsets_d,
+                     lengths=len_d if padded else None, order=order_d, chains=chains, n_chain=layout.n_chain,
+                     max_T=max_T, windows_c=win, in_ld=D, var_ld=D, go_ld=0, out_ld=layout.D_out,
+                     dtype_code=_lib.NNK_F64, go_f64=0, n_utt=n_utt, device=device, check=False, status=status[0:1])
+        return out
+
+    E = torch.empty((n_rows, D), dtype=torch.float64, device=device)
+    V = torch.empty((n_rows, D), dtype=torch.float64, device=device)
+    lnorm = torch.empty((n_rows, M), dtype=torch.float64, device=device)
+    ll = torch.zeros((n_iter + 1, n_tiles), dtype=torch.float64, device=device) if want_ll else None
+    a = _NnkMixGenArgs()
+    a.log_weights, a.means, a.vars = lw.data_ptr(), mu.data_ptr(), s2.data_ptr()
+    a.dtype, a.M, a.D, a.n_utt = dev.torch_dtype_code(mu.dtype), M, D, n_utt
+    a.utt_off, a.utt_len, a.tile_off, a.n_tiles = utt_off_d.data_ptr(), len_d.data_ptr(), tile_d.data_ptr(), n_tiles
+    a.col_map, a.win = cmap_d.data_ptr(), win
+    a.c_ld, a.c_cols = layout.D_out, layout.D_out
+    a.lnorm, a.E, a.V = lnorm.data_ptr(), E.data_ptr(), V.data_ptr()
+    a.status_word = status[1:2].data_ptr()
+    stream = dev.current_stream_ptr(device)
+
+    def launch(mode, c, k):
+        a.mode = mode
+        a.c = c.data_ptr() if c is not None else None
+        a.ll_part = ll[k].data_ptr() if (want_ll and mode != _lib.NNK_MIX_GEN_SELECT) else None
+        _lib.check(_lib.lib.nnk_mix_gen(ctypes.byref(a), stream), "nnk_mix_gen")
+
+    launch(_lib.NNK_MIX_GEN_SELECT, None, 0)
+    y = solve(E, V)
+    for k in range(n_iter):
+        launch(_lib.NNK_MIX_GEN_ESTEP, y, k)
+        y = solve(E, V)
+    if want_ll:
+        launch(_lib.NNK_MIX_GEN_OBJECTIVE, y, n_iter)
+    # the one host synchronisation: status words and objective partials come back together
+    host_status = torch.empty(2, dtype=torch.int64).pin_memory()
+    host_status.copy_(status, non_blocking=True)
+    if want_ll:
+        host_ll = torch.empty(ll.shape, dtype=torch.float64).pin_memory()
+        host_ll.copy_(ll, non_blocking=True)
+    torch.cuda.current_stream(device).synchronize()
+    word = int(host_status[1]) & 0xFFFFFFFFFFFFFFFF
+    if word:
+        key = ~word & 0xFFFFFFFFFFFFFFFF
+        row, kind = key >> 2, key & 3
+        u = int(np.searchsorted(off, row, side="right")) - 1
+        raise ValueError("mlpg_mixture: %s at frame %d of utterance %d" % (_MIX_DATA_ERRORS[kind], row - off[u], u))
+    dev._raise_word(int(host_status[0]))
+    if want_ll:
+        parts = host_ll.numpy()
+        L = np.array([[math.fsum(parts[k, tile_off[u]:tile_off[u + 1]]) for k in range(n_iter + 1)]
+                      for u in range(n_utt)])
+    if padded:
+        y = y.reshape(mu.shape[0], mu.shape[1], layout.D_out)
+    return y, L
+
+
+def mlpg_mixture(log_weights, means, variances, windows, n_iter=5, return_log_likelihood=False):
+    """Parameter generation from per-frame mixtures for one utterance: ``log_weights (T, M)``, ``means`` and
+    ``variances (T, M, D)`` -> ``(T, static_dim)``, see :func:`mlpg_mixture_batch`.  With
+    ``return_log_likelihood`` also ``L(c_0) .. L(c_n_iter)``, ``(n_iter + 1,)`` float64.  NumPy in, NumPy out (a
+    CUDA tensor stays a CUDA tensor)."""
+    if len(means.shape) != 3:
+        raise ValueError("means must be (T, M, D), got shape %s" % (tuple(means.shape),))
+    out = mlpg_mixture_batch(log_weights, means, variances, windows, lengths=[means.shape[0]], n_iter=n_iter,
+                             return_log_likelihood=return_log_likelihood)
+    return (out[0], out[1][0]) if return_log_likelihood else out
 
 
 # ---------------------------------------------------------------------------------------------------
