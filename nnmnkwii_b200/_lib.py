@@ -283,6 +283,14 @@ MIX_GEN_SIGNATURES = {
     "nnk_mix_gen": (ctypes.c_int, [vp, vp]),
 }
 
+
+# the trajectory-model log-likelihood (include/nnk_traj_ll.h), in the same library; the nnk_traj_ll_t argument is
+# passed by reference to paramgen's ctypes mirror of it
+TRAJ_LL_SIGNATURES = {
+    "nnk_mlpg_traj_ll": (ctypes.c_int, [P(NnkMlpgArgs), vp, vp]),
+    "nnk_mlpg_traj_ll_workspace_bytes": (size_t, [i32, i32, i32, P(NnkWindows)]),
+}
+
 class NnkError(RuntimeError):
     pass
 
@@ -297,7 +305,8 @@ def _load():
     if L.nnk_abi_version() != ABI_VERSION:
         raise ImportError("libnnk_b200.so ABI %d != binding ABI %d: rebuild" % (L.nnk_abi_version(), ABI_VERSION))
     for name, (restype, argtypes) in (list(SIGNATURES.items()) + list(MS_SEGMENT_SIGNATURES.items()) +
-                                      list(MS_GEN_SIGNATURES.items()) + list(MIX_GEN_SIGNATURES.items())):
+                                      list(MS_GEN_SIGNATURES.items()) + list(MIX_GEN_SIGNATURES.items()) +
+                                      list(TRAJ_LL_SIGNATURES.items())):
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, argtypes
     return L

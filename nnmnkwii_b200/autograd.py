@@ -9,6 +9,9 @@ Differences that are additions, not signature changes:
     reduced once to its numerical band and applied as a banded stencil sweep
     (csrc/nnk_uvmlpg.cu) instead of two dense GEMMs that multiply ~95 % zeros.
 
+Additive, not in ``__all__``: ``TrajectoryLogLikelihood`` / ``trajectory_log_likelihood``, the log-likelihood of
+target trajectories under the trajectory model of the MLPG inputs, differentiable in targets, means and variances.
+
 The modulation-spectrum part (nnmnkwii/autograd/_impl/modspec.py): ``ModSpec`` and ``modspec``, plus the batched
 ``ModSpecBatch`` / ``modspec_batch``, on csrc/nnk_modspec.cu.
 """
@@ -200,6 +203,67 @@ def modspec(y, n=2048, norm=None):
 def modspec_batch(y, lengths, n=2048, norm=None):
     """Additive: batched :func:`modspec` (see :class:`ModSpecBatch`)."""
     return ModSpecBatch.apply(y, n, norm, lengths)
+
+
+class TrajectoryLogLikelihood(Function):
+    """Additive: the trajectory-model log-likelihood of :func:`nnmnkwii_b200.paramgen.trajectory_log_likelihood_batch`
+    as an autograd function, ``f : (targets, means, variances) -> (B, D_out)`` float64, differentiable in all three
+    (the variance gradient is what :class:`MLPG` and :class:`MLPGBatch` do not give).  CUDA tensors, flat
+    ``(sum_T, D)`` or zero-padded ``(B, Tmax, D)`` with ``lengths``; variances per frame or global ``(D,)``;
+    ``targets`` shaped like :func:`mlpg_batch`'s result.  The forward is one kernel launch, with the gradients
+    computed in the same launch only when an input needs them; the backward scales them by ``grad_output[u, column]``
+    with elementwise ops (and, for ``(D,)`` variances, a sum over utterances in a fixed order).  Gradients have each
+    input's shape and dtype; padded frames and copied columns get zero."""
+
+    @staticmethod
+    def forward(ctx, targets, means, variances, windows, lengths, layout=None):
+        layout, padded, on_device = G._traj_ll_check(targets, means, variances, windows, lengths, None, layout)
+        if not on_device:
+            raise ValueError("TrajectoryLogLikelihood takes CUDA tensors")
+        grad = any(ctx.needs_input_grad[:3])
+        ll, lens, grads = G._traj_ll_device(targets.detach(), means.detach(), variances.detach(), windows, lengths,
+                                            None, layout, padded, grad)
+        ctx.padded, ctx.lens, ctx.layout, ctx.nw = padded, lens, layout, len(windows)
+        ctx.shapes = (targets.shape, means.shape, variances.shape)
+        if grad:
+            ctx.save_for_backward(*grads)
+        return G._traj_ll_scatter(ll, layout)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        g_m, g_v, g_x = ctx.saved_tensors
+        layout, lens = ctx.layout, ctx.lens
+        device = g_m.device
+        go = grad_output.to(torch.float64)
+        D = g_m.shape[-1]
+        # scale of input column i of utterance u: grad_output[u, out_col of the chain that reads i], 0 if none
+        col_out = np.full(D, layout.D_out, dtype=np.int64)  # D_out: a zero column appended to grad_output
+        for c in layout.chains[layout.chains["flags"] == 0]:
+            col_out[int(c["in_col"]) + np.arange(ctx.nw) * int(c["win_stride"])] = int(c["out_col"])
+        go_ext = torch.cat([go, torch.zeros((go.shape[0], 1), dtype=torch.float64, device=device)], dim=1)
+        s_in = go_ext[:, torch.from_numpy(col_out).to(device)]  # (B, D)
+        s_out = go  # (B, D_out)
+        if ctx.padded:
+            rows_in, rows_out = s_in[:, None, :], s_out[:, None, :]
+        else:
+            reps = torch.from_numpy(np.asarray(lens, dtype=np.int64)).to(device)
+            rows_in = torch.repeat_interleave(s_in, reps, dim=0, output_size=int(np.sum(lens)))
+            rows_out = torch.repeat_interleave(s_out, reps, dim=0, output_size=int(np.sum(lens)))
+        gm = (g_m.to(torch.float64) * rows_in).to(g_m.dtype) if ctx.needs_input_grad[1] else None
+        if ctx.needs_input_grad[2]:
+            if len(ctx.shapes[2]) == 1:
+                gv = (g_v * s_in).sum(dim=0).to(g_m.dtype)
+            else:
+                gv = (g_v.to(torch.float64) * rows_in).to(g_v.dtype)
+        else:
+            gv = None
+        gx = (g_x.to(torch.float64) * rows_out).to(g_x.dtype) if ctx.needs_input_grad[0] else None
+        return gx, gm, gv, None, None, None
+
+
+def trajectory_log_likelihood(targets, means, variances, windows, lengths, layout=None):
+    """Additive: differentiable trajectory-model log-likelihood (see :class:`TrajectoryLogLikelihood`)."""
+    return TrajectoryLogLikelihood.apply(targets, means, variances, windows, lengths, layout)
 
 
 def mlpg(means, variances, windows):

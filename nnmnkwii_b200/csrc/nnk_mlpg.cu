@@ -25,6 +25,7 @@
 // (nw == NW), with NT <= 5 and rows narrow enough for as_geometry; everything else runs mlpg_kernel.
 #include <type_traits>
 
+#include "../../include/nnk_traj_ll.h"
 #include "nnk_mlpg.cuh"
 #include "nnk_mlpg_as.cuh"
 
@@ -149,12 +150,29 @@ __device__ __forceinline__ void gv_refine(double* ws, int T, double mu, double p
   for (int t = 0; t < T; ++t) st_stream(out + (int64_t)t * out_ld, (Tout)at(t, cur));
 }
 
+// ---- trajectory-model log-likelihood (MODE_TLL, MODE_TLL_GRAD; nnk_mlpg_traj_ll) ------------------------------
+// The forward sweep is MODE_FWD's; it also sums log d_t and, with the gradient, stores 1 / d_t in scratch column NT.
+// The backward sweep recomputes cbar = P^-1 b as MODE_FWD does, keeps windows of cbar and of the targets x, and at
+// step t handles row r = t + L (the row MODE_GRAD emits at the same step): u = W_w x and ubar = W_w cbar over frames
+// t .. t + S give the tau (u - ubar)^2 term of l and dl/dmu = tau (u - ubar).  With the gradient it also carries
+// the (S+1) x (S+1) block Sigma[t + a][t + b] of Sigma = P^-1, by the backward recurrence for the band of an
+// inverse (Takahashi et al. 1973; l_k[t] = L[t+k][t]):
+//   Sigma[t][t+j] = -sum_k l_k[t] Sigma[t+k][t+j]  (j = 1..S),   Sigma[t][t] = 1/d_t - sum_k l_k[t] Sigma[t][t+k],
+// which gives w_r^T Sigma w_r and dl/dvar, and emits dl/dx at frame t + S from a window of the dl/dmu rows.
+// The block is upper-triangular in registers (a <= b).
+template <int S>
+__device__ __forceinline__ double sym_at(const double (&sg)[S + 1][S + 1], int a, int b) {
+  return a <= b ? sg[a][b] : sg[b][a];
+}
+
 template <typename Tin, int NW, int L, int U, int MODE, int PF>
-__global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgParams<Tin, NW, L, U> p) {
+__global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typename KernelParams<Tin, NW, L, U, MODE>::type p) {
   constexpr int S = L + U;
   constexpr int NT = S + 1;
   constexpr int NTS = WsCols<MODE, NT>::value;
-  constexpr bool FWDLIKE = (MODE == MODE_FWD || MODE == MODE_GV);  // means in, trajectories out
+  constexpr bool TLL = (MODE == MODE_TLL || MODE == MODE_TLL_GRAD);
+  constexpr bool TGRAD = (MODE == MODE_TLL_GRAD);
+  constexpr bool FWDLIKE = (MODE == MODE_FWD || MODE == MODE_GV || TLL);  // means in (trajectories out, but TLL)
   const int lane = threadIdx.x;
   const int item = blockIdx.x;
   const int urank = p.urank0 + item / p.n_groups;
@@ -180,7 +198,9 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
 
   // ---- pass-through chains (flags & 1): plain copy (fwd) / gradient of a copy (grad) -----------
   if (active && (ch.flags & 1)) {
-    if (FWDLIKE) {
+    if constexpr (TLL) {
+      p.ll[(int64_t)utt * p.n_chain + chain] = 0.0;
+    } else if (FWDLIKE) {
       Tin* o = reinterpret_cast<Tin*>(p.out) + orow0 * p.out_ld + ch.out_col;
       for (int t = 0; t < T; ++t) o[(int64_t)t * p.out_ld] = mptr[(int64_t)t * p.in_ld];
     } else if (MODE == MODE_GRAD) {
@@ -253,6 +273,7 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
   }
   double iv1 = 0.0;
   bool reported = false;
+  double sld = 0.0;  // TLL: sum_t log d_t
 
   for (int t0 = 0; t0 < T; t0 += PF) {
 #pragma unroll
@@ -313,6 +334,8 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
         double* wsp = ws + (size_t)t * (NTS * 32);
         wsp[0] = bb * ivd;
         if (MODE == MODE_GV) wsp[NT * 32] = d;
+        if constexpr (TGRAD) wsp[NT * 32] = ivd;
+        if constexpr (TLL) sld += log(d);
 #pragma unroll
         for (int k = S; k >= 2; --k) {
           zz[k] = zz[k - 1];
@@ -353,7 +376,34 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
 #pragma unroll
   for (int j = 0; j < PF; ++j) load_ws(T - 1 - j, rz[j], rl[j]);
 
-  const int t_end = (MODE == MODE_GRAD) ? -L : 0;
+  // TLL state: windows of the targets (xw[j] = x[t + j]) and of dl/dmu (gw[i][w] = row t + L + i), the Sigma
+  // block, the prefetch rings of x and 1 / d, the quadratic term of l and the global-variance gradient sums
+  double xw[S + 1], gw[S + 1][NW], sg[S + 1][S + 1], rx[PF], rdi[PF], qll = 0.0, vsum[NW];
+  auto load_tll = [&](int t, double& x, double& di) {
+    x = 0.0; di = 0.0;
+    if constexpr (TLL) {
+      if (t >= 0 && solve) {
+        x = (double)ld_stream(p.targets + (orow0 + t) * p.tgt_ld + ch.out_col);
+        if constexpr (TGRAD) di = ws[(size_t)t * (NTS * 32) + NT * 32];
+      }
+    }
+  };
+  if constexpr (TLL) {
+#pragma unroll
+    for (int j = 0; j <= S; ++j) {
+      xw[j] = 0.0;
+#pragma unroll
+      for (int w = 0; w < NW; ++w) gw[j][w] = 0.0;
+#pragma unroll
+      for (int k = 0; k <= S; ++k) sg[j][k] = 0.0;
+    }
+#pragma unroll
+    for (int w = 0; w < NW; ++w) vsum[w] = 0.0;
+#pragma unroll
+    for (int j = 0; j < PF; ++j) load_tll(T - 1 - j, rx[j], rdi[j]);
+  }
+
+  const int t_end = (MODE == MODE_GRAD || MODE == MODE_TLL) ? -L : (MODE == MODE_TLL_GRAD) ? -S : 0;
   for (int t0 = T - 1; t0 >= t_end; t0 -= PF) {
 #pragma unroll
     for (int jj = 0; jj < PF; ++jj) {
@@ -366,8 +416,106 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
         for (int j = 1; j <= S; ++j) y = fma(-rl[jj][j], yw[j], y);
         if (t < 0) y = 0.0;
         yw[0] = y;
+        double lt[S + 1];  // TLL_GRAD: l_k[t], before the ring slot is refilled
+        if constexpr (TGRAD) {
+#pragma unroll
+          for (int k = 1; k <= S; ++k) lt[k] = rl[jj][k];
+        }
         load_ws(t - PF, rz[jj], rl[jj]);
-        if (MODE == MODE_GV) {
+        if constexpr (TLL) {
+#pragma unroll
+          for (int j = S; j > 0; --j) xw[j] = xw[j - 1];
+          xw[0] = rx[jj];
+          double di = rdi[jj];
+          load_tll(t - PF, rx[jj], rdi[jj]);
+          if constexpr (TGRAD) {
+            // Sigma block of rows t .. t + S from that of rows t + 1 .. t + S + 1 (zero past T, and for t < 0,
+            // where l and 1 / d load as zero)
+#pragma unroll
+            for (int a = S; a > 0; --a)
+#pragma unroll
+              for (int b = S; b >= a; --b) sg[a][b] = sg[a - 1][b - 1];
+#pragma unroll
+            for (int j = 1; j <= S; ++j) {
+              double s = 0.0;
+#pragma unroll
+              for (int k = 1; k <= S; ++k) s = fma(-lt[k], sym_at<S>(sg, k, j), s);
+              sg[0][j] = s;
+            }
+#pragma unroll
+            for (int k = 1; k <= S; ++k) di = fma(-lt[k], sg[0][k], di);
+            sg[0][0] = di;
+          }
+          // row r = t + L
+          const int r = t + L;
+          double gr[NW];
+#pragma unroll
+          for (int w = 0; w < NW; ++w) gr[w] = 0.0;
+          if (r >= 0 && r < T && solve) {
+            Tin m[NW], v[NW];
+            double tau[NW], tm[NW];
+#pragma unroll
+            for (int w = 0; w < NW; ++w) { m[w] = Tin(0); v[w] = Tin(1); }
+#pragma unroll
+            for (int w = 0; w < NW; ++w)
+              if (w < nw) {
+                if constexpr (TGRAD) m[w] = mptr[(int64_t)r * p.in_ld + w * ch.win_stride];
+                v[w] = var_global ? gv[w] : vptr[(int64_t)r * p.var_ld + w * ch.win_stride];
+              }
+            to_frame(r, m, v, tau, tm);
+#pragma unroll
+            for (int w = 0; w < NW; ++w) {
+              if (w < nw) {
+                double ux = 0.0, uc = 0.0;
+#pragma unroll
+                for (int i = 0; i < NT; ++i) {  // c[w][L+k], k = i-L: frames r + k = t + i
+                  ux = fma(p.win.c[w][i], xw[i], ux);
+                  uc = fma(p.win.c[w][i], yw[i], uc);
+                }
+                const double e = ux - uc;
+                const double g = tau[w] * e;
+                qll = fma(g, e, qll);
+                if constexpr (TGRAD) {
+                  gr[w] = g;
+                  double wsw = 0.0;  // w_r^T Sigma w_r = sum_m (2 - [m == 0]) sum_i q[w][m][i] Sigma[t+i][t+i+m]
+#pragma unroll
+                  for (int mm = S; mm >= 1; --mm) {
+#pragma unroll
+                    for (int i = 0; i + mm < NT; ++i) wsw = fma(p.win.q[w][mm][i], sg[i][i + mm], wsw);
+                  }
+                  wsw *= 2.0;
+#pragma unroll
+                  for (int i = 0; i < NT; ++i) wsw = fma(p.win.q[w][0][i], sg[i][i], wsw);
+                  const double mu = (double)m[w];
+                  const double dx = ux - mu, dc = uc - mu;
+                  const double gvr = -0.5 * tau[w] * tau[w] * (wsw - dx * dx + dc * dc);
+                  const int64_t col = ch.in_col + w * ch.win_stride;
+                  p.grad_means[(row0 + r) * p.gm_ld + col] = (Tin)g;
+                  if (var_global) vsum[w] += gvr;
+                  else reinterpret_cast<Tin*>(p.grad_vars)[(row0 + r) * p.gv_ld + col] = (Tin)gvr;
+                }
+              }
+            }
+          }
+          if constexpr (TGRAD) {
+            // dl/dx at frame s = t + S: -sum_w sum_i c[w][S - i] dl/dmu[row t + L + i][w]
+#pragma unroll
+            for (int i = S; i > 0; --i)
+#pragma unroll
+              for (int w = 0; w < NW; ++w) gw[i][w] = gw[i - 1][w];
+#pragma unroll
+            for (int w = 0; w < NW; ++w) gw[0][w] = gr[w];
+            const int s = t + S;
+            if (s >= 0 && s < T && solve) {
+              double gx = 0.0;
+#pragma unroll
+              for (int w = 0; w < NW; ++w)
+#pragma unroll
+                for (int i = 0; i <= S; ++i) gx = fma(p.win.c[w][S - i], gw[i][w], gx);
+              p.grad_targets[(orow0 + s) * p.gx_ld + ch.out_col] = (Tin)(-gx);
+            }
+          }
+        } else if (MODE == MODE_GV) {
           ws[(size_t)t * (NTS * 32) + (NT + 1) * 32] = y;  // c_m, refined below
         } else if (MODE != MODE_GRAD) {
           if (solve) st_stream(reinterpret_cast<Tin*>(p.out) + (orow0 + t) * p.out_ld + ch.out_col, (Tin)y);
@@ -394,6 +542,21 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ MlpgPa
               }
             }
           }
+        }
+      }
+    }
+  }
+
+  if constexpr (TLL) {
+    if (solve) {
+      constexpr double LOG_2PI = 1.8378770664093454836;
+      p.ll[(int64_t)utt * p.n_chain + chain] = 0.5 * (sld - qll) - 0.5 * LOG_2PI * (double)T;
+      if constexpr (TGRAD) {
+        if (var_global) {
+          double* gp = reinterpret_cast<double*>(p.grad_vars) + (int64_t)utt * p.gv_ld + ch.in_col;
+#pragma unroll
+          for (int w = 0; w < NW; ++w)
+            if (w < nw) gp[w * ch.win_stride] = vsum[w];
         }
       }
     }
@@ -480,13 +643,20 @@ static int launch_as(const MlpgParams<Tin, NW, L, U>& p, const AsGeom& g, size_t
 }
 
 template <typename Tin, int NW, int L, int U, int MODE>
-static int launch_mlpg(const nnk_mlpg_args_t& a, const nnk_mlpg_gv_t* gv, cudaStream_t st) {
+static int launch_mlpg(const nnk_mlpg_args_t& a, const nnk_mlpg_gv_t* gv, cudaStream_t st,
+                       const nnk_traj_ll_t* tl = nullptr) {
   constexpr int NT = L + U + 1;
   constexpr int NTS = WsCols<MODE, NT>::value;
   constexpr int PF = (L + U <= 2) ? 4 : 2;
   constexpr int ES = (int)sizeof(Tin);
   constexpr bool GRAD = (MODE == MODE_GRAD);
-  MlpgParams<Tin, NW, L, U> p;
+  typename KernelParams<Tin, NW, L, U, MODE>::type p;
+  if constexpr (MODE == MODE_TLL || MODE == MODE_TLL_GRAD) {
+    p.targets = (const Tin*)tl->targets; p.tgt_ld = tl->tgt_ld; p.ll = tl->ll;
+    p.grad_means = (Tin*)tl->grad_means; p.gm_ld = tl->gm_ld;
+    p.grad_vars = tl->grad_vars; p.gv_ld = tl->gv_ld;
+    p.grad_targets = (Tin*)tl->grad_targets; p.gx_ld = tl->gx_ld;
+  }
   if (!fill_wintab<NW, L, U>(a.win, p.win)) { set_error("window set does not fit kernel instance"); return NNK_ERR_UNSUPPORTED; }
   p.means = (const Tin*)a.means; p.vars = (const Tin*)a.vars; p.go = a.grad_out; p.go_f64 = a.go_f64; p.out = a.out;
   p.in_ld = a.in_ld; p.var_ld = a.var_ld; p.go_ld = a.go_ld; p.out_ld = a.out_ld;
@@ -544,17 +714,18 @@ static int launch_mlpg(const nnk_mlpg_args_t& a, const nnk_mlpg_gv_t* gv, cudaSt
 }
 
 template <typename Tin, int MODE>
-static int dispatch_inst(const nnk_mlpg_args_t& a, cudaStream_t st, const nnk_mlpg_gv_t* gv = nullptr) {
+static int dispatch_inst(const nnk_mlpg_args_t& a, cudaStream_t st, const nnk_mlpg_gv_t* gv = nullptr,
+                         const nnk_traj_ll_t* tl = nullptr) {
   int inst = -1;
   if (pick_instance(a.win, inst) < 0) {
     set_error("unsupported window set: nw=%d (max %d) or half-width > %d", a.win.nw, NNK_MAX_WIN, NNK_MAX_HALF);
     return NNK_ERR_UNSUPPORTED;
   }
   switch (inst) {
-    case 0: return launch_mlpg<Tin, 1, 0, 0, MODE>(a, gv, st);
-    case 1: return launch_mlpg<Tin, 3, 1, 1, MODE>(a, gv, st);
-    case 2: return launch_mlpg<Tin, 3, 2, 2, MODE>(a, gv, st);
-    default: return launch_mlpg<Tin, NNK_MAX_WIN, NNK_MAX_HALF, NNK_MAX_HALF, MODE>(a, gv, st);
+    case 0: return launch_mlpg<Tin, 1, 0, 0, MODE>(a, gv, st, tl);
+    case 1: return launch_mlpg<Tin, 3, 1, 1, MODE>(a, gv, st, tl);
+    case 2: return launch_mlpg<Tin, 3, 2, 2, MODE>(a, gv, st, tl);
+    default: return launch_mlpg<Tin, NNK_MAX_WIN, NNK_MAX_HALF, NNK_MAX_HALF, MODE>(a, gv, st, tl);
   }
 }
 
@@ -589,6 +760,11 @@ extern "C" size_t nnk_mlpg_workspace_bytes(int32_t n_utt, int32_t n_chain, int32
 
 extern "C" size_t nnk_mlpg_gv_workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T, const nnk_windows_t* win) {
   return workspace_bytes(n_utt, n_chain, max_T, win, WsCols<MODE_GV, 0>::value);
+}
+
+extern "C" size_t nnk_mlpg_traj_ll_workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T,
+                                                   const nnk_windows_t* win) {
+  return workspace_bytes(n_utt, n_chain, max_T, win, WsCols<MODE_TLL, 0>::value);
 }
 
 #ifdef NNK_AS_PROF
@@ -641,4 +817,24 @@ extern "C" int nnk_mlpg_gv(const nnk_mlpg_args_t* a, const nnk_mlpg_gv_t* gv, vo
   DeviceGuard guard(a->out);
   cudaStream_t st = (cudaStream_t)stream;
   return a->dtype == NNK_F32 ? dispatch_inst<float, MODE_GV>(*a, st, gv) : dispatch_inst<double, MODE_GV>(*a, st, gv);
+}
+
+extern "C" int nnk_mlpg_traj_ll(const nnk_mlpg_args_t* a, const nnk_traj_ll_t* tl, void* stream) {
+  NNK_REQUIRE(a != nullptr && tl != nullptr, NNK_ERR_ARG, "args or tl is NULL");
+  NNK_REQUIRE(a->dtype == NNK_F32 || a->dtype == NNK_F64, NNK_ERR_ARG, "dtype must be NNK_F32 or NNK_F64");
+  NNK_REQUIRE(a->n_utt >= 0 && a->n_chain >= 0 && a->max_T >= 0, NNK_ERR_ARG, "negative size");
+  NNK_REQUIRE(a->n_chain < (1 << 21) && a->max_T < (1 << 21) - 1 && a->n_utt < (1 << 22), NNK_ERR_ARG, "size exceeds status key range");
+  NNK_REQUIRE(tl->grad == 0 || tl->grad == 1, NNK_ERR_ARG, "grad must be 0 or 1");
+  if (a->n_utt == 0 || a->n_chain == 0 || a->max_T == 0) return NNK_OK;
+  NNK_REQUIRE(a->means && a->vars && a->utt_off && a->chains && a->status_word, NNK_ERR_ARG, "NULL device pointer");
+  NNK_REQUIRE(tl->targets && tl->ll, NNK_ERR_ARG, "NULL targets or ll");
+  NNK_REQUIRE(!tl->grad || (tl->grad_means && tl->grad_vars && tl->grad_targets), NNK_ERR_ARG, "NULL gradient output");
+  NNK_REQUIRE(a->workspace != nullptr, NNK_ERR_WORKSPACE, "NULL workspace");
+  DeviceGuard guard(tl->ll);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (tl->grad)
+    return a->dtype == NNK_F32 ? dispatch_inst<float, MODE_TLL_GRAD>(*a, st, nullptr, tl)
+                               : dispatch_inst<double, MODE_TLL_GRAD>(*a, st, nullptr, tl);
+  return a->dtype == NNK_F32 ? dispatch_inst<float, MODE_TLL>(*a, st, nullptr, tl)
+                             : dispatch_inst<double, MODE_TLL>(*a, st, nullptr, tl);
 }

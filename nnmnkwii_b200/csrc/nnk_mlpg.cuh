@@ -4,14 +4,16 @@
 
 namespace nnk {
 
-// MODE_GV: the forward solve followed by the global-variance refinement of nnk_mlpg_gv (mlpg_kernel only)
-enum { MODE_FWD = 0, MODE_GRAD = 1, MODE_SOLVE = 2, MODE_GV = 3 };
+// MODE_GV: the forward solve followed by the global-variance refinement of nnk_mlpg_gv (mlpg_kernel only).
+// MODE_TLL / MODE_TLL_GRAD: the trajectory-model log-likelihood of nnk_mlpg_traj_ll, without / with its
+// gradients (mlpg_kernel only).
+enum { MODE_FWD = 0, MODE_GRAD = 1, MODE_SOLVE = 2, MODE_GV = 3, MODE_TLL = 4, MODE_TLL_GRAD = 5 };
 
-// scratch columns per frame of one work item: the S + 1 factor columns, and in MODE_GV four more
-// (pivot d, c_m, and the current / trial trajectory)
+// scratch columns per frame of one work item: the S + 1 factor columns, in MODE_GV four more (pivot d, c_m, and
+// the current / trial trajectory), in the MODE_TLL pair one more (1 / d)
 template <int MODE, int NT>
 struct WsCols {
-  static constexpr int value = NT + (MODE == MODE_GV ? 4 : 0);
+  static constexpr int value = NT + (MODE == MODE_GV ? 4 : (MODE == MODE_TLL || MODE == MODE_TLL_GRAD) ? 1 : 0);
 };
 
 template <int NW, int L, int U>
@@ -47,6 +49,34 @@ struct MlpgParams {
   const double* gv_var;
   double gv_step, gv_weight;
   int gv_n_iter;
+};
+
+// MODE_TLL / MODE_TLL_GRAD: MlpgParams plus the targets and outputs of nnk_traj_ll_t.  Only those instances take
+// it (KernelParams), so every other instance keeps MlpgParams and its parameter layout.
+template <typename Tin, int NW, int L, int U>
+struct TllParams : MlpgParams<Tin, NW, L, U> {
+  const Tin* targets;
+  int64_t tgt_ld;
+  double* ll;  // (n_utt, n_chain)
+  Tin* grad_means;
+  int64_t gm_ld;
+  void* grad_vars;  // Tin rows of gv_ld, or (n_utt, gv_ld) float64 partials for global variances
+  int64_t gv_ld;
+  Tin* grad_targets;
+  int64_t gx_ld;
+};
+
+template <typename Tin, int NW, int L, int U, int MODE>
+struct KernelParams {
+  using type = MlpgParams<Tin, NW, L, U>;
+};
+template <typename Tin, int NW, int L, int U>
+struct KernelParams<Tin, NW, L, U, MODE_TLL> {
+  using type = TllParams<Tin, NW, L, U>;
+};
+template <typename Tin, int NW, int L, int U>
+struct KernelParams<Tin, NW, L, U, MODE_TLL_GRAD> {
+  using type = TllParams<Tin, NW, L, U>;
 };
 
 }  // namespace nnk

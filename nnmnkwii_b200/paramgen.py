@@ -29,6 +29,10 @@ Additive, parameter generation considering the modulation spectrum (DESIGN.md 3.
 Additive, parameter generation from per-frame mixture outputs over all components (DESIGN.md 3.19):
 :func:`mlpg_mixture`, :func:`mlpg_mixture_batch` (csrc/nnk_mix_gen.cu ``nnk_mix_gen``, C ABI
 include/nnk_mix_gen.h).  Not in ``__all__``.
+
+Additive, the log-likelihood of target trajectories under the trajectory model of the MLPG inputs (DESIGN.md
+3.20): :func:`trajectory_log_likelihood`, :func:`trajectory_log_likelihood_batch` (csrc/nnk_mlpg.cu
+``nnk_mlpg_traj_ll``, C ABI include/nnk_traj_ll.h).  Not in ``__all__``.
 """
 import ctypes
 
@@ -1131,3 +1135,185 @@ def unit_variance_mlpg_matrix(windows, T):
             windows_c=_lib.make_windows(windows), in_ld=1, var_ld=0, go_ld=n_chain, out_ld=n_chain,
             dtype_code=_lib.NNK_F64, go_f64=1, n_utt=1, device=device, check=True)
     return out.to(torch.float32).cpu().numpy()
+
+
+# ---------------------------------------------------------------------------------------------------
+# trajectory-model log-likelihood (additive)
+# ---------------------------------------------------------------------------------------------------
+class _NnkTrajLl(ctypes.Structure):
+    """ctypes mirror of nnk_traj_ll_t (include/nnk_traj_ll.h)."""
+    _fields_ = [
+        ("targets", ctypes.c_void_p),
+        ("tgt_ld", ctypes.c_int64),
+        ("ll", ctypes.c_void_p),
+        ("grad", ctypes.c_int32),
+        ("grad_means", ctypes.c_void_p),
+        ("gm_ld", ctypes.c_int64),
+        ("grad_vars", ctypes.c_void_p),
+        ("gv_ld", ctypes.c_int64),
+        ("grad_targets", ctypes.c_void_p),
+        ("gx_ld", ctypes.c_int64),
+    ]
+
+
+def _traj_ll_check(targets, means, variances, windows, lengths, offsets, layout):
+    """Checked shapes of :func:`trajectory_log_likelihood_batch`'s arguments: ``(layout, padded, on_device)``.
+    Raises ValueError for every argument error, before anything touches the device."""
+    from ._device import is_tensor
+    arrays = (targets, means, variances)
+    kinds = [is_tensor(a) for a in arrays]
+    if any(kinds) and not all(kinds):
+        raise ValueError("targets, means and variances must all be NumPy arrays or all torch tensors")
+    on_device = all(kinds)
+    if on_device and not all(a.is_cuda for a in arrays):
+        raise ValueError("torch inputs must be CUDA tensors (there is no CPU fallback)")
+    if not on_device:
+        targets, means, variances = (np.asarray(a) for a in arrays)
+    dts = [str(a.dtype).replace("torch.", "") for a in (targets, means, variances)]
+    if dts[0] != dts[1] or dts[1] != dts[2] or dts[0] not in ("float32", "float64"):
+        raise ValueError("targets, means and variances must share one dtype, float32 or float64 (got %s)" % ", ".join(dts))
+    if means.ndim not in (2, 3):
+        raise ValueError("means must be (sum_T, D) or (B, Tmax, D), got shape %s" % (tuple(means.shape),))
+    padded = means.ndim == 3
+    D = means.shape[-1]
+    if padded and lengths is None:
+        raise ValueError("padded (B, Tmax, D) input needs lengths")
+    if not (variances.ndim == 1 and variances.shape[0] == D) and tuple(variances.shape) != tuple(means.shape):
+        raise ValueError("variances must have the shape of means or be (D,) = (%d,), got %s"
+                         % (D, tuple(variances.shape)))
+    if not isinstance(windows, (list, tuple)) or not 1 <= len(windows) <= _lib.NNK_MAX_WIN:
+        raise ValueError("windows must be a list of 1 to %d (l, u, coeff) triples" % _lib.NNK_MAX_WIN)
+    for w in windows:
+        l, u, c = w
+        if not (0 <= int(l) <= _lib.NNK_MAX_HALF and 0 <= int(u) <= _lib.NNK_MAX_HALF) or \
+                np.asarray(c).size != int(l) + int(u) + 1:
+            raise ValueError("window %r: need 0 <= l, u <= %d and l + u + 1 coefficients" % (w, _lib.NNK_MAX_HALF))
+    if layout is None:
+        layout = StreamLayout.single(D, len(windows))
+    if layout.D_in != D:
+        raise ValueError("layout covers %d input columns, means have %d" % (layout.D_in, D))
+    want = tuple(means.shape[:-1]) + (layout.D_out,)
+    if tuple(targets.shape) != want:
+        raise ValueError("targets must have the shape mlpg_batch returns, %s, got %s" % (want, tuple(targets.shape)))
+    n_rows = means.shape[0] * means.shape[1] if padded else means.shape[0]
+    try:
+        lens = np.asarray(lengths.cpu().numpy() if is_tensor(lengths) else lengths) if lengths is not None else None
+        if padded:
+            if lens.ndim != 1 or len(lens) != means.shape[0] or np.any(lens < 0) or np.any(lens > means.shape[1]):
+                raise ValueError
+        else:
+            off = _offsets_from(lens, offsets, n_rows)
+            if off.ndim != 1 or off[0] != 0 or off[-1] != n_rows or np.any(np.diff(off) < 0):
+                raise ValueError
+    except (ValueError, TypeError, AttributeError):
+        raise ValueError("lengths / offsets do not describe the %d rows of the batch" % n_rows)
+    return layout, padded, on_device
+
+
+def _traj_ll_device(targets, means, variances, windows, lengths, offsets, layout, padded, grad):
+    """One launch of ``nnk_mlpg_traj_ll`` on checked CUDA tensors, on the current stream, with one host
+    synchronisation (the status word).  Returns ``(ll (n_utt, n_chain) float64, lens, grads)``; ``grads`` is
+    ``(g_means, g_vars, g_targets)`` in the layouts of nnk_traj_ll.h (``g_vars`` float64 ``(n_utt, D)`` partials
+    for ``(D,)`` variances), or None."""
+    import torch
+
+    from . import _device as dev
+    device = means.device
+    dev.poll_errors()
+    m, v, x = means.contiguous(), variances.contiguous(), targets.contiguous()
+    D = m.shape[-1]
+    n_rows = m.shape[0] * m.shape[1] if padded else m.shape[0]
+    off, lens, order, max_T, n_utt = _utterance_table(lengths, offsets, n_rows, m.shape[:2] if padded else None)
+    var1d = v.dim() == 1
+    ll = torch.zeros((n_utt, layout.n_chain), dtype=torch.float64, device=device)
+    grads = None
+    if grad:
+        grads = (torch.zeros_like(m), torch.zeros((n_utt, D), dtype=torch.float64, device=device) if var1d
+                 else torch.zeros_like(v), torch.zeros_like(x))
+    if not (n_utt and max_T and layout.n_chain):
+        return ll, lens, grads
+    win = _lib.make_windows(windows)
+    a = _lib.NnkMlpgArgs()
+    a.means, a.vars = m.data_ptr(), v.data_ptr()
+    a.dtype, a.n_utt = dev.torch_dtype_code(m.dtype), n_utt
+    a.in_ld, a.var_ld = D, 0 if var1d else D
+    offsets_d = torch.from_numpy(off).to(device)
+    order_d = torch.from_numpy(order).to(device)
+    lens_d = dev.lengths_on(lens, device) if padded else None
+    a.utt_off, a.order = offsets_d.data_ptr(), order_d.data_ptr()
+    a.utt_len = lens_d.data_ptr() if lens_d is not None else None
+    chains = dev.chains_on_device(layout.chains, device)
+    a.chains, a.n_chain, a.max_T, a.win = chains.data_ptr(), layout.n_chain, max_T, win
+    need = _lib.lib.nnk_mlpg_traj_ll_workspace_bytes(n_utt, layout.n_chain, max_T, ctypes.byref(win))
+    if need == 0:
+        raise NotImplementedError("window set not supported by the CUDA kernels")
+    per_utt = need // n_utt
+    ws = dev.workspace(device, max(per_utt, min(need, max(dev.WORKSPACE_CAP_BYTES, per_utt))))
+    a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
+    status = torch.zeros(1, dtype=torch.int64, device=device)
+    a.status_word = status.data_ptr()
+    t = _NnkTrajLl()
+    t.targets, t.tgt_ld, t.ll, t.grad = x.data_ptr(), layout.D_out, ll.data_ptr(), int(bool(grad))
+    if grad:
+        t.grad_means, t.gm_ld = grads[0].data_ptr(), D
+        t.grad_vars, t.gv_ld = grads[1].data_ptr(), D
+        t.grad_targets, t.gx_ld = grads[2].data_ptr(), layout.D_out
+    _lib.check(_lib.lib.nnk_mlpg_traj_ll(ctypes.byref(a), ctypes.byref(t), dev.current_stream_ptr(device)),
+               "nnk_mlpg_traj_ll")
+    dev.raise_if_failed(status)
+    return ll, lens, grads
+
+
+def _traj_ll_scatter(ll, layout):
+    """(n_utt, n_chain) per-chain log-likelihoods -> (n_utt, D_out), zero in columns no chain solves."""
+    import torch
+    out = torch.zeros((ll.shape[0], layout.D_out), dtype=torch.float64, device=ll.device)
+    if layout.n_chain:
+        out[:, torch.from_numpy(layout.chains["out_col"].astype(np.int64)).to(ll.device)] = ll
+    return out
+
+
+def trajectory_log_likelihood_batch(targets, means, variances, windows, lengths=None, offsets=None, layout=None):
+    r"""Log-likelihood of target trajectories under the trajectory model of the MLPG inputs (additive API).
+
+    Per utterance and smoothed output column, with ``P`` and ``b`` exactly as :func:`mlpg_batch` builds them
+    (its edge rule included) and :math:`\bar c = P^{-1} b` the trajectory it returns, the target static
+    trajectory :math:`x` scores
+
+    .. math:: \ell = \tfrac12 \log\det P - \tfrac12 (x - \bar c)^T P (x - \bar c) - \tfrac T2 \log 2\pi,
+
+    the log-density of :math:`N(x; \bar c, P^{-1})` (Zen, Tokuda & Kitamura 2007).  Use it as an objective
+    measure of an acoustic model or, through :func:`nnmnkwii_b200.autograd.trajectory_log_likelihood`, as a
+    training loss.  See DESIGN.md 3.20.
+
+    Args:
+        targets: natural static trajectories, shaped like :func:`mlpg_batch`'s result (``(sum_T, D_out)`` or
+            ``(B, Tmax, D_out)``); copied columns are not read.
+        means, variances, windows, lengths, offsets, layout: as :func:`mlpg_batch` (flat or padded, per-frame
+            or global ``(D,)`` variances).  All three arrays are NumPy arrays or all CUDA tensors, of one dtype.
+
+    Returns:
+        ``(n_utt, D_out)`` float64 log-likelihoods, zero in copied columns; NumPy for NumPy input, a CUDA
+        tensor for tensors (computed on the current stream).  Arithmetic is float64.  Targets and means are not
+        checked: non-finite values give NaN.  A variance that makes a pivot of ``P`` non-positive raises
+        ``numpy.linalg.LinAlgError`` as :func:`mlpg_batch` does.
+    """
+    import torch
+
+    from . import _device as dev
+    layout, padded, on_device = _traj_ll_check(targets, means, variances, windows, lengths, offsets, layout)
+    dev.require_cuda()
+    if not on_device:
+        device = dev.cuda_device()
+        targets, means, variances = (torch.from_numpy(np.ascontiguousarray(a)).to(device)
+                                     for a in (targets, means, variances))
+    ll, _, _ = _traj_ll_device(targets, means, variances, windows, lengths, offsets, layout, padded, False)
+    out = _traj_ll_scatter(ll, layout)
+    return out if on_device else out.cpu().numpy()
+
+
+def trajectory_log_likelihood(targets, mean_frames, variance_frames, windows):
+    """:func:`trajectory_log_likelihood_batch` of one utterance: ``targets (T, static_dim)``, :func:`mlpg`'s
+    ``(T, D)`` means and variances (or ``(D,)``); returns the ``(static_dim,)`` float64 log-likelihoods."""
+    return trajectory_log_likelihood_batch(targets, mean_frames, variance_frames, windows,
+                                           lengths=[mean_frames.shape[0]])[0]
