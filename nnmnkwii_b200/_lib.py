@@ -291,6 +291,14 @@ TRAJ_LL_SIGNATURES = {
     "nnk_mlpg_traj_ll_workspace_bytes": (size_t, [i32, i32, i32, P(NnkWindows)]),
 }
 
+
+# sampling from the trajectory model (include/nnk_traj_sample.h), in the same library; the nnk_traj_sample_t
+# argument is passed by reference to paramgen's ctypes mirror of it
+TRAJ_SAMPLE_SIGNATURES = {
+    "nnk_mlpg_traj_sample": (ctypes.c_int, [P(NnkMlpgArgs), vp, vp]),
+    "nnk_mlpg_traj_sample_workspace_bytes": (size_t, [i32, i32, i32, P(NnkWindows)]),
+}
+
 class NnkError(RuntimeError):
     pass
 
@@ -306,7 +314,7 @@ def _load():
         raise ImportError("libnnk_b200.so ABI %d != binding ABI %d: rebuild" % (L.nnk_abi_version(), ABI_VERSION))
     for name, (restype, argtypes) in (list(SIGNATURES.items()) + list(MS_SEGMENT_SIGNATURES.items()) +
                                       list(MS_GEN_SIGNATURES.items()) + list(MIX_GEN_SIGNATURES.items()) +
-                                      list(TRAJ_LL_SIGNATURES.items())):
+                                      list(TRAJ_LL_SIGNATURES.items()) + list(TRAJ_SAMPLE_SIGNATURES.items())):
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, argtypes
     return L

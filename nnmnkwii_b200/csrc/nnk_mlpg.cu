@@ -26,6 +26,7 @@
 #include <type_traits>
 
 #include "../../include/nnk_traj_ll.h"
+#include "../../include/nnk_traj_sample.h"
 #include "nnk_mlpg.cuh"
 #include "nnk_mlpg_as.cuh"
 
@@ -165,6 +166,99 @@ __device__ __forceinline__ double sym_at(const double (&sg)[S + 1][S + 1], int a
   return a <= b ? sg[a][b] : sg[b][a];
 }
 
+// ---- sampling from the trajectory model (MODE_SAMPLE, nnk_mlpg_traj_sample) --------------------------------------
+// include/nnk_traj_sample.h is the normative definition of the noise; these two functions restate it.
+// Philox4x32-10 (Salmon et al. 2011); the key bump after the last round is not used.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+    k0 += 0x9E3779B9u;
+    k1 += 0xBB67AE85u;
+  }
+  return c;
+}
+
+// the Box-Muller pair of counter c: zc for the even frame 2 (t >> 1), zs for the odd one
+__device__ __forceinline__ void normal_pair(uint4 c, unsigned long long seed, double& zc, double& zs) {
+  const uint4 r = philox4x32_10(c, (uint32_t)seed, (uint32_t)(seed >> 32));
+  const unsigned long long nu = ((unsigned long long)(r.x >> 6) << 26) | (r.y >> 6);
+  const unsigned long long nv = ((unsigned long long)(r.z >> 6) << 26) | (r.w >> 6);
+  const double u = ((double)nu + 0.5) * 0x1p-52;  // exact: nu < 2^52
+  const double v = (double)nv * 0x1p-52;
+  const double rad = sqrt(-2.0 * log(u));
+  double sn, cs;
+  sincospi(2.0 * v, &sn, &cs);
+  zc = rad * cs;
+  zs = rad * sn;
+}
+
+// One chain (one lane).  The forward sweep has left per frame t, in the lane's scratch column col (stride 32):
+//   0: zs_t = (L^-1 b)_t / d_t,   1..S: l_j[t] = L[t+j][t],   NT: 1 / sqrt(d_t), computed as sqrt(1 / d_t)
+// Each sample is one backward sweep over those factors, MODE_FWD's term for term but for its start value:
+//   y_t = fma(scale * z_{s,t}, 1 / sqrt(d_t), zs_t) - sum_j l_j[t] y_{t+j}   (j = 1 .. S in that order, as fmas)
+// so scale = 0 gives MODE_FWD's trajectory.  Sample s goes to out + s * sample_stride.  The frames of a PF block
+// get their noise first, off the serial chain; one Philox call serves the pair (t, t - 1) for odd t, and an even
+// last frame T - 1 takes the cosine of its own call.  A sample's bits depend on s, never on n_samples.
+template <int S, int NTS, int PF, typename Tout>
+__device__ __forceinline__ void sample_sweeps(const double* ws, int T, int n_samples, int64_t sample_stride,
+                                              uint32_t out_col, uint32_t key, unsigned long long seed, double scale,
+                                              Tout* out, int64_t out_ld) {
+  constexpr int NT = S + 1;
+  auto load = [&](int t, double& z, double(&l)[S + 1], double& isd) {
+    z = 0.0; isd = 0.0;
+#pragma unroll
+    for (int j = 0; j <= S; ++j) l[j] = 0.0;
+    if (t >= 0) {
+      const double* wsp = ws + (size_t)t * (NTS * 32);
+      z = wsp[0];
+#pragma unroll
+      for (int j = 1; j <= S; ++j) l[j] = wsp[j * 32];
+      isd = wsp[NT * 32];
+    }
+  };
+  for (int s = 0; s < n_samples; ++s) {
+    Tout* o = out + (int64_t)s * sample_stride;
+    double yw[S + 1];
+#pragma unroll
+    for (int j = 0; j <= S; ++j) yw[j] = 0.0;
+    double rz[PF], rl[PF][S + 1], ri[PF];
+#pragma unroll
+    for (int j = 0; j < PF; ++j) load(T - 1 - j, rz[j], rl[j], ri[j]);
+    double zc = 0.0;  // the cosine normal of the pair of the last odd frame
+    for (int t0 = T - 1; t0 >= 0; t0 -= PF) {
+      double y0[PF];
+#pragma unroll
+      for (int jj = 0; jj < PF; ++jj) {
+        const int t = t0 - jj;
+        double z = zc;
+        if (t >= 0 && ((t & 1) || t == T - 1)) {
+          double zs;
+          normal_pair(make_uint4((uint32_t)t >> 1, out_col, (uint32_t)s, key), seed, zc, zs);
+          z = (t & 1) ? zs : zc;
+        }
+        y0[jj] = fma(scale * z, ri[jj], rz[jj]);
+      }
+#pragma unroll
+      for (int jj = 0; jj < PF; ++jj) {
+        const int t = t0 - jj;
+        if (t >= 0) {
+#pragma unroll
+          for (int j = S; j > 0; --j) yw[j] = yw[j - 1];
+          double y = y0[jj];
+#pragma unroll
+          for (int j = 1; j <= S; ++j) y = fma(-rl[jj][j], yw[j], y);
+          yw[0] = y;
+          load(t - PF, rz[jj], rl[jj], ri[jj]);
+          st_stream(o + (int64_t)t * out_ld, (Tout)y);
+        }
+      }
+    }
+  }
+}
+
 template <typename Tin, int NW, int L, int U, int MODE, int PF>
 __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typename KernelParams<Tin, NW, L, U, MODE>::type p) {
   constexpr int S = L + U;
@@ -172,7 +266,8 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
   constexpr int NTS = WsCols<MODE, NT>::value;
   constexpr bool TLL = (MODE == MODE_TLL || MODE == MODE_TLL_GRAD);
   constexpr bool TGRAD = (MODE == MODE_TLL_GRAD);
-  constexpr bool FWDLIKE = (MODE == MODE_FWD || MODE == MODE_GV || TLL);  // means in (trajectories out, but TLL)
+  // means in (trajectories out, but TLL)
+  constexpr bool FWDLIKE = (MODE == MODE_FWD || MODE == MODE_GV || TLL || MODE == MODE_SAMPLE);
   const int lane = threadIdx.x;
   const int item = blockIdx.x;
   const int urank = p.urank0 + item / p.n_groups;
@@ -200,6 +295,11 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
   if (active && (ch.flags & 1)) {
     if constexpr (TLL) {
       p.ll[(int64_t)utt * p.n_chain + chain] = 0.0;
+    } else if constexpr (MODE == MODE_SAMPLE) {
+      for (int s = 0; s < p.n_samples; ++s) {
+        Tin* o = reinterpret_cast<Tin*>(p.out) + s * p.sample_stride + orow0 * p.out_ld + ch.out_col;
+        for (int t = 0; t < T; ++t) o[(int64_t)t * p.out_ld] = mptr[(int64_t)t * p.in_ld];
+      }
     } else if (FWDLIKE) {
       Tin* o = reinterpret_cast<Tin*>(p.out) + orow0 * p.out_ld + ch.out_col;
       for (int t = 0; t < T; ++t) o[(int64_t)t * p.out_ld] = mptr[(int64_t)t * p.in_ld];
@@ -336,6 +436,7 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
         if (MODE == MODE_GV) wsp[NT * 32] = d;
         if constexpr (TGRAD) wsp[NT * 32] = ivd;
         if constexpr (TLL) sld += log(d);
+        if constexpr (MODE == MODE_SAMPLE) wsp[NT * 32] = sqrt(ivd);
 #pragma unroll
         for (int k = S; k >= 2; --k) {
           zz[k] = zz[k - 1];
@@ -403,7 +504,9 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
     for (int j = 0; j < PF; ++j) load_tll(T - 1 - j, rx[j], rdi[j]);
   }
 
-  const int t_end = (MODE == MODE_GRAD || MODE == MODE_TLL) ? -L : (MODE == MODE_TLL_GRAD) ? -S : 0;
+  // MODE_SAMPLE runs its own sweeps (sample_sweeps, below) instead of this one
+  const int t_end = (MODE == MODE_GRAD || MODE == MODE_TLL) ? -L : (MODE == MODE_TLL_GRAD) ? -S
+                    : (MODE == MODE_SAMPLE) ? T : 0;
   for (int t0 = T - 1; t0 >= t_end; t0 -= PF) {
 #pragma unroll
     for (int jj = 0; jj < PF; ++jj) {
@@ -562,6 +665,13 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
     }
   }
 
+  if constexpr (MODE == MODE_SAMPLE) {
+    if (solve)
+      sample_sweeps<S, NTS, PF>(ws, T, p.n_samples, p.sample_stride, (uint32_t)ch.out_col,
+                                p.keys ? p.keys[utt] : (uint32_t)utt, p.seed, p.scale,
+                                reinterpret_cast<Tin*>(p.out) + orow0 * p.out_ld + ch.out_col, p.out_ld);
+  }
+
   if constexpr (MODE == MODE_GV) {
     if (solve) {
       Tin* o = reinterpret_cast<Tin*>(p.out) + orow0 * p.out_ld + ch.out_col;
@@ -644,7 +754,7 @@ static int launch_as(const MlpgParams<Tin, NW, L, U>& p, const AsGeom& g, size_t
 
 template <typename Tin, int NW, int L, int U, int MODE>
 static int launch_mlpg(const nnk_mlpg_args_t& a, const nnk_mlpg_gv_t* gv, cudaStream_t st,
-                       const nnk_traj_ll_t* tl = nullptr) {
+                       const nnk_traj_ll_t* tl = nullptr, const nnk_traj_sample_t* ts = nullptr) {
   constexpr int NT = L + U + 1;
   constexpr int NTS = WsCols<MODE, NT>::value;
   constexpr int PF = (L + U <= 2) ? 4 : 2;
@@ -656,6 +766,10 @@ static int launch_mlpg(const nnk_mlpg_args_t& a, const nnk_mlpg_gv_t* gv, cudaSt
     p.grad_means = (Tin*)tl->grad_means; p.gm_ld = tl->gm_ld;
     p.grad_vars = tl->grad_vars; p.gv_ld = tl->gv_ld;
     p.grad_targets = (Tin*)tl->grad_targets; p.gx_ld = tl->gx_ld;
+  }
+  if constexpr (MODE == MODE_SAMPLE) {
+    p.sample_stride = ts->sample_stride; p.n_samples = ts->n_samples; p.seed = ts->seed; p.keys = ts->keys;
+    p.scale = ts->scale;
   }
   if (!fill_wintab<NW, L, U>(a.win, p.win)) { set_error("window set does not fit kernel instance"); return NNK_ERR_UNSUPPORTED; }
   p.means = (const Tin*)a.means; p.vars = (const Tin*)a.vars; p.go = a.grad_out; p.go_f64 = a.go_f64; p.out = a.out;
@@ -715,17 +829,17 @@ static int launch_mlpg(const nnk_mlpg_args_t& a, const nnk_mlpg_gv_t* gv, cudaSt
 
 template <typename Tin, int MODE>
 static int dispatch_inst(const nnk_mlpg_args_t& a, cudaStream_t st, const nnk_mlpg_gv_t* gv = nullptr,
-                         const nnk_traj_ll_t* tl = nullptr) {
+                         const nnk_traj_ll_t* tl = nullptr, const nnk_traj_sample_t* ts = nullptr) {
   int inst = -1;
   if (pick_instance(a.win, inst) < 0) {
     set_error("unsupported window set: nw=%d (max %d) or half-width > %d", a.win.nw, NNK_MAX_WIN, NNK_MAX_HALF);
     return NNK_ERR_UNSUPPORTED;
   }
   switch (inst) {
-    case 0: return launch_mlpg<Tin, 1, 0, 0, MODE>(a, gv, st, tl);
-    case 1: return launch_mlpg<Tin, 3, 1, 1, MODE>(a, gv, st, tl);
-    case 2: return launch_mlpg<Tin, 3, 2, 2, MODE>(a, gv, st, tl);
-    default: return launch_mlpg<Tin, NNK_MAX_WIN, NNK_MAX_HALF, NNK_MAX_HALF, MODE>(a, gv, st, tl);
+    case 0: return launch_mlpg<Tin, 1, 0, 0, MODE>(a, gv, st, tl, ts);
+    case 1: return launch_mlpg<Tin, 3, 1, 1, MODE>(a, gv, st, tl, ts);
+    case 2: return launch_mlpg<Tin, 3, 2, 2, MODE>(a, gv, st, tl, ts);
+    default: return launch_mlpg<Tin, NNK_MAX_WIN, NNK_MAX_HALF, NNK_MAX_HALF, MODE>(a, gv, st, tl, ts);
   }
 }
 
@@ -765,6 +879,11 @@ extern "C" size_t nnk_mlpg_gv_workspace_bytes(int32_t n_utt, int32_t n_chain, in
 extern "C" size_t nnk_mlpg_traj_ll_workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T,
                                                    const nnk_windows_t* win) {
   return workspace_bytes(n_utt, n_chain, max_T, win, WsCols<MODE_TLL, 0>::value);
+}
+
+extern "C" size_t nnk_mlpg_traj_sample_workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T,
+                                                       const nnk_windows_t* win) {
+  return workspace_bytes(n_utt, n_chain, max_T, win, WsCols<MODE_SAMPLE, 0>::value);
 }
 
 #ifdef NNK_AS_PROF
@@ -837,4 +956,18 @@ extern "C" int nnk_mlpg_traj_ll(const nnk_mlpg_args_t* a, const nnk_traj_ll_t* t
                                : dispatch_inst<double, MODE_TLL_GRAD>(*a, st, nullptr, tl);
   return a->dtype == NNK_F32 ? dispatch_inst<float, MODE_TLL>(*a, st, nullptr, tl)
                              : dispatch_inst<double, MODE_TLL>(*a, st, nullptr, tl);
+}
+
+extern "C" int nnk_mlpg_traj_sample(const nnk_mlpg_args_t* a, const nnk_traj_sample_t* ts, void* stream) {
+  NNK_REQUIRE(ts != nullptr, NNK_ERR_ARG, "ts is NULL");
+  int r = check_args(a, false);
+  if (r < 0) return r;
+  NNK_REQUIRE(ts->n_samples >= 1, NNK_ERR_ARG, "n_samples must be >= 1");
+  NNK_REQUIRE(ts->sample_stride >= 0, NNK_ERR_ARG, "sample_stride must be >= 0");
+  NNK_REQUIRE(ts->scale >= 0.0 && ts->scale <= 1.7976931348623157e308, NNK_ERR_ARG, "scale must be finite and >= 0");
+  if (r > 0) return NNK_OK;
+  DeviceGuard guard(a->out);
+  cudaStream_t st = (cudaStream_t)stream;
+  return a->dtype == NNK_F32 ? dispatch_inst<float, MODE_SAMPLE>(*a, st, nullptr, nullptr, ts)
+                             : dispatch_inst<double, MODE_SAMPLE>(*a, st, nullptr, nullptr, ts);
 }

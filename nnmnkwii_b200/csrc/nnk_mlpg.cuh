@@ -6,14 +6,16 @@ namespace nnk {
 
 // MODE_GV: the forward solve followed by the global-variance refinement of nnk_mlpg_gv (mlpg_kernel only).
 // MODE_TLL / MODE_TLL_GRAD: the trajectory-model log-likelihood of nnk_mlpg_traj_ll, without / with its
-// gradients (mlpg_kernel only).
-enum { MODE_FWD = 0, MODE_GRAD = 1, MODE_SOLVE = 2, MODE_GV = 3, MODE_TLL = 4, MODE_TLL_GRAD = 5 };
+// gradients (mlpg_kernel only).  MODE_SAMPLE: samples of the trajectory model of nnk_mlpg_traj_sample (mlpg_kernel
+// only).
+enum { MODE_FWD = 0, MODE_GRAD = 1, MODE_SOLVE = 2, MODE_GV = 3, MODE_TLL = 4, MODE_TLL_GRAD = 5, MODE_SAMPLE = 6 };
 
 // scratch columns per frame of one work item: the S + 1 factor columns, in MODE_GV four more (pivot d, c_m, and
-// the current / trial trajectory), in the MODE_TLL pair one more (1 / d)
+// the current / trial trajectory), in the MODE_TLL pair one more (1 / d), in MODE_SAMPLE one more (1 / sqrt(d))
 template <int MODE, int NT>
 struct WsCols {
-  static constexpr int value = NT + (MODE == MODE_GV ? 4 : (MODE == MODE_TLL || MODE == MODE_TLL_GRAD) ? 1 : 0);
+  static constexpr int value =
+      NT + (MODE == MODE_GV ? 4 : (MODE == MODE_TLL || MODE == MODE_TLL_GRAD || MODE == MODE_SAMPLE) ? 1 : 0);
 };
 
 template <int NW, int L, int U>
@@ -66,6 +68,16 @@ struct TllParams : MlpgParams<Tin, NW, L, U> {
   int64_t gx_ld;
 };
 
+// MODE_SAMPLE: MlpgParams plus the sample count, stride, seed, keys and scale of nnk_traj_sample_t
+template <typename Tin, int NW, int L, int U>
+struct SampleParams : MlpgParams<Tin, NW, L, U> {
+  int64_t sample_stride;  // elements between samples in out
+  int n_samples;
+  unsigned long long seed;
+  const uint32_t* keys;  // (n_utt,) or NULL: key_u = u
+  double scale;
+};
+
 template <typename Tin, int NW, int L, int U, int MODE>
 struct KernelParams {
   using type = MlpgParams<Tin, NW, L, U>;
@@ -77,6 +89,10 @@ struct KernelParams<Tin, NW, L, U, MODE_TLL> {
 template <typename Tin, int NW, int L, int U>
 struct KernelParams<Tin, NW, L, U, MODE_TLL_GRAD> {
   using type = TllParams<Tin, NW, L, U>;
+};
+template <typename Tin, int NW, int L, int U>
+struct KernelParams<Tin, NW, L, U, MODE_SAMPLE> {
+  using type = SampleParams<Tin, NW, L, U>;
 };
 
 }  // namespace nnk

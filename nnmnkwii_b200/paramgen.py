@@ -33,6 +33,10 @@ include/nnk_mix_gen.h).  Not in ``__all__``.
 Additive, the log-likelihood of target trajectories under the trajectory model of the MLPG inputs (DESIGN.md
 3.20): :func:`trajectory_log_likelihood`, :func:`trajectory_log_likelihood_batch` (csrc/nnk_mlpg.cu
 ``nnk_mlpg_traj_ll``, C ABI include/nnk_traj_ll.h).  Not in ``__all__``.
+
+Additive, samples from that trajectory model with counter-based noise (DESIGN.md 3.21): :func:`trajectory_sample`,
+:func:`trajectory_sample_batch` (csrc/nnk_mlpg.cu ``nnk_mlpg_traj_sample``, C ABI include/nnk_traj_sample.h).  Not
+in ``__all__``.
 """
 import ctypes
 
@@ -1158,9 +1162,10 @@ class _NnkTrajLl(ctypes.Structure):
 
 def _traj_ll_check(targets, means, variances, windows, lengths, offsets, layout):
     """Checked shapes of :func:`trajectory_log_likelihood_batch`'s arguments: ``(layout, padded, on_device)``.
-    Raises ValueError for every argument error, before anything touches the device."""
+    Raises ValueError for every argument error, before anything touches the device.  With ``targets=None`` it
+    checks the means, variances, windows, lengths and layout alone (:func:`trajectory_sample_batch`)."""
     from ._device import is_tensor
-    arrays = (targets, means, variances)
+    arrays = tuple(a for a in (targets, means, variances) if a is not None)
     kinds = [is_tensor(a) for a in arrays]
     if any(kinds) and not all(kinds):
         raise ValueError("targets, means and variances must all be NumPy arrays or all torch tensors")
@@ -1168,9 +1173,9 @@ def _traj_ll_check(targets, means, variances, windows, lengths, offsets, layout)
     if on_device and not all(a.is_cuda for a in arrays):
         raise ValueError("torch inputs must be CUDA tensors (there is no CPU fallback)")
     if not on_device:
-        targets, means, variances = (np.asarray(a) for a in arrays)
-    dts = [str(a.dtype).replace("torch.", "") for a in (targets, means, variances)]
-    if dts[0] != dts[1] or dts[1] != dts[2] or dts[0] not in ("float32", "float64"):
+        targets, means, variances = (None if a is None else np.asarray(a) for a in (targets, means, variances))
+    dts = [str(a.dtype).replace("torch.", "") for a in (targets, means, variances) if a is not None]
+    if len(set(dts)) != 1 or dts[0] not in ("float32", "float64"):
         raise ValueError("targets, means and variances must share one dtype, float32 or float64 (got %s)" % ", ".join(dts))
     if means.ndim not in (2, 3):
         raise ValueError("means must be (sum_T, D) or (B, Tmax, D), got shape %s" % (tuple(means.shape),))
@@ -1193,7 +1198,7 @@ def _traj_ll_check(targets, means, variances, windows, lengths, offsets, layout)
     if layout.D_in != D:
         raise ValueError("layout covers %d input columns, means have %d" % (layout.D_in, D))
     want = tuple(means.shape[:-1]) + (layout.D_out,)
-    if tuple(targets.shape) != want:
+    if targets is not None and tuple(targets.shape) != want:
         raise ValueError("targets must have the shape mlpg_batch returns, %s, got %s" % (want, tuple(targets.shape)))
     n_rows = means.shape[0] * means.shape[1] if padded else means.shape[0]
     try:
@@ -1223,7 +1228,8 @@ def _traj_ll_device(targets, means, variances, windows, lengths, offsets, layout
     m, v, x = means.contiguous(), variances.contiguous(), targets.contiguous()
     D = m.shape[-1]
     n_rows = m.shape[0] * m.shape[1] if padded else m.shape[0]
-    off, lens, order, max_T, n_utt = _utterance_table(lengths, offsets, n_rows, m.shape[:2] if padded else None)
+    table = _utterance_table(lengths, offsets, n_rows, m.shape[:2] if padded else None)
+    _, lens, _, max_T, n_utt = table
     var1d = v.dim() == 1
     ll = torch.zeros((n_utt, layout.n_chain), dtype=torch.float64, device=device)
     grads = None
@@ -1232,26 +1238,7 @@ def _traj_ll_device(targets, means, variances, windows, lengths, offsets, layout
                  else torch.zeros_like(v), torch.zeros_like(x))
     if not (n_utt and max_T and layout.n_chain):
         return ll, lens, grads
-    win = _lib.make_windows(windows)
-    a = _lib.NnkMlpgArgs()
-    a.means, a.vars = m.data_ptr(), v.data_ptr()
-    a.dtype, a.n_utt = dev.torch_dtype_code(m.dtype), n_utt
-    a.in_ld, a.var_ld = D, 0 if var1d else D
-    offsets_d = torch.from_numpy(off).to(device)
-    order_d = torch.from_numpy(order).to(device)
-    lens_d = dev.lengths_on(lens, device) if padded else None
-    a.utt_off, a.order = offsets_d.data_ptr(), order_d.data_ptr()
-    a.utt_len = lens_d.data_ptr() if lens_d is not None else None
-    chains = dev.chains_on_device(layout.chains, device)
-    a.chains, a.n_chain, a.max_T, a.win = chains.data_ptr(), layout.n_chain, max_T, win
-    need = _lib.lib.nnk_mlpg_traj_ll_workspace_bytes(n_utt, layout.n_chain, max_T, ctypes.byref(win))
-    if need == 0:
-        raise NotImplementedError("window set not supported by the CUDA kernels")
-    per_utt = need // n_utt
-    ws = dev.workspace(device, max(per_utt, min(need, max(dev.WORKSPACE_CAP_BYTES, per_utt))))
-    a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-    status = torch.zeros(1, dtype=torch.int64, device=device)
-    a.status_word = status.data_ptr()
+    a, keep, status = _traj_args(m, v, windows, table, layout, padded, _lib.lib.nnk_mlpg_traj_ll_workspace_bytes)
     t = _NnkTrajLl()
     t.targets, t.tgt_ld, t.ll, t.grad = x.data_ptr(), layout.D_out, ll.data_ptr(), int(bool(grad))
     if grad:
@@ -1262,6 +1249,40 @@ def _traj_ll_device(targets, means, variances, windows, lengths, offsets, layout
                "nnk_mlpg_traj_ll")
     dev.raise_if_failed(status)
     return ll, lens, grads
+
+
+def _traj_args(m, v, windows, table, layout, padded, sizing):
+    """``(args, keep, status)``: the nnk_mlpg_args_t of contiguous CUDA means and variances and the batch table
+    ``table`` of :func:`_utterance_table`, with a workspace sized by ``sizing`` (``nnk_mlpg_traj_*_workspace_bytes``,
+    capped at ``_device.WORKSPACE_CAP_BYTES`` but never below one utterance) and a zeroed status word.  ``keep``
+    holds the device tables the launch reads."""
+    import torch
+
+    from . import _device as dev
+    device = m.device
+    off, lens, order, max_T, n_utt = table
+    D = m.shape[-1]
+    win = _lib.make_windows(windows)
+    a = _lib.NnkMlpgArgs()
+    a.means, a.vars = m.data_ptr(), v.data_ptr()
+    a.dtype, a.n_utt = dev.torch_dtype_code(m.dtype), n_utt
+    a.in_ld, a.var_ld = D, 0 if v.dim() == 1 else D
+    offsets_d = torch.from_numpy(off).to(device)
+    order_d = torch.from_numpy(order).to(device)
+    lens_d = dev.lengths_on(lens, device) if padded else None
+    a.utt_off, a.order = offsets_d.data_ptr(), order_d.data_ptr()
+    a.utt_len = lens_d.data_ptr() if lens_d is not None else None
+    chains = dev.chains_on_device(layout.chains, device)
+    a.chains, a.n_chain, a.max_T, a.win = chains.data_ptr(), layout.n_chain, max_T, win
+    need = sizing(n_utt, layout.n_chain, max_T, ctypes.byref(win))
+    if need == 0:
+        raise NotImplementedError("window set not supported by the CUDA kernels")
+    per_utt = need // n_utt
+    ws = dev.workspace(device, max(per_utt, min(need, max(dev.WORKSPACE_CAP_BYTES, per_utt))))
+    a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
+    status = torch.zeros(1, dtype=torch.int64, device=device)
+    a.status_word = status.data_ptr()
+    return a, (offsets_d, order_d, lens_d, chains, ws), status
 
 
 def _traj_ll_scatter(ll, layout):
@@ -1317,3 +1338,124 @@ def trajectory_log_likelihood(targets, mean_frames, variance_frames, windows):
     ``(T, D)`` means and variances (or ``(D,)``); returns the ``(static_dim,)`` float64 log-likelihoods."""
     return trajectory_log_likelihood_batch(targets, mean_frames, variance_frames, windows,
                                            lengths=[mean_frames.shape[0]])[0]
+
+
+# ---------------------------------------------------------------------------------------------------
+# sampling from the trajectory model (additive)
+# ---------------------------------------------------------------------------------------------------
+class _NnkTrajSample(ctypes.Structure):
+    """ctypes mirror of nnk_traj_sample_t (include/nnk_traj_sample.h)."""
+    _fields_ = [
+        ("sample_stride", ctypes.c_int64),
+        ("n_samples", ctypes.c_int32),
+        ("seed", ctypes.c_uint64),
+        ("keys", ctypes.c_void_p),
+        ("scale", ctypes.c_double),
+    ]
+
+
+def _is_int(x):
+    return isinstance(x, (int, np.integer)) and not isinstance(x, (bool, np.bool_))
+
+
+def _traj_sample_check(n_samples, seed, keys, scale, n_utt):
+    """Checked ``(n_samples, seed, keys (uint32 array or None), scale)`` of :func:`trajectory_sample_batch`; raises
+    ValueError for every argument error."""
+    from ._device import is_tensor
+    if not _is_int(n_samples) or not 1 <= int(n_samples) < 2 ** 31:
+        raise ValueError("n_samples must be an int in [1, 2^31), got %r" % (n_samples,))
+    if not _is_int(seed) or not 0 <= int(seed) < 2 ** 64:
+        raise ValueError("seed must be an int in [0, 2^64), got %r" % (seed,))
+    if keys is not None:
+        k = np.asarray(keys.detach().cpu().numpy() if is_tensor(keys) else keys)
+        if k.shape != (n_utt,) or (k.size and (not np.issubdtype(k.dtype, np.integer) or k.min() < 0
+                                               or int(k.max()) >= 2 ** 32)):
+            raise ValueError("keys must be %d integers in [0, 2^32), one per utterance" % n_utt)
+        keys = k.astype(np.uint32)
+    try:
+        scale = float(scale)
+    except (TypeError, ValueError):
+        raise ValueError("scale must be a finite number >= 0, got %r" % (scale,))
+    if not (np.isfinite(scale) and scale >= 0.0):
+        raise ValueError("scale must be a finite number >= 0, got %r" % (scale,))
+    return int(n_samples), int(seed), keys, scale
+
+
+def _traj_sample_device(means, variances, windows, table, layout, padded, n_samples, seed, keys, scale):
+    """One launch of ``nnk_mlpg_traj_sample`` per workspace wave on checked CUDA tensors, on the current stream,
+    with one host synchronisation (the status word).  Returns the ``(n_samples,) + mlpg_batch`` shaped samples."""
+    import torch
+
+    from . import _device as dev
+    device = means.device
+    dev.poll_errors()
+    m, v = means.contiguous(), variances.contiguous()
+    _, _, _, max_T, n_utt = table
+    out = torch.zeros((n_samples,) + tuple(m.shape[:-1]) + (layout.D_out,), dtype=m.dtype, device=device)
+    if not (n_utt and max_T and layout.n_chain):
+        return out
+    a, keep, status = _traj_args(m, v, windows, table, layout, padded, _lib.lib.nnk_mlpg_traj_sample_workspace_bytes)
+    a.out, a.out_ld = out.data_ptr(), layout.D_out
+    keys_d = torch.from_numpy(keys.view(np.int32)).to(device) if keys is not None else None
+    t = _NnkTrajSample()
+    t.sample_stride, t.n_samples, t.seed, t.scale = out[0].numel(), n_samples, seed, scale
+    t.keys = keys_d.data_ptr() if keys_d is not None else None
+    _lib.check(_lib.lib.nnk_mlpg_traj_sample(ctypes.byref(a), ctypes.byref(t), dev.current_stream_ptr(device)),
+               "nnk_mlpg_traj_sample")
+    dev.raise_if_failed(status)
+    return out
+
+
+def trajectory_sample_batch(means, variances, windows, n_samples=1, seed=0, keys=None, scale=1.0, lengths=None,
+                            offsets=None, layout=None):
+    r"""Samples from the trajectory model of the MLPG inputs (additive API).
+
+    Per utterance and smoothed output column, with ``P`` and ``b`` exactly as :func:`mlpg_batch` builds them (its
+    edge rule included) and :math:`\bar c = P^{-1} b` the trajectory it returns, each sample is a draw of
+    :math:`N(\bar c, \mathrm{scale}^2 P^{-1})` (Zen, Tokuda & Kitamura 2007): the static trajectories the model
+    that :func:`trajectory_log_likelihood_batch` scores spreads around its mode.  ``scale = 0`` gives
+    :func:`mlpg_batch`'s result in every sample.  See DESIGN.md 3.21.
+
+    The noise is counter-based (Philox4x32-10, Box-Muller; include/nnk_traj_sample.h defines it bit for bit): a
+    draw is a pure function of ``(seed, key, sample index, frame, output column)``.  It does not depend on the
+    batch around an utterance, its padding, the dtype or ``n_samples``: the first ``k`` of 16 samples are the
+    ``k`` samples of ``n_samples = k``.
+
+    Args:
+        means, variances, windows, lengths, offsets, layout: as :func:`mlpg_batch` (flat or padded, per-frame or
+            global ``(D,)`` variances).  Both arrays are NumPy arrays or both CUDA tensors, of one dtype.
+        n_samples: samples per utterance, an int in [1, 2^31).
+        seed: an int in [0, 2^64).
+        keys: ``n_utt`` integers in [0, 2^32), the key of each utterance's noise (for example its index in the
+            dataset, so that a draw does not depend on how the batch was shuffled).  Default: the utterance's
+            index in the batch (the order of ``offsets``, or the batch index of padded input).
+        scale: multiplies the standard deviation; finite and >= 0.
+
+    Returns:
+        ``(n_samples,) + mlpg_batch's result shape`` in the input dtype: NumPy for NumPy input, a CUDA tensor
+        for tensors (computed on the current stream).  Copied columns repeat the means in every sample; padded
+        tail rows are zero.  Arithmetic is float64.  A variance that makes a pivot of ``P`` non-positive raises
+        ``numpy.linalg.LinAlgError`` as :func:`mlpg_batch` does.
+    """
+    import torch
+
+    from . import _device as dev
+    layout, padded, on_device = _traj_ll_check(None, means, variances, windows, lengths, offsets, layout)
+    if not on_device:
+        means, variances = np.asarray(means), np.asarray(variances)
+    n_rows = means.shape[0] * means.shape[1] if padded else means.shape[0]
+    table = _utterance_table(lengths, offsets, n_rows, tuple(means.shape[:2]) if padded else None)
+    n_samples, seed, keys, scale = _traj_sample_check(n_samples, seed, keys, scale, table[4])
+    dev.require_cuda()
+    if not on_device:
+        device = dev.cuda_device()
+        means, variances = (torch.from_numpy(np.ascontiguousarray(a)).to(device) for a in (means, variances))
+    out = _traj_sample_device(means, variances, windows, table, layout, padded, n_samples, seed, keys, scale)
+    return out if on_device else out.cpu().numpy()
+
+
+def trajectory_sample(mean_frames, variance_frames, windows, n_samples=1, seed=0, scale=1.0):
+    """:func:`trajectory_sample_batch` of one utterance (key 0): :func:`mlpg`'s ``(T, D)`` means and variances
+    (or ``(D,)``); returns the ``(n_samples, T, static_dim)`` samples."""
+    return trajectory_sample_batch(mean_frames, variance_frames, windows, n_samples=n_samples, seed=seed,
+                                   scale=scale, lengths=[mean_frames.shape[0]])
