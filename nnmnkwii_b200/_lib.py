@@ -299,6 +299,14 @@ TRAJ_SAMPLE_SIGNATURES = {
     "nnk_mlpg_traj_sample_workspace_bytes": (size_t, [i32, i32, i32, P(NnkWindows)]),
 }
 
+
+# the gradient of MLPG in its means and variances (include/nnk_mlpg_vjp.h), in the same library; the
+# nnk_mlpg_vjp_t argument is passed by reference to paramgen's ctypes mirror of it
+VJP_SIGNATURES = {
+    "nnk_mlpg_vjp": (ctypes.c_int, [P(NnkMlpgArgs), vp, vp]),
+    "nnk_mlpg_vjp_workspace_bytes": (size_t, [i32, i32, i32, P(NnkWindows)]),
+}
+
 class NnkError(RuntimeError):
     pass
 
@@ -314,7 +322,8 @@ def _load():
         raise ImportError("libnnk_b200.so ABI %d != binding ABI %d: rebuild" % (L.nnk_abi_version(), ABI_VERSION))
     for name, (restype, argtypes) in (list(SIGNATURES.items()) + list(MS_SEGMENT_SIGNATURES.items()) +
                                       list(MS_GEN_SIGNATURES.items()) + list(MIX_GEN_SIGNATURES.items()) +
-                                      list(TRAJ_LL_SIGNATURES.items()) + list(TRAJ_SAMPLE_SIGNATURES.items())):
+                                      list(TRAJ_LL_SIGNATURES.items()) + list(TRAJ_SAMPLE_SIGNATURES.items()) +
+                                      list(VJP_SIGNATURES.items())):
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, argtypes
     return L

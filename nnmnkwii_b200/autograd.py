@@ -11,6 +11,8 @@ Differences that are additions, not signature changes:
 
 Additive, not in ``__all__``: ``TrajectoryLogLikelihood`` / ``trajectory_log_likelihood``, the log-likelihood of
 target trajectories under the trajectory model of the MLPG inputs, differentiable in targets, means and variances.
+``MLPGWithVariances`` / ``mlpg_with_variances``: MLPG differentiable in its means and its variances, for minimum
+generation error training of models that predict variances.
 
 The modulation-spectrum part (nnmnkwii/autograd/_impl/modspec.py): ``ModSpec`` and ``modspec``, plus the batched
 ``ModSpecBatch`` / ``modspec_batch``, on csrc/nnk_modspec.cu.
@@ -208,7 +210,7 @@ def modspec_batch(y, lengths, n=2048, norm=None):
 class TrajectoryLogLikelihood(Function):
     """Additive: the trajectory-model log-likelihood of :func:`nnmnkwii_b200.paramgen.trajectory_log_likelihood_batch`
     as an autograd function, ``f : (targets, means, variances) -> (B, D_out)`` float64, differentiable in all three
-    (the variance gradient is what :class:`MLPG` and :class:`MLPGBatch` do not give).  CUDA tensors, flat
+    (:class:`MLPGWithVariances` gives the variance gradient of a generation error).  CUDA tensors, flat
     ``(sum_T, D)`` or zero-padded ``(B, Tmax, D)`` with ``lengths``; variances per frame or global ``(D,)``;
     ``targets`` shaped like :func:`mlpg_batch`'s result.  The forward is one kernel launch, with the gradients
     computed in the same launch only when an input needs them; the backward scales them by ``grad_output[u, column]``
@@ -264,6 +266,41 @@ class TrajectoryLogLikelihood(Function):
 def trajectory_log_likelihood(targets, means, variances, windows, lengths, layout=None):
     """Additive: differentiable trajectory-model log-likelihood (see :class:`TrajectoryLogLikelihood`)."""
     return TrajectoryLogLikelihood.apply(targets, means, variances, windows, lengths, layout)
+
+
+class MLPGWithVariances(Function):
+    """Additive: MLPG differentiable in its means and its variances, ``f : (means, variances) -> mlpg_batch(...)``,
+    for minimum generation error training (Wu & Wang 2006) of models that predict variances.  :class:`MLPG` and
+    :class:`MLPGBatch` return no variance gradient.
+
+    CUDA tensors only, of one dtype (float32 or float64): flat ``(sum_T, D)`` with ``lengths`` (a 2-D input without
+    ``lengths`` is one utterance) or zero-padded ``(B, Tmax, D)`` with ``lengths``; variances per frame or global
+    ``(D,)``; any :class:`~nnmnkwii_b200.paramgen.StreamLayout`.  The forward is
+    :func:`nnmnkwii_b200.paramgen.mlpg_batch` (the same bits) in the means' dtype; the backward is one kernel launch
+    of :func:`nnmnkwii_b200.paramgen.mlpg_vjp_batch`.  A stride-0 ``v.expand(T, D)`` is materialised and gets true
+    per-frame gradients, which autograd sums back through the expand."""
+
+    @staticmethod
+    def forward(ctx, means, variances, windows, lengths, layout=None):
+        layout, padded, on_device = G._traj_ll_check(None, means, variances, windows, lengths, None, layout)
+        if not on_device:
+            raise ValueError("MLPGWithVariances takes CUDA tensors")
+        m, v = means.detach(), variances.detach().contiguous()
+        ctx.windows, ctx.lengths, ctx.layout = windows, lengths, layout
+        ctx.save_for_backward(m, v)
+        return G.mlpg_batch(m, v, windows, lengths=lengths, layout=layout)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        m, v = ctx.saved_tensors
+        g_m, g_v = G.mlpg_vjp_batch(m, v, ctx.windows, grad_output.to(m.dtype), lengths=ctx.lengths,
+                                    layout=ctx.layout)
+        return (g_m if ctx.needs_input_grad[0] else None), (g_v if ctx.needs_input_grad[1] else None), None, None, None
+
+
+def mlpg_with_variances(means, variances, windows, lengths=None, layout=None):
+    """Additive: MLPG differentiable in means and variances (see :class:`MLPGWithVariances`)."""
+    return MLPGWithVariances.apply(means, variances, windows, lengths, layout)
 
 
 def mlpg(means, variances, windows):

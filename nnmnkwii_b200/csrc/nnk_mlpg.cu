@@ -4,6 +4,7 @@
 //   paramgen.mlpg       paramgen/_mlpg.py:92-199  (build_poe :53-89 -> _bandmat/tensor.pyx:20-64,
 //                       82-174; bla.solveh -> _bandmat/linalg.pyx:36-104, 106-176, 290-304)
 //   paramgen.mlpg_grad  paramgen/_mlpg.py:202-281 (closed form  tau_w * (W_w P^-1 o), O(T))
+// and, additive, the gradient in the means and the variances together (MODE_VJP, nnk_mlpg_vjp).
 //
 // Mapping: one "chain" = one static dimension of one stream of one utterance = one symmetric
 // banded T x T system  P y = b,  P = sum_w W_w^T diag(tau_w) W_w,  b = sum_w W_w^T (tau_w * mu_w).
@@ -25,6 +26,7 @@
 // (nw == NW), with NT <= 5 and rows narrow enough for as_geometry; everything else runs mlpg_kernel.
 #include <type_traits>
 
+#include "../../include/nnk_mlpg_vjp.h"
 #include "../../include/nnk_traj_ll.h"
 #include "../../include/nnk_traj_sample.h"
 #include "nnk_mlpg.cuh"
@@ -259,6 +261,14 @@ __device__ __forceinline__ void sample_sweeps(const double* ws, int T, int n_sam
   }
 }
 
+// ---- gradient in means and variances (MODE_VJP, nnk_mlpg_vjp) ---------------------------------------------------
+// The forward sweep eliminates two right-hand sides with the same factors: b from the means (MODE_FWD's) and o, the
+// gradient with respect to the trajectory, read at the output's rows and columns (MODE_GRAD's, which reads it by
+// chain); (L^-1 o)_t / d_t goes to scratch column NT.  The backward sweep back-substitutes both, cbar = P^-1 b and
+// g = P^-1 o, keeps windows of them over frames t .. t + S, and at step t emits row r = t + L (as MODE_GRAD does),
+// reloading that row's means and variances:
+//   dL/dmu_{r,w} = tau_{r,w} (W_w g)_r,   dL/dvar_{r,w} = -tau_{r,w}^2 (W_w g)_r (mu_{r,w} - (W_w cbar)_r).
+// Global variances sum dL/dvar over the rows in that order in the lane (TLL_GRAD's partials).
 template <typename Tin, int NW, int L, int U, int MODE, int PF>
 __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typename KernelParams<Tin, NW, L, U, MODE>::type p) {
   constexpr int S = L + U;
@@ -266,8 +276,9 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
   constexpr int NTS = WsCols<MODE, NT>::value;
   constexpr bool TLL = (MODE == MODE_TLL || MODE == MODE_TLL_GRAD);
   constexpr bool TGRAD = (MODE == MODE_TLL_GRAD);
-  // means in (trajectories out, but TLL)
-  constexpr bool FWDLIKE = (MODE == MODE_FWD || MODE == MODE_GV || TLL || MODE == MODE_SAMPLE);
+  constexpr bool VJP = (MODE == MODE_VJP);
+  // means in (trajectories out, but TLL and VJP)
+  constexpr bool FWDLIKE = (MODE == MODE_FWD || MODE == MODE_GV || TLL || MODE == MODE_SAMPLE || VJP);
   const int lane = threadIdx.x;
   const int item = blockIdx.x;
   const int urank = p.urank0 + item / p.n_groups;
@@ -300,6 +311,10 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
         Tin* o = reinterpret_cast<Tin*>(p.out) + s * p.sample_stride + orow0 * p.out_ld + ch.out_col;
         for (int t = 0; t < T; ++t) o[(int64_t)t * p.out_ld] = mptr[(int64_t)t * p.in_ld];
       }
+    } else if constexpr (VJP) {
+      const Tin* go = reinterpret_cast<const Tin*>(p.go) + orow0 * p.go_ld + ch.out_col;
+      Tin* o = p.grad_means + row0 * p.gm_ld + ch.in_col;
+      for (int t = 0; t < T; ++t) o[(int64_t)t * p.gm_ld] = go[(int64_t)t * p.go_ld];
     } else if (FWDLIKE) {
       Tin* o = reinterpret_cast<Tin*>(p.out) + orow0 * p.out_ld + ch.out_col;
       for (int t = 0; t < T; ++t) o[(int64_t)t * p.out_ld] = mptr[(int64_t)t * p.in_ld];
@@ -313,6 +328,8 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
 #pragma unroll
   for (int w = 0; w < NW; ++w) gv[w] = (solve && var_global && w < nw) ? vptr[w * ch.win_stride] : Tin(1);
 
+  // VJP: o of the chain's frame 0, at the output's row and column
+  const Tin* gop = VJP ? reinterpret_cast<const Tin*>(p.go) + orow0 * p.go_ld + ch.out_col : nullptr;
   // raw (un-converted) frame loads; t outside [0, T) or idle lanes give zeros
   auto load_raw = [&](int t, Tin(&m)[NW], Tin(&v)[NW], double& g) {
 #pragma unroll
@@ -326,7 +343,8 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
           v[w] = var_global ? gv[w] : ld_stream(vptr + (int64_t)t * p.var_ld + w * ch.win_stride);
         }
       }
-      if (!FWDLIKE) g = load_go(p.go, p.go_f64, (row0 + t) * p.go_ld + chain);
+      if constexpr (VJP) g = (double)ld_stream(gop + (int64_t)t * p.go_ld);
+      else if (!FWDLIKE) g = load_go(p.go, p.go_f64, (row0 + t) * p.go_ld + chain);
     }
   };
   // tau_w[t] with the reference's edge rule; tm = tau * mu (paramgen/_mlpg.py:188-195)
@@ -344,7 +362,7 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
 
   // ---- forward sweep -----------------------------------------------------------------------------
   double wt[NT][NW], wm[NT][NW];  // wt[i] = tau of frame (t + L - i)
-  double wg[NT];                  // grad/solve mode: right-hand side of frame (t + L - i)
+  double wg[NT];                  // grad/solve mode, VJP: right-hand side (o) of frame (t + L - i)
 #pragma unroll
   for (int i = 0; i < NT; ++i) {
     wg[i] = 0.0;
@@ -365,9 +383,11 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
   for (int j = 0; j < PF; ++j) load_raw(L + j, rm[j], rv[j], rg[j]);
 
   double vcol[S + 1][S + 1], lcol[S + 1][S + 1], zz[S + 1];
+  double zo[S + 1];  // VJP: zz of the second right-hand side, o
 #pragma unroll
   for (int k = 0; k <= S; ++k) {
     zz[k] = 0.0;
+    zo[k] = 0.0;
 #pragma unroll
     for (int j = 0; j <= S; ++j) { vcol[k][j] = 0.0; lcol[k][j] = 0.0; }
   }
@@ -412,18 +432,22 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
         } else {
           bb = wg[L];
         }
+        double bo = 0.0;
+        if constexpr (VJP) bo = wg[L];
         // eliminate: older columns first (their normalised entries are ready) ...
 #pragma unroll
         for (int k = 2; k <= S; ++k) {
 #pragma unroll
           for (int m = 0; m + k <= S; ++m) acc[m] = fma(-vcol[k][k + m], lcol[k][k], acc[m]);
           bb = fma(-lcol[k][k], zz[k], bb);
+          if constexpr (VJP) bo = fma(-lcol[k][k], zo[k], bo);
         }
         // ... the newest column last: only this part waits on the previous pivot's reciprocal
         if (S >= 1) {
 #pragma unroll
           for (int m = 0; m + 1 <= S; ++m) acc[m] = fma(-(vcol[1][1 + m] * vcol[1][1]), iv1, acc[m]);
           bb = fma(-(vcol[1][1] * zz[1]), iv1, bb);
+          if constexpr (VJP) bo = fma(-(vcol[1][1] * zo[1]), iv1, bo);
         }
         const double d = acc[0];
         if (!(d > 0.0) && solve && !reported) {  // linalg.pyx:79-82
@@ -437,14 +461,17 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
         if constexpr (TGRAD) wsp[NT * 32] = ivd;
         if constexpr (TLL) sld += log(d);
         if constexpr (MODE == MODE_SAMPLE) wsp[NT * 32] = sqrt(ivd);
+        if constexpr (VJP) wsp[NT * 32] = bo * ivd;
 #pragma unroll
         for (int k = S; k >= 2; --k) {
           zz[k] = zz[k - 1];
+          if constexpr (VJP) zo[k] = zo[k - 1];
 #pragma unroll
           for (int j = 0; j <= S; ++j) { vcol[k][j] = vcol[k - 1][j]; lcol[k][j] = lcol[k - 1][j]; }
         }
         if (S >= 1) {
           zz[1] = bb;
+          if constexpr (VJP) zo[1] = bo;
 #pragma unroll
           for (int j = 1; j <= S; ++j) {
             vcol[1][j] = acc[j];
@@ -503,9 +530,19 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
 #pragma unroll
     for (int j = 0; j < PF; ++j) load_tll(T - 1 - j, rx[j], rdi[j]);
   }
+  // VJP state: the window of g = P^-1 o (gq[j] = g[t + j]) and the prefetch ring of (L^-1 o)_t / d_t
+  double gq[S + 1], rgo[PF];
+  if constexpr (VJP) {
+#pragma unroll
+    for (int j = 0; j <= S; ++j) gq[j] = 0.0;
+#pragma unroll
+    for (int w = 0; w < NW; ++w) vsum[w] = 0.0;
+#pragma unroll
+    for (int j = 0; j < PF; ++j) rgo[j] = T - 1 - j >= 0 ? ws[(size_t)(T - 1 - j) * (NTS * 32) + NT * 32] : 0.0;
+  }
 
   // MODE_SAMPLE runs its own sweeps (sample_sweeps, below) instead of this one
-  const int t_end = (MODE == MODE_GRAD || MODE == MODE_TLL) ? -L : (MODE == MODE_TLL_GRAD) ? -S
+  const int t_end = (MODE == MODE_GRAD || MODE == MODE_TLL || VJP) ? -L : (MODE == MODE_TLL_GRAD) ? -S
                     : (MODE == MODE_SAMPLE) ? T : 0;
   for (int t0 = T - 1; t0 >= t_end; t0 -= PF) {
 #pragma unroll
@@ -519,6 +556,15 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
         for (int j = 1; j <= S; ++j) y = fma(-rl[jj][j], yw[j], y);
         if (t < 0) y = 0.0;
         yw[0] = y;
+        if constexpr (VJP) {  // the same back substitution for g, before the ring slot is refilled
+#pragma unroll
+          for (int j = S; j > 0; --j) gq[j] = gq[j - 1];
+          double g = rgo[jj];
+#pragma unroll
+          for (int j = 1; j <= S; ++j) g = fma(-rl[jj][j], gq[j], g);
+          gq[0] = t < 0 ? 0.0 : g;
+          rgo[jj] = t - PF >= 0 ? ws[(size_t)(t - PF) * (NTS * 32) + NT * 32] : 0.0;
+        }
         double lt[S + 1];  // TLL_GRAD: l_k[t], before the ring slot is refilled
         if constexpr (TGRAD) {
 #pragma unroll
@@ -618,6 +664,38 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
               p.grad_targets[(orow0 + s) * p.gx_ld + ch.out_col] = (Tin)(-gx);
             }
           }
+        } else if constexpr (VJP) {
+          const int r = t + L;  // >= 0
+          if (r < T && solve) {
+            Tin m[NW], v[NW];
+            double tau[NW], tm[NW];
+#pragma unroll
+            for (int w = 0; w < NW; ++w) { m[w] = Tin(0); v[w] = Tin(1); }
+#pragma unroll
+            for (int w = 0; w < NW; ++w)
+              if (w < nw) {
+                m[w] = mptr[(int64_t)r * p.in_ld + w * ch.win_stride];
+                v[w] = var_global ? gv[w] : vptr[(int64_t)r * p.var_ld + w * ch.win_stride];
+              }
+            to_frame(r, m, v, tau, tm);
+#pragma unroll
+            for (int w = 0; w < NW; ++w) {
+              if (w < nw) {
+                double ug = 0.0, uc = 0.0;
+#pragma unroll
+                for (int i = 0; i < NT; ++i) {  // c[w][L+k], k = i-L: frames r + k = t + i
+                  ug = fma(p.win.c[w][i], gq[i], ug);
+                  uc = fma(p.win.c[w][i], yw[i], uc);
+                }
+                const double gm = tau[w] * ug;
+                const double gvr = -tau[w] * gm * ((double)m[w] - uc);
+                const int64_t col = ch.in_col + w * ch.win_stride;
+                p.grad_means[(row0 + r) * p.gm_ld + col] = (Tin)gm;
+                if (var_global) vsum[w] += gvr;
+                else reinterpret_cast<Tin*>(p.grad_vars)[(row0 + r) * p.gv_ld + col] = (Tin)gvr;
+              }
+            }
+          }
         } else if (MODE == MODE_GV) {
           ws[(size_t)t * (NTS * 32) + (NT + 1) * 32] = y;  // c_m, refined below
         } else if (MODE != MODE_GRAD) {
@@ -662,6 +740,15 @@ __global__ void __launch_bounds__(32) mlpg_kernel(const __grid_constant__ typena
             if (w < nw) gp[w * ch.win_stride] = vsum[w];
         }
       }
+    }
+  }
+
+  if constexpr (VJP) {
+    if (solve && var_global) {
+      double* gp = reinterpret_cast<double*>(p.grad_vars) + (int64_t)utt * p.gv_ld + ch.in_col;
+#pragma unroll
+      for (int w = 0; w < NW; ++w)
+        if (w < nw) gp[w * ch.win_stride] = vsum[w];
     }
   }
 
@@ -754,7 +841,8 @@ static int launch_as(const MlpgParams<Tin, NW, L, U>& p, const AsGeom& g, size_t
 
 template <typename Tin, int NW, int L, int U, int MODE>
 static int launch_mlpg(const nnk_mlpg_args_t& a, const nnk_mlpg_gv_t* gv, cudaStream_t st,
-                       const nnk_traj_ll_t* tl = nullptr, const nnk_traj_sample_t* ts = nullptr) {
+                       const nnk_traj_ll_t* tl = nullptr, const nnk_traj_sample_t* ts = nullptr,
+                       const nnk_mlpg_vjp_t* vj = nullptr) {
   constexpr int NT = L + U + 1;
   constexpr int NTS = WsCols<MODE, NT>::value;
   constexpr int PF = (L + U <= 2) ? 4 : 2;
@@ -779,6 +867,10 @@ static int launch_mlpg(const nnk_mlpg_args_t& a, const nnk_mlpg_gv_t* gv, cudaSt
   p.ws = (double*)a.workspace; p.status = (unsigned long long*)a.status_word;
   p.gv_mean = gv ? gv->gv_mean : nullptr; p.gv_var = gv ? gv->gv_var : nullptr;
   p.gv_step = gv ? gv->step : 0.0; p.gv_weight = gv ? gv->weight : 0.0; p.gv_n_iter = gv ? gv->n_iter : 0;
+  if constexpr (MODE == MODE_VJP) {  // grad_out is of Tin and read at the output's rows and columns
+    p.go = vj->grad_out; p.go_ld = vj->go_ld; p.go_f64 = 0;
+    p.grad_means = (Tin*)vj->grad_means; p.gm_ld = vj->gm_ld; p.grad_vars = vj->grad_vars; p.gv_ld = vj->gv_ld;
+  }
   const size_t per_item = (size_t)a.max_T * NTS * 32 * sizeof(double);
   size_t items_cap = per_item ? a.workspace_bytes / per_item : 0;
   int utt_per_launch = (int)(items_cap / (size_t)p.n_groups);
@@ -829,17 +921,18 @@ static int launch_mlpg(const nnk_mlpg_args_t& a, const nnk_mlpg_gv_t* gv, cudaSt
 
 template <typename Tin, int MODE>
 static int dispatch_inst(const nnk_mlpg_args_t& a, cudaStream_t st, const nnk_mlpg_gv_t* gv = nullptr,
-                         const nnk_traj_ll_t* tl = nullptr, const nnk_traj_sample_t* ts = nullptr) {
+                         const nnk_traj_ll_t* tl = nullptr, const nnk_traj_sample_t* ts = nullptr,
+                         const nnk_mlpg_vjp_t* vj = nullptr) {
   int inst = -1;
   if (pick_instance(a.win, inst) < 0) {
     set_error("unsupported window set: nw=%d (max %d) or half-width > %d", a.win.nw, NNK_MAX_WIN, NNK_MAX_HALF);
     return NNK_ERR_UNSUPPORTED;
   }
   switch (inst) {
-    case 0: return launch_mlpg<Tin, 1, 0, 0, MODE>(a, gv, st, tl, ts);
-    case 1: return launch_mlpg<Tin, 3, 1, 1, MODE>(a, gv, st, tl, ts);
-    case 2: return launch_mlpg<Tin, 3, 2, 2, MODE>(a, gv, st, tl, ts);
-    default: return launch_mlpg<Tin, NNK_MAX_WIN, NNK_MAX_HALF, NNK_MAX_HALF, MODE>(a, gv, st, tl, ts);
+    case 0: return launch_mlpg<Tin, 1, 0, 0, MODE>(a, gv, st, tl, ts, vj);
+    case 1: return launch_mlpg<Tin, 3, 1, 1, MODE>(a, gv, st, tl, ts, vj);
+    case 2: return launch_mlpg<Tin, 3, 2, 2, MODE>(a, gv, st, tl, ts, vj);
+    default: return launch_mlpg<Tin, NNK_MAX_WIN, NNK_MAX_HALF, NNK_MAX_HALF, MODE>(a, gv, st, tl, ts, vj);
   }
 }
 
@@ -884,6 +977,10 @@ extern "C" size_t nnk_mlpg_traj_ll_workspace_bytes(int32_t n_utt, int32_t n_chai
 extern "C" size_t nnk_mlpg_traj_sample_workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T,
                                                        const nnk_windows_t* win) {
   return workspace_bytes(n_utt, n_chain, max_T, win, WsCols<MODE_SAMPLE, 0>::value);
+}
+
+extern "C" size_t nnk_mlpg_vjp_workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T, const nnk_windows_t* win) {
+  return workspace_bytes(n_utt, n_chain, max_T, win, WsCols<MODE_VJP, 0>::value);
 }
 
 #ifdef NNK_AS_PROF
@@ -970,4 +1067,20 @@ extern "C" int nnk_mlpg_traj_sample(const nnk_mlpg_args_t* a, const nnk_traj_sam
   cudaStream_t st = (cudaStream_t)stream;
   return a->dtype == NNK_F32 ? dispatch_inst<float, MODE_SAMPLE>(*a, st, nullptr, nullptr, ts)
                              : dispatch_inst<double, MODE_SAMPLE>(*a, st, nullptr, nullptr, ts);
+}
+
+extern "C" int nnk_mlpg_vjp(const nnk_mlpg_args_t* a, const nnk_mlpg_vjp_t* vj, void* stream) {
+  NNK_REQUIRE(a != nullptr && vj != nullptr, NNK_ERR_ARG, "args or vj is NULL");
+  NNK_REQUIRE(a->dtype == NNK_F32 || a->dtype == NNK_F64, NNK_ERR_ARG, "dtype must be NNK_F32 or NNK_F64");
+  NNK_REQUIRE(a->n_utt >= 0 && a->n_chain >= 0 && a->max_T >= 0, NNK_ERR_ARG, "negative size");
+  NNK_REQUIRE(a->n_chain < (1 << 21) && a->max_T < (1 << 21) - 1 && a->n_utt < (1 << 22), NNK_ERR_ARG, "size exceeds status key range");
+  NNK_REQUIRE(vj->go_ld >= 0 && vj->gm_ld >= 0 && vj->gv_ld >= 0, NNK_ERR_ARG, "negative row stride");
+  if (a->n_utt == 0 || a->n_chain == 0 || a->max_T == 0) return NNK_OK;
+  NNK_REQUIRE(a->means && a->vars && a->utt_off && a->chains && a->status_word, NNK_ERR_ARG, "NULL device pointer");
+  NNK_REQUIRE(vj->grad_out && vj->grad_means && vj->grad_vars, NNK_ERR_ARG, "NULL grad_out or gradient output");
+  NNK_REQUIRE(a->workspace != nullptr, NNK_ERR_WORKSPACE, "NULL workspace");
+  DeviceGuard guard(vj->grad_means);
+  cudaStream_t st = (cudaStream_t)stream;
+  return a->dtype == NNK_F32 ? dispatch_inst<float, MODE_VJP>(*a, st, nullptr, nullptr, nullptr, vj)
+                             : dispatch_inst<double, MODE_VJP>(*a, st, nullptr, nullptr, nullptr, vj);
 }

@@ -7,15 +7,18 @@ namespace nnk {
 // MODE_GV: the forward solve followed by the global-variance refinement of nnk_mlpg_gv (mlpg_kernel only).
 // MODE_TLL / MODE_TLL_GRAD: the trajectory-model log-likelihood of nnk_mlpg_traj_ll, without / with its
 // gradients (mlpg_kernel only).  MODE_SAMPLE: samples of the trajectory model of nnk_mlpg_traj_sample (mlpg_kernel
-// only).
-enum { MODE_FWD = 0, MODE_GRAD = 1, MODE_SOLVE = 2, MODE_GV = 3, MODE_TLL = 4, MODE_TLL_GRAD = 5, MODE_SAMPLE = 6 };
+// only).  MODE_VJP: the gradients of the forward solve in its means and variances, nnk_mlpg_vjp (mlpg_kernel only).
+enum { MODE_FWD = 0, MODE_GRAD = 1, MODE_SOLVE = 2, MODE_GV = 3, MODE_TLL = 4, MODE_TLL_GRAD = 5, MODE_SAMPLE = 6,
+       MODE_VJP = 7 };
 
 // scratch columns per frame of one work item: the S + 1 factor columns, in MODE_GV four more (pivot d, c_m, and
-// the current / trial trajectory), in the MODE_TLL pair one more (1 / d), in MODE_SAMPLE one more (1 / sqrt(d))
+// the current / trial trajectory), in the MODE_TLL pair one more (1 / d), in MODE_SAMPLE one more (1 / sqrt(d)), in
+// MODE_VJP one more ((L^-1 o)_t / d_t)
 template <int MODE, int NT>
 struct WsCols {
   static constexpr int value =
-      NT + (MODE == MODE_GV ? 4 : (MODE == MODE_TLL || MODE == MODE_TLL_GRAD || MODE == MODE_SAMPLE) ? 1 : 0);
+      NT + (MODE == MODE_GV ? 4
+            : (MODE == MODE_TLL || MODE == MODE_TLL_GRAD || MODE == MODE_SAMPLE || MODE == MODE_VJP) ? 1 : 0);
 };
 
 template <int NW, int L, int U>
@@ -78,6 +81,15 @@ struct SampleParams : MlpgParams<Tin, NW, L, U> {
   double scale;
 };
 
+// MODE_VJP: MlpgParams (grad_out and go_ld in go / go_ld, of Tin) plus the outputs of nnk_mlpg_vjp_t
+template <typename Tin, int NW, int L, int U>
+struct VjpParams : MlpgParams<Tin, NW, L, U> {
+  Tin* grad_means;
+  int64_t gm_ld;
+  void* grad_vars;  // Tin rows of gv_ld, or (n_utt, gv_ld) float64 partials for global variances
+  int64_t gv_ld;
+};
+
 template <typename Tin, int NW, int L, int U, int MODE>
 struct KernelParams {
   using type = MlpgParams<Tin, NW, L, U>;
@@ -93,6 +105,10 @@ struct KernelParams<Tin, NW, L, U, MODE_TLL_GRAD> {
 template <typename Tin, int NW, int L, int U>
 struct KernelParams<Tin, NW, L, U, MODE_SAMPLE> {
   using type = SampleParams<Tin, NW, L, U>;
+};
+template <typename Tin, int NW, int L, int U>
+struct KernelParams<Tin, NW, L, U, MODE_VJP> {
+  using type = VjpParams<Tin, NW, L, U>;
 };
 
 }  // namespace nnk

@@ -37,6 +37,10 @@ Additive, the log-likelihood of target trajectories under the trajectory model o
 Additive, samples from that trajectory model with counter-based noise (DESIGN.md 3.21): :func:`trajectory_sample`,
 :func:`trajectory_sample_batch` (csrc/nnk_mlpg.cu ``nnk_mlpg_traj_sample``, C ABI include/nnk_traj_sample.h).  Not
 in ``__all__``.
+
+Additive, the gradient of :func:`mlpg_batch` in its means and its variances for minimum-generation-error training
+(DESIGN.md 3.22): :func:`mlpg_vjp_batch` (csrc/nnk_mlpg.cu ``nnk_mlpg_vjp``, C ABI include/nnk_mlpg_vjp.h).  Not in
+``__all__``.
 """
 import ctypes
 
@@ -1459,3 +1463,93 @@ def trajectory_sample(mean_frames, variance_frames, windows, n_samples=1, seed=0
     (or ``(D,)``); returns the ``(n_samples, T, static_dim)`` samples."""
     return trajectory_sample_batch(mean_frames, variance_frames, windows, n_samples=n_samples, seed=seed,
                                    scale=scale, lengths=[mean_frames.shape[0]])
+
+
+# ---------------------------------------------------------------------------------------------------
+# gradient of MLPG in means and variances (additive)
+# ---------------------------------------------------------------------------------------------------
+class _NnkMlpgVjp(ctypes.Structure):
+    """ctypes mirror of nnk_mlpg_vjp_t (include/nnk_mlpg_vjp.h)."""
+    _fields_ = [
+        ("grad_out", ctypes.c_void_p),
+        ("go_ld", ctypes.c_int64),
+        ("grad_means", ctypes.c_void_p),
+        ("gm_ld", ctypes.c_int64),
+        ("grad_vars", ctypes.c_void_p),
+        ("gv_ld", ctypes.c_int64),
+    ]
+
+
+def _mlpg_vjp_device(means, variances, windows, grad_output, table, layout, padded):
+    """One launch of ``nnk_mlpg_vjp`` per workspace wave on checked CUDA tensors, on the current stream, with one
+    host synchronisation (the status word).  Returns ``(grad_means, grad_variances)`` shaped like the inputs, in
+    their dtype; ``(D,)`` variances get the per-utterance float64 partials summed over the batch."""
+    import torch
+
+    from . import _device as dev
+    device = means.device
+    dev.poll_errors()
+    m, v, go = means.contiguous(), variances.contiguous(), grad_output.contiguous()
+    _, _, _, max_T, n_utt = table
+    D = m.shape[-1]
+    var1d = v.dim() == 1
+    g_m = torch.zeros_like(m)
+    g_v = torch.zeros((n_utt, D), dtype=torch.float64, device=device) if var1d else torch.zeros_like(v)
+    if n_utt and max_T and layout.n_chain:
+        a, keep, status = _traj_args(m, v, windows, table, layout, padded, _lib.lib.nnk_mlpg_vjp_workspace_bytes)
+        t = _NnkMlpgVjp()
+        t.grad_out, t.go_ld = go.data_ptr(), layout.D_out
+        t.grad_means, t.gm_ld = g_m.data_ptr(), D
+        t.grad_vars, t.gv_ld = g_v.data_ptr(), D
+        _lib.check(_lib.lib.nnk_mlpg_vjp(ctypes.byref(a), ctypes.byref(t), dev.current_stream_ptr(device)),
+                   "nnk_mlpg_vjp")
+        dev.raise_if_failed(status)
+    if var1d:
+        g_v = g_v.sum(dim=0).to(m.dtype)
+    return g_m, g_v
+
+
+def mlpg_vjp_batch(means, variances, windows, grad_output, lengths=None, offsets=None, layout=None):
+    r"""Gradient of :func:`mlpg_batch` in its means and its variances (additive API), for minimum generation error
+    training through MLPG (Wu & Wang 2006; Wu & King 2015).
+
+    Per utterance and smoothed output column, with ``P``, ``b`` and :math:`\bar c = P^{-1} b` exactly as
+    :func:`mlpg_batch` builds them (its edge rule included), :math:`o = \partial L / \partial \bar c` the
+    matching column of ``grad_output`` and :math:`g = P^{-1} o`:
+
+    .. math::
+        \partial L / \partial \mu_{t,w} = \tau_{t,w} (W_w g)_t, \qquad
+        \partial L / \partial \sigma^2_{t,w} = -\tau_{t,w}^2 (W_w g)_t (\mu_{t,w} - (W_w \bar c)_t),
+
+    with :math:`\tau = 1 / \sigma^2`.  Both are 0 where the edge rule sets the precision to zero.  Copied columns
+    pass the gradient through to their mean and get a zero variance gradient.  The mean gradient is what
+    :func:`mlpg_grad_batch` returns, here in the input dtype.  See DESIGN.md 3.22.
+
+    Args:
+        means, variances, windows, lengths, offsets, layout: as :func:`mlpg_batch` (flat or padded, per-frame or
+            global ``(D,)`` variances).
+        grad_output: the gradient with respect to :func:`mlpg_batch`'s result, of its shape.  All three arrays are
+            NumPy arrays or all CUDA tensors, of one dtype (float32 or float64).
+
+    Returns:
+        ``(grad_means, grad_variances)`` shaped like ``means`` and ``variances``, in their dtype: NumPy for NumPy
+        input, CUDA tensors for tensors (computed on the current stream, one kernel launch).  Padded rows get zero.
+        For ``(D,)`` variances the per-frame gradients are summed over every frame of the batch.  Arithmetic is
+        float64.  A variance that makes a pivot of ``P`` non-positive raises ``numpy.linalg.LinAlgError`` as
+        :func:`mlpg_batch` does.
+    """
+    import torch
+
+    from . import _device as dev
+    layout, padded, on_device = _traj_ll_check(grad_output, means, variances, windows, lengths, offsets, layout)
+    if not on_device:
+        means, variances, grad_output = (np.asarray(a) for a in (means, variances, grad_output))
+    n_rows = means.shape[0] * means.shape[1] if padded else means.shape[0]
+    table = _utterance_table(lengths, offsets, n_rows, tuple(means.shape[:2]) if padded else None)
+    dev.require_cuda()
+    if not on_device:
+        device = dev.cuda_device()
+        means, variances, grad_output = (torch.from_numpy(np.ascontiguousarray(a)).to(device)
+                                         for a in (means, variances, grad_output))
+    g_m, g_v = _mlpg_vjp_device(means, variances, windows, grad_output, table, layout, padded)
+    return (g_m, g_v) if on_device else (g_m.cpu().numpy(), g_v.cpu().numpy())
