@@ -553,6 +553,289 @@ int nnk_modspec(int32_t mode, int32_t dtype, int32_t n, const void* in, const vo
                 int32_t B, int32_t T_in, int32_t T_out, int32_t D, const int32_t* lengths, double fwd_scale,
                 double inv_scale, int32_t limit_bin, int32_t log_domain, void* stream);
 
+/* ---- parameter generation considering the modulation spectrum (paramgen.mlpg_ms_batch; csrc/nnk_ms_gen.cu;
+ * DESIGN.md 3.18) -----------------------------------------------------------------------------------------------
+ * nnk_mlpg_ms: per chain c (one smoothed output column s = c.out_col of one utterance of T <= n frames) and with
+ * tau, P, b and c_m = P^-1 b exactly as nnk_mlpg_fwd builds them (edge rule included), Y = rfft(c, n) and
+ * s_k(c) = log(max(|Y_k|^2, DBL_MIN)), maximises
+ *   F(c) = omega (b^T c - c^T P c / 2) - 1/2 sum_{k=1}^{n/2} q_k (s_k(c) - nu_k)^2,
+ *   nu_k = ms_mean[k * args->out_ld + s],  q_k = 1 / ms_var[k * args->out_ld + s]  (q_k = 0 when ms_var is inf)
+ * from c0 = c_m by n_iter trials: g = grad of the MS term at c, h = P^-1 g, delta = (c_m - c) + h / omega,
+ * c' = c + alpha delta is kept when F(c') >= F(c), otherwise alpha halves (alpha starts at `step`; a rejected
+ * trial still counts).  Bin 0 has no term; a bin of power <= DBL_MIN adds a constant and no gradient.
+ * omega = weight, or 1 / (nw T) when weight == 0.  Pass-through chains are copied.
+ *
+ * Everything is float64: args->dtype must be NNK_F64 (callers widen float32 inputs once) and args->out_off
+ * NULL.  Every utterance must have T <= n frames (args->max_T <= n); longer ones are left unwritten.  One call
+ * enqueues, on `stream` and without a host synchronisation, 2 + 2 n_iter launches: nnk_mlpg_fwd into the
+ * workspace, one launch that copies c_m to out and forms the first gradient, then per trial one nnk_mlpg_solve
+ * (float64 right-hand side) and one launch of ms_gen_kernel (csrc/nnk_ms_gen.cu).  Non-positive pivots set the
+ * status word as for nnk_mlpg_fwd.  The workspace must hold nnk_mlpg_ms_workspace_bytes(): the MLPG factor
+ * scratch of the whole batch, c_m and h ((n_rows, out_ld) each), g ((n_rows, n_chain)) and two numbers per
+ * chain (F and alpha).  Per-chain sums run in a fixed order inside one CTA, so a chain's result does not depend
+ * on the batch around it and repeated calls give the same bits. */
+typedef struct nnk_mlpg_ms {
+  const double* ms_mean; /* device (n / 2 + 1, args->out_ld): nu, finite where ms_var is finite          */
+  const double* ms_var;  /* device (n / 2 + 1, args->out_ld): > 0, inf exempts the bin                    */
+  int32_t n;             /* DFT length: 256, 512, 1024, 2048 or 4096                                      */
+  int32_t n_iter;        /* >= 0 trials                                                                   */
+  double step;           /* > 0 initial step alpha                                                        */
+  double weight;         /* omega > 0, or 0 => 1 / (nw T) per utterance                                   */
+  int64_t n_rows;        /* rows of means / vars / out (utt_off[n_utt] at most); sizes the workspace      */
+} nnk_mlpg_ms_t;
+
+int nnk_mlpg_ms(const nnk_mlpg_args_t* args, const nnk_mlpg_ms_t* ms, void* stream);
+size_t nnk_mlpg_ms_workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T, int64_t n_rows, int64_t out_ld,
+                                   const nnk_windows_t* win);
+
+/* ---- segment-level modulation spectrum (postfilters.modspec_*(segment=L), paramgen.mlpg_ms_batch(segment=L);
+ * csrc/nnk_ms_segment.cu, csrc/nnk_ms_gen.cu; DESIGN.md 3.16, 3.18) --------------------------------------------
+ * nnk_ms_segment: the segment-level MS of Takamichi et al. (ICASSP 2014) over a padded batch x (B, T, D),
+ * row-major, in dtype (NNK_F32 / NNK_F64).  Utterance b has len_b = min(max(lengths[b], 0), T) frames
+ * (lengths NULL: T); later frames are never read.  With the hop H = L / 2 and the periodic Hann window
+ * w_m = 0.5 - 0.5 cos(2 pi m / L), utterance b has J_b = ceil(len_b / H) + 1 segments (0 when len_b = 0);
+ * segment j starts at frame (j - 1) H, frames outside [0, len_b) are 0, and Y_j = rfft(w * x[seg j], n),
+ * K = n / 2 + 1 bins, s_jk = log(max(|Y_jk|^2, tiny)).
+ *   mode 0 (log power):   out (S, D, K) in dtype, S = sum_b J_b: row seg_off[b] + j, column d, bin k holds
+ *                         s_jk of column d.  seg_off (B,) int64 on the device, the exclusive prefix sums of J_b
+ *                         computed from the same lengths; table is unused (may be NULL).
+ *   mode 1 (post-filter): table (K, D, 2) in dtype holds (a, c); every bin k >= 1 of non-zero power becomes
+ *                         C_jk = Y_jk / |Y_jk| exp((a s_jk + c) / 2), bin 0 and zero-power bins as for
+ *                         nnk_modspec's post-filter; out (B, T, D) = sum_j irfft(C_j, n)[t - (j - 1) H] over
+ *                         the segments with 0 <= t - (j - 1) H < L for t < len_b, 0 for len_b <= t < T.
+ *                         seg_off is unused (may be NULL).
+ * n is 32, 64, 128, 256 or 512 and L even with 4 <= L <= n (else NNK_ERR_ARG).  Every output element is
+ * written exactly once, without atomics: repeated calls give the same bits.
+ *
+ * nnk_mlpg_ms_segment: parameter generation considering the segment-level MS (paramgen.mlpg_ms_batch(segment=L),
+ * DESIGN.md 3.18).  args, ms, tau, P, b, c_m = P^-1 b, omega, the start point c0 = c_m and the trials are exactly
+ * those of nnk_mlpg_ms; only the MS term differs.  Per chain (one smoothed output column s = c.out_col of one
+ * utterance of T >= 1 frames, any T), with the segments of nnk_ms_segment (H = L / 2, J = ceil(T / H) + 1,
+ * segment j starts at frame (j - 1) H, frames outside [0, T) are 0, periodic Hann window w),
+ * Y_j = rfft(w * c[seg j], n) and s_jk = log(max(|Y_jk|^2, DBL_MIN)), it maximises
+ *   F(c) = omega (b^T c - c^T P c / 2) - 1/(2 J) sum_j sum_{k=1}^{n/2} q_k (s_jk - nu_k)^2
+ * (nu_k, q_k from ms->ms_mean / ms->ms_var as for nnk_mlpg_ms): the mean of the utterance level's term over the J
+ * segments, edge segments included.  Bin 0 has no term; a bin of power <= DBL_MIN adds a constant and no
+ * gradient; ms_var = inf exempts a bin.  The gradient at frame t = (j - 1) H + m (0 <= m < L) is
+ *   g_t = 1/J sum_{j containing t} w_m [n irfft(C_j, n)]_m,  C_jk = -q_k (s_jk - nu_k) / |Y_jk|^2 Y_jk
+ * (C_j,n/2 doubled, C_j0 = 0): every frame lies in two segments, so g_t is one addition of two terms.
+ * ms->n is 32, 64, 128, 256 or 512 and L even with 4 <= L <= n; there is no limit on args->max_T.  NNK_ERR_ARG:
+ * args or ms NULL, dtype not NNK_F64, out_off not NULL, a negative size, a bad n or L, n_iter < 0, step <= 0,
+ * weight < 0 or NaN, a NULL device pointer or NULL ms_mean / ms_var.  The workspace is
+ * nnk_mlpg_ms_workspace_bytes() of the same arguments.  One call enqueues 2 + 2 n_iter launches on `stream`
+ * without a host synchronisation, whatever the batch and T: nnk_mlpg_fwd, one launch that copies c_m to out and
+ * forms the first gradient, then per trial one nnk_mlpg_solve and one launch of ms_gen_segment_kernel
+ * (csrc/nnk_ms_gen.cu).  Non-positive pivots set the status word as for nnk_mlpg_ms.  Sums run in a fixed order
+ * inside one CTA per chain, so a chain's bits do not depend on the batch and repeated calls give the same bits. */
+#define NNK_MSSEG_LOGPOWER 0
+#define NNK_MSSEG_POSTFILTER 1
+int nnk_ms_segment(int32_t mode, int32_t dtype, int32_t n, int32_t L, const void* x, const void* table, void* out,
+                   int32_t B, int32_t T, int32_t D, const int32_t* lengths, const int64_t* seg_off, void* stream);
+int nnk_mlpg_ms_segment(const nnk_mlpg_args_t* args, const nnk_mlpg_ms_t* ms, int32_t L, void* stream);
+
+/* ---- parameter generation from mixture outputs (paramgen.mlpg_mixture_batch; csrc/nnk_mix_gen.cu;
+ * DESIGN.md 3.19) -----------------------------------------------------------------------------------------------
+ * nnk_mix_gen: one launch of mix_gen_kernel, the E-step side of the EM of paramgen.mlpg_mixture_batch (Tokuda et
+ * al., ICASSP 2000).  Frame r (a row of the batch) has M components: log-weights lw[r, m] (log_weights,
+ * (n_rows, M)), means mu[r, m, i] and variances s2[r, m, i] (means / vars, (n_rows, M, D)), all of `dtype` and
+ * row-major; float32 inputs are widened in registers and every operation is float64.  Utterance u has rows
+ * utt_off[u] .. utt_off[u] + utt_len[u] - 1 and the tiles tile_off[u] .. tile_off[u + 1] - 1 of
+ * NNK_MIX_GEN_TILE frames (n_tiles = tile_off[n_utt]); rows outside every utterance are never read or written.
+ * col_map[i] describes input column i:
+ *   -1                        the column takes no part (no chain reads it);
+ *   (out_col << 3) | 0        a copied column: Y_t[i] = c[t, out_col];
+ *   (out_col << 3) | (w + 1)  window w of a smoothed column: Y_t[i] = sum_j coef_w[j] c[t + j, out_col], with
+ *                             c = 0 outside the utterance.
+ * On the first and last H = max_w max(l_w, u_w) frames of an utterance, and on every frame when H = 0, only the
+ * copied columns and those of window 0 count; elsewhere every column with col_map >= 0 counts.
+ *   NNK_MIX_GEN_SELECT:    per frame the component a with the largest lw (the lowest index on ties) goes to
+ *                          E[r, :] = mu[r, a, :], V[r, :] = s2[r, a, :]; every component's log-normaliser
+ *                          lnorm[r, m] = lw[r, m] - 1/2 sum_{counted i} (log s2[r, m, i] + log 2 pi) goes to
+ *                          lnorm.  Data errors set *status_word (below).
+ *   NNK_MIX_GEN_ESTEP:     with l[r, m] = lnorm[r, m] - 1/2 sum_{counted i} (Y_r[i] - mu[r, m, i])^2 / s2[r, m, i]
+ *                          and gamma its softmax over m: P = sum_m gamma / s2, E[r, i] = (sum_m gamma mu / s2) / P
+ *                          and V[r, i] = 1 / P for every column with col_map >= 0 (0 and 1 for the others).
+ *                          With ll_part, ll_part[tile] = sum over the tile's frames, in frame order, of
+ *                          log sum_m exp(l[r, m]).
+ *   NNK_MIX_GEN_OBJECTIVE: ll_part only (required).
+ * c (rows of c_ld doubles, the first c_cols staged per tile) is read by ESTEP and OBJECTIVE only.
+ * Status word (device, zeroed by the caller): 0, or ~((row << 2) | kind) of the first failing row, lowest kind
+ * first: kind 1 = a NaN or +inf log-weight, 2 = every log-weight -inf, 3 = a variance of a column with
+ * col_map >= 0 that is not positive and finite.  Results of a failing call are undefined but never fault.
+ * Errors: NNK_ERR_ARG for NULL pointers, bad sizes, a bad mode, dtype or window set; NNK_ERR_UNSUPPORTED for
+ * D > NNK_MIX_GEN_MAX_D or M > NNK_MIX_GEN_MAX_M; all before anything touches the device.  Every output element
+ * is written by one thread in a fixed order: repeated calls give the same bits. */
+#define NNK_MIX_GEN_SELECT 0
+#define NNK_MIX_GEN_ESTEP 1
+#define NNK_MIX_GEN_OBJECTIVE 2
+#define NNK_MIX_GEN_TILE 32    /* frames per tile */
+#define NNK_MIX_GEN_MAX_D 256  /* input columns   */
+#define NNK_MIX_GEN_MAX_M 64   /* components      */
+
+typedef struct nnk_mix_gen_args {
+  const void* log_weights; /* device (n_rows, M) of dtype                                                   */
+  const void* means;       /* device (n_rows, M, D) of dtype                                                */
+  const void* vars;        /* device (n_rows, M, D) of dtype                                                */
+  int32_t dtype;           /* NNK_F32 / NNK_F64                                                             */
+  int32_t M;               /* components, 1 .. NNK_MIX_GEN_MAX_M                                            */
+  int32_t D;               /* input columns, 1 .. NNK_MIX_GEN_MAX_D                                         */
+  int32_t n_utt;           /* >= 1                                                                          */
+  const int32_t* utt_off;  /* device (n_utt): first row of each utterance                                   */
+  const int32_t* utt_len;  /* device (n_utt): frames of each utterance                                      */
+  const int32_t* tile_off; /* device (n_utt + 1): first tile of each utterance                              */
+  int32_t n_tiles;         /* tile_off[n_utt]                                                               */
+  const int32_t* col_map;  /* device (D)                                                                    */
+  nnk_windows_t win;
+  int32_t mode;            /* NNK_MIX_GEN_SELECT / _ESTEP / _OBJECTIVE                                      */
+  const double* c;         /* device, ESTEP / OBJECTIVE: current trajectories, row r at c + r * c_ld        */
+  int64_t c_ld;
+  int32_t c_cols;          /* columns of c the column map addresses (out_col < c_cols <= c_ld)             */
+  double* lnorm;           /* device (n_rows, M): written by SELECT, read by ESTEP / OBJECTIVE              */
+  double* E;               /* device (n_rows, D): written by SELECT / ESTEP                                 */
+  double* V;               /* device (n_rows, D): written by SELECT / ESTEP                                 */
+  double* ll_part;         /* device (n_tiles) or NULL (ESTEP); required for OBJECTIVE                      */
+  uint64_t* status_word;   /* device, SELECT                                                                */
+} nnk_mix_gen_args_t;
+
+int nnk_mix_gen(const nnk_mix_gen_args_t* args, void* stream);
+
+/* ---- trajectory-model log-likelihood (paramgen.trajectory_log_likelihood_batch; csrc/nnk_mlpg.cu;
+ * DESIGN.md 3.20) -----------------------------------------------------------------------------------------------
+ * nnk_mlpg_traj_ll: one launch of mlpg_kernel in MODE_TLL / MODE_TLL_GRAD per workspace wave.  Per chain c of
+ * utterance u (a static column, exactly as nnk_mlpg_fwd sees it: T frames, tau_{t,w} = 1 / var with the edge rule
+ * of nnk_mlpg_fwd, mu_{t,w}, P = sum_w W_w^T diag(tau_w) W_w, b = sum_w W_w^T (tau_w mu_w), cbar = P^-1 b,
+ * P = L D L^T with pivots d_t) and its target static trajectory x (x_t at targets[(out_off or utt_off)[u] + t) *
+ * tgt_ld + chains[c].out_col]), the Gaussian trajectory model N(x; cbar, P^-1) (Zen, Tokuda & Kitamura 2007) has
+ * the log-likelihood
+ *
+ *   l = 1/2 sum_t log d_t - 1/2 sum_{t,w} tau_{t,w} (u_{t,w} - ubar_{t,w})^2 - (T/2) log 2 pi,
+ *   u_{t,w} = (W_w x)_t,  ubar_{t,w} = (W_w cbar)_t,
+ *
+ * written to ll[u * n_chain + c] (0 for copied chains, flags & 1).  With grad != 0 the gradients are written too,
+ * with w_t row t of W_w and Sigma = P^-1:
+ *
+ *   dl/dmu_{t,w}   = tau_{t,w} (u_{t,w} - ubar_{t,w})                                         -> grad_means
+ *   dl/dvar_{t,w}  = -tau_{t,w}^2 / 2 [w_t^T Sigma w_t - (u_{t,w} - mu_{t,w})^2 + (ubar_{t,w} - mu_{t,w})^2]
+ *   dl/dx          = -P (x - cbar) = -sum_w W_w^T (dl/dmu_{.,w})                               -> grad_targets
+ *
+ * grad_means has the rows of means (utt_off[u] + t) and columns chains[c].in_col + w * win_stride with row stride
+ * gm_ld; grad_targets has the rows and columns of the targets with row stride gx_ld; both are of `dtype`.  Per-frame
+ * variances (var_ld > 0): grad_vars has the layout of grad_means with row stride gv_ld, of `dtype`.  Global (D,)
+ * variances (var_ld == 0): grad_vars is a float64 (n_utt, gv_ld) array and grad_vars[u * gv_ld + column] is the
+ * sum of the per-frame values over the utterance's frames.  Only the elements of solved chains at frames
+ * 0 .. T - 1 are written: the caller zeroes the others.  Where the edge rule sets tau to zero, both gradients are 0.
+ * Every sum runs in a fixed order in one thread, so a chain's results do not depend on the batch and repeated calls
+ * give the same bits.  Arithmetic is float64; float32 inputs are widened exactly as nnk_mlpg_fwd widens them.
+ * Targets and means are not checked: non-finite values give NaN.  A pivot d_t <= 0 sets the status word as
+ * nnk_mlpg_fwd does.  Errors: NNK_ERR_ARG for NULL pointers or bad sizes, NNK_ERR_UNSUPPORTED for a window set no
+ * instance serves, NNK_ERR_WORKSPACE for a workspace below one utterance's share of
+ * nnk_mlpg_traj_ll_workspace_bytes; all before anything is launched.  args->out, grad_out, go_ld and go_f64 are
+ * not used. */
+typedef struct nnk_traj_ll {
+  const void* targets; /* device, dtype: target static trajectories (rows and columns of the nnk_mlpg_fwd output) */
+  int64_t tgt_ld;      /* row stride of targets, in elements                                                      */
+  double* ll;          /* device (n_utt, n_chain) float64                                                         */
+  int32_t grad;        /* 0: ll only; 1: ll and the three gradients                                               */
+  void* grad_means;    /* device, dtype, rows and columns of means                                                */
+  int64_t gm_ld;
+  void* grad_vars;     /* device: per-frame, dtype, rows and columns of vars; global, float64 (n_utt, gv_ld)      */
+  int64_t gv_ld;
+  void* grad_targets;  /* device, dtype, rows and columns of targets                                              */
+  int64_t gx_ld;
+} nnk_traj_ll_t;
+
+int nnk_mlpg_traj_ll(const nnk_mlpg_args_t* args, const nnk_traj_ll_t* tl, void* stream);
+size_t nnk_mlpg_traj_ll_workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T, const nnk_windows_t* win);
+
+/* ---- sampling from the trajectory model (paramgen.trajectory_sample_batch; csrc/nnk_mlpg.cu; DESIGN.md 3.21) ---
+ * nnk_mlpg_traj_sample: one launch of mlpg_kernel in MODE_SAMPLE per workspace wave.  Per chain c of utterance u
+ * (a static column, exactly as nnk_mlpg_fwd sees it: T frames, tau_{t,w} = 1 / var with the edge rule of
+ * nnk_mlpg_fwd, P = sum_w W_w^T diag(tau_w) W_w, b = sum_w W_w^T (tau_w mu_w), and the top-down factorisation
+ * P = L D L^T with unit lower L, pivots d_t, multipliers l_j[t] = L[t+j][t] and zs_t = (L^-1 b)_t / d_t),
+ * sample s = 0 .. n_samples - 1 is
+ *
+ *   y_t = zs_t + scale * z_{s,t} / sqrt(d_t) - sum_{j=1..S} l_j[t] y_{t+j}      (t = T-1 .. 0, y_t = 0 for t >= T)
+ *
+ * that is y = L^-T (D^-1 L^-1 b + scale D^-1/2 z) ~ N(cbar, scale^2 P^-1), cbar = P^-1 b, for z ~ N(0, I).  It is
+ * written in the dtype of the inputs to args->out + s * sample_stride at row (out_off or utt_off)[u] + t, column
+ * chains[c].out_col, row stride out_ld.  With scale = 0 the recurrence is nnk_mlpg_fwd's backward sweep term for
+ * term.  Copied chains (flags & 1) get the means column, unchanged and without noise, in every sample.  Elements
+ * no chain writes are not touched.  Arithmetic is float64; float32 inputs are widened exactly as nnk_mlpg_fwd
+ * widens them.
+ *
+ * The noise z_{s,t} of chain c of utterance u is a pure function of (seed, key_u, s, t, out_col = chains[c].out_col):
+ * it does not depend on the batch around the utterance, the layout, the padding, the dtype, n_samples or the
+ * workspace waves.  Normative definition:
+ *
+ *   Philox4x32-10 (Salmon, Moraes, Dror & Shaw, SC 2011) with multipliers M0 = 0xD2511F53, M1 = 0xCD9E8D57 and key
+ *   increments W0 = 0x9E3779B9, W1 = 0xBB67AE85.  A round maps the counter (c0, c1, c2, c3) to
+ *     (hi(M1 * c2) ^ c1 ^ k0, lo(M1 * c2), hi(M0 * c0) ^ c3 ^ k1, lo(M0 * c0))
+ *   (hi / lo: upper / lower 32 bits of the 64-bit product); after each of the first nine rounds the key becomes
+ *   (k0 + W0, k1 + W1) mod 2^32.  Ten rounds give the output words (r0, r1, r2, r3).
+ *     key      (k0, k1)         = (seed mod 2^32, seed >> 32)
+ *     counter  (c0, c1, c2, c3) = (t >> 1, out_col, s, key_u),   key_u = keys ? keys[u] : u
+ *   u is the caller's utterance index (the index into utt_off), never a position in args->order.
+ *     N_U = (r0 >> 6) * 2^26 + (r1 >> 6),   U = (N_U + 0.5) * 2^-52   in (0, 1)
+ *     N_V = (r2 >> 6) * 2^26 + (r3 >> 6),   V = N_V * 2^-52           in [0, 1)
+ *     R = sqrt(-2 log U),   z_{s,t} = R cos(2 pi V) for even t,  R sin(2 pi V) for odd t   (Box & Muller 1958)
+ *   so one Philox call serves frames 2k and 2k + 1 of one chain and sample.  Known answers of the rounds
+ *   (Random123's philox4x32-10 vectors): counter 0, key 0 -> 6627e8d5 e169c58d bc57ac4c 9b00dbd8; all ones ->
+ *   408f276d 41c83b0e a20bc7c6 6d5451fd; counter 243f6a88 85a308d3 13198a2e 03707344, key a4093822 299f31d0 ->
+ *   d16cfe09 94fdcceb 5001e420 24126ea1.
+ *
+ * A pivot d_t <= 0 sets the status word as nnk_mlpg_fwd does.  Errors: NNK_ERR_ARG for NULL pointers, bad sizes,
+ * n_samples < 1, sample_stride < 0 or a scale that is negative or not finite; NNK_ERR_UNSUPPORTED for a window set
+ * no instance serves; NNK_ERR_WORKSPACE for a workspace below one utterance's share of
+ * nnk_mlpg_traj_sample_workspace_bytes; all before anything is launched.  args->grad_out, go_ld and go_f64 are
+ * not used. */
+typedef struct nnk_traj_sample {
+  int64_t sample_stride; /* elements between samples in args->out                                        */
+  int32_t n_samples;     /* >= 1                                                                           */
+  uint64_t seed;
+  const uint32_t* keys;  /* device (n_utt,), or NULL for key_u = u                                         */
+  double scale;          /* >= 0, finite                                                                   */
+} nnk_traj_sample_t;
+
+int nnk_mlpg_traj_sample(const nnk_mlpg_args_t* args, const nnk_traj_sample_t* ts, void* stream);
+size_t nnk_mlpg_traj_sample_workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T, const nnk_windows_t* win);
+
+/* ---- the gradient of MLPG in its means and variances (paramgen.mlpg_vjp_batch; csrc/nnk_mlpg.cu;
+ * DESIGN.md 3.22) -----------------------------------------------------------------------------------------------
+ * nnk_mlpg_vjp: one launch of mlpg_kernel in MODE_VJP per workspace wave.  Per chain c of utterance u (a static
+ * column, exactly as nnk_mlpg_fwd sees it: T frames, tau_{t,w} = 1 / var with the edge rule of nnk_mlpg_fwd,
+ * mu_{t,w}, P = sum_w W_w^T diag(tau_w) W_w, b = sum_w W_w^T (tau_w mu_w), cbar = P^-1 b, the trajectory
+ * nnk_mlpg_fwd writes) and the gradient o = dL/dcbar of a loss L with respect to that trajectory (o_t at
+ * grad_out[((out_off or utt_off)[u] + t) * go_ld + chains[c].out_col], of `dtype`), with g = P^-1 o:
+ *
+ *   dL/dmu_{t,w}  = tau_{t,w} (W_w g)_t                                                      -> grad_means
+ *   dL/dvar_{t,w} = -tau_{t,w}^2 (W_w g)_t (mu_{t,w} - (W_w cbar)_t)                          -> grad_vars
+ *
+ * (Wu & Wang 2006: minimum generation error training through MLPG in both).  Where the edge rule sets tau to zero,
+ * both gradients are 0.  Copied chains (flags & 1) pass o through: dL/dmu = o, and their dL/dvar is not written.
+ * grad_means has the rows of means (utt_off[u] + t) and columns chains[c].in_col + w * win_stride with row stride
+ * gm_ld, of `dtype`.  Per-frame variances (var_ld > 0): grad_vars has the layout of grad_means with row stride
+ * gv_ld, of `dtype`.  Global (D,) variances (var_ld == 0): grad_vars is a float64 (n_utt, gv_ld) array and
+ * grad_vars[u * gv_ld + column] is the sum of the per-frame values over the utterance's frames.  Only the elements
+ * of chains at frames 0 .. T - 1 are written: the caller zeroes the others.  Every sum runs in a fixed order in one
+ * thread, so a chain's results do not depend on the batch and repeated calls give the same bits.  Arithmetic is
+ * float64; float32 inputs are widened exactly as nnk_mlpg_fwd widens them, and the results are stored in `dtype`.
+ * Means and grad_out are not checked: non-finite values give NaN.  A pivot d_t <= 0 sets the status word as
+ * nnk_mlpg_fwd does.  Errors: NNK_ERR_ARG for NULL pointers or bad sizes, NNK_ERR_UNSUPPORTED for a window set no
+ * instance serves, NNK_ERR_WORKSPACE for a workspace below one utterance's share of nnk_mlpg_vjp_workspace_bytes;
+ * all before anything is launched.  args->out, args->grad_out, args->go_ld, args->out_ld and args->go_f64 are not
+ * used. */
+typedef struct nnk_mlpg_vjp {
+  const void* grad_out; /* device, dtype: dL/dcbar (rows and columns of the nnk_mlpg_fwd output)                  */
+  int64_t go_ld;        /* row stride of grad_out, in elements                                                     */
+  void* grad_means;     /* device, dtype, rows and columns of means                                                */
+  int64_t gm_ld;
+  void* grad_vars;      /* device: per-frame, dtype, rows and columns of vars; global, float64 (n_utt, gv_ld)      */
+  int64_t gv_ld;
+} nnk_mlpg_vjp_t;
+
+int nnk_mlpg_vjp(const nnk_mlpg_args_t* args, const nnk_mlpg_vjp_t* vj, void* stream);
+size_t nnk_mlpg_vjp_workspace_bytes(int32_t n_utt, int32_t n_chain, int32_t max_T, const nnk_windows_t* win);
+
 /* ---- sharded batches (SURVEY.md 8e; the reference has no multi-device path) ------------------------
  * Copies n_seg row segments (whole utterances) between two row-major device matrices:
  * dst[dst_row[s] + r, 0:cols] = src[src_row[s] + r, 0:cols] for r < len[s].  Used to bring the

@@ -186,6 +186,88 @@ class NnkDtwArgs(ctypes.Structure):
     ]
 
 
+NNK_MSSEG_LOGPOWER, NNK_MSSEG_POSTFILTER = 0, 1
+
+
+class NnkMlpgMs(ctypes.Structure):
+    _fields_ = [
+        ("ms_mean", ctypes.c_void_p),
+        ("ms_var", ctypes.c_void_p),
+        ("n", ctypes.c_int32),
+        ("n_iter", ctypes.c_int32),
+        ("step", ctypes.c_double),
+        ("weight", ctypes.c_double),
+        ("n_rows", ctypes.c_int64),
+    ]
+
+
+NNK_MIX_GEN_SELECT, NNK_MIX_GEN_ESTEP, NNK_MIX_GEN_OBJECTIVE = 0, 1, 2
+NNK_MIX_GEN_TILE, NNK_MIX_GEN_MAX_D, NNK_MIX_GEN_MAX_M = 32, 256, 64
+
+
+class NnkMixGenArgs(ctypes.Structure):
+    _fields_ = [
+        ("log_weights", ctypes.c_void_p),
+        ("means", ctypes.c_void_p),
+        ("vars", ctypes.c_void_p),
+        ("dtype", ctypes.c_int32),
+        ("M", ctypes.c_int32),
+        ("D", ctypes.c_int32),
+        ("n_utt", ctypes.c_int32),
+        ("utt_off", ctypes.c_void_p),
+        ("utt_len", ctypes.c_void_p),
+        ("tile_off", ctypes.c_void_p),
+        ("n_tiles", ctypes.c_int32),
+        ("col_map", ctypes.c_void_p),
+        ("win", NnkWindows),
+        ("mode", ctypes.c_int32),
+        ("c", ctypes.c_void_p),
+        ("c_ld", ctypes.c_int64),
+        ("c_cols", ctypes.c_int32),
+        ("lnorm", ctypes.c_void_p),
+        ("E", ctypes.c_void_p),
+        ("V", ctypes.c_void_p),
+        ("ll_part", ctypes.c_void_p),
+        ("status_word", ctypes.c_void_p),
+    ]
+
+
+class NnkTrajLl(ctypes.Structure):
+    _fields_ = [
+        ("targets", ctypes.c_void_p),
+        ("tgt_ld", ctypes.c_int64),
+        ("ll", ctypes.c_void_p),
+        ("grad", ctypes.c_int32),
+        ("grad_means", ctypes.c_void_p),
+        ("gm_ld", ctypes.c_int64),
+        ("grad_vars", ctypes.c_void_p),
+        ("gv_ld", ctypes.c_int64),
+        ("grad_targets", ctypes.c_void_p),
+        ("gx_ld", ctypes.c_int64),
+    ]
+
+
+class NnkTrajSample(ctypes.Structure):
+    _fields_ = [
+        ("sample_stride", ctypes.c_int64),
+        ("n_samples", ctypes.c_int32),
+        ("seed", ctypes.c_uint64),
+        ("keys", ctypes.c_void_p),
+        ("scale", ctypes.c_double),
+    ]
+
+
+class NnkMlpgVjp(ctypes.Structure):
+    _fields_ = [
+        ("grad_out", ctypes.c_void_p),
+        ("go_ld", ctypes.c_int64),
+        ("grad_means", ctypes.c_void_p),
+        ("gm_ld", ctypes.c_int64),
+        ("grad_vars", ctypes.c_void_p),
+        ("gv_ld", ctypes.c_int64),
+    ]
+
+
 CHAIN_DTYPE = np.dtype([("in_col", np.int32), ("win_stride", np.int32), ("out_col", np.int32), ("flags", np.int32)])
 
 P, vp, i32, i64, f64 = ctypes.POINTER, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_double
@@ -250,6 +332,17 @@ SIGNATURES = {
     "nnk_preemphasis": (ctypes.c_int, [vp, vp, i32, i64, i64, vp, f64, i32, vp, i64, vp, vp]),
     "nnk_mulaw": (ctypes.c_int, [vp, i32, vp, i32, i32, i64, f64, vp]),
     "nnk_modspec": (ctypes.c_int, [i32, i32, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp, f64, f64, i32, i32, vp]),
+    "nnk_mlpg_ms": (ctypes.c_int, [P(NnkMlpgArgs), P(NnkMlpgMs), vp]),
+    "nnk_mlpg_ms_workspace_bytes": (size_t, [i32, i32, i32, i64, i64, P(NnkWindows)]),
+    "nnk_ms_segment": (ctypes.c_int, [i32, i32, i32, i32, vp, vp, vp, i32, i32, i32, vp, vp, vp]),
+    "nnk_mlpg_ms_segment": (ctypes.c_int, [P(NnkMlpgArgs), P(NnkMlpgMs), i32, vp]),
+    "nnk_mix_gen": (ctypes.c_int, [P(NnkMixGenArgs), vp]),
+    "nnk_mlpg_traj_ll": (ctypes.c_int, [P(NnkMlpgArgs), P(NnkTrajLl), vp]),
+    "nnk_mlpg_traj_ll_workspace_bytes": (size_t, [i32, i32, i32, P(NnkWindows)]),
+    "nnk_mlpg_traj_sample": (ctypes.c_int, [P(NnkMlpgArgs), P(NnkTrajSample), vp]),
+    "nnk_mlpg_traj_sample_workspace_bytes": (size_t, [i32, i32, i32, P(NnkWindows)]),
+    "nnk_mlpg_vjp": (ctypes.c_int, [P(NnkMlpgArgs), P(NnkMlpgVjp), vp]),
+    "nnk_mlpg_vjp_workspace_bytes": (size_t, [i32, i32, i32, P(NnkWindows)]),
     "nnk_peer_alloc": (ctypes.c_int, [size_t, P(vp)]),
     "nnk_peer_free": (ctypes.c_int, [vp]),
     "nnk_peer_export": (ctypes.c_int, [vp, vp]),
@@ -259,53 +352,6 @@ SIGNATURES = {
 }
 EXPORTS = list(SIGNATURES)
 
-# the segment-level modulation-spectrum kernels (include/nnk_ms_segment.h), in the same library; the
-# nnk_mlpg_ms_t argument of nnk_mlpg_ms_segment is passed by reference to paramgen's ctypes mirror of it
-NNK_MSSEG_LOGPOWER, NNK_MSSEG_POSTFILTER = 0, 1
-MS_SEGMENT_SIGNATURES = {
-    "nnk_ms_segment": (ctypes.c_int, [i32, i32, i32, i32, vp, vp, vp, i32, i32, i32, vp, vp, vp]),
-    "nnk_mlpg_ms_segment": (ctypes.c_int, [P(NnkMlpgArgs), vp, i32, vp]),
-}
-
-# parameter generation considering the modulation spectrum (include/nnk_ms_gen.h), in the same library; the
-# nnk_mlpg_ms_t argument is passed by reference to paramgen's ctypes mirror of it
-MS_GEN_SIGNATURES = {
-    "nnk_mlpg_ms": (ctypes.c_int, [P(NnkMlpgArgs), vp, vp]),
-    "nnk_mlpg_ms_workspace_bytes": (size_t, [i32, i32, i32, i64, i64, P(NnkWindows)]),
-}
-
-# parameter generation from mixture outputs (include/nnk_mix_gen.h), in the same library; the nnk_mix_gen_args_t
-# argument is passed by reference to paramgen's ctypes mirror of it
-NNK_MIX_GEN_SELECT, NNK_MIX_GEN_ESTEP, NNK_MIX_GEN_OBJECTIVE = 0, 1, 2
-NNK_MIX_GEN_TILE, NNK_MIX_GEN_MAX_D, NNK_MIX_GEN_MAX_M = 32, 256, 64
-
-MIX_GEN_SIGNATURES = {
-    "nnk_mix_gen": (ctypes.c_int, [vp, vp]),
-}
-
-
-# the trajectory-model log-likelihood (include/nnk_traj_ll.h), in the same library; the nnk_traj_ll_t argument is
-# passed by reference to paramgen's ctypes mirror of it
-TRAJ_LL_SIGNATURES = {
-    "nnk_mlpg_traj_ll": (ctypes.c_int, [P(NnkMlpgArgs), vp, vp]),
-    "nnk_mlpg_traj_ll_workspace_bytes": (size_t, [i32, i32, i32, P(NnkWindows)]),
-}
-
-
-# sampling from the trajectory model (include/nnk_traj_sample.h), in the same library; the nnk_traj_sample_t
-# argument is passed by reference to paramgen's ctypes mirror of it
-TRAJ_SAMPLE_SIGNATURES = {
-    "nnk_mlpg_traj_sample": (ctypes.c_int, [P(NnkMlpgArgs), vp, vp]),
-    "nnk_mlpg_traj_sample_workspace_bytes": (size_t, [i32, i32, i32, P(NnkWindows)]),
-}
-
-
-# the gradient of MLPG in its means and variances (include/nnk_mlpg_vjp.h), in the same library; the
-# nnk_mlpg_vjp_t argument is passed by reference to paramgen's ctypes mirror of it
-VJP_SIGNATURES = {
-    "nnk_mlpg_vjp": (ctypes.c_int, [P(NnkMlpgArgs), vp, vp]),
-    "nnk_mlpg_vjp_workspace_bytes": (size_t, [i32, i32, i32, P(NnkWindows)]),
-}
 
 class NnkError(RuntimeError):
     pass
@@ -320,10 +366,7 @@ def _load():
     L.nnk_abi_version.restype = ctypes.c_int
     if L.nnk_abi_version() != ABI_VERSION:
         raise ImportError("libnnk_b200.so ABI %d != binding ABI %d: rebuild" % (L.nnk_abi_version(), ABI_VERSION))
-    for name, (restype, argtypes) in (list(SIGNATURES.items()) + list(MS_SEGMENT_SIGNATURES.items()) +
-                                      list(MS_GEN_SIGNATURES.items()) + list(MIX_GEN_SIGNATURES.items()) +
-                                      list(TRAJ_LL_SIGNATURES.items()) + list(TRAJ_SAMPLE_SIGNATURES.items()) +
-                                      list(VJP_SIGNATURES.items())):
+    for name, (restype, argtypes) in SIGNATURES.items():
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, argtypes
     return L

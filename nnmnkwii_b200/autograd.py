@@ -9,7 +9,7 @@ Differences that are additions, not signature changes:
     reduced once to its numerical band and applied as a banded stencil sweep
     (csrc/nnk_uvmlpg.cu) instead of two dense GEMMs that multiply ~95 % zeros.
 
-Additive, not in ``__all__``: ``TrajectoryLogLikelihood`` / ``trajectory_log_likelihood``, the log-likelihood of
+Additive: ``TrajectoryLogLikelihood`` / ``trajectory_log_likelihood``, the log-likelihood of
 target trajectories under the trajectory model of the MLPG inputs, differentiable in targets, means and variances.
 ``MLPGWithVariances`` / ``mlpg_with_variances``: MLPG differentiable in its means and its variances, for minimum
 generation error training of models that predict variances.
@@ -326,5 +326,6 @@ def unit_variance_mlpg(R, means):
 
 
 __all__ = ["MLPG", "MLPGBatch", "UnitVarianceMLPG", "mlpg", "mlpg_batch", "unit_variance_mlpg", "ModSpec",
-           "ModSpecBatch", "modspec", "modspec_batch"]
+           "ModSpecBatch", "modspec", "modspec_batch", "TrajectoryLogLikelihood", "trajectory_log_likelihood",
+           "MLPGWithVariances", "mlpg_with_variances"]
 _ = np  # numpy is part of the reference module's namespace

@@ -1,5 +1,5 @@
 // nnk_mix_gen.cu -- parameter generation from mixture outputs (paramgen.mlpg_mixture_batch) on sm_90a, float64
-// arithmetic (C ABI: include/nnk_mix_gen.h, definition: DESIGN.md 3.19).
+// arithmetic (C ABI: nnk_mix_gen in include/nnk_b200.h, definition: DESIGN.md 3.19).
 //
 // The E-step of the EM of Tokuda et al. (ICASSP 2000) over explicit per-frame mixtures: for every frame t and
 // component m the log-weight  l_{t,m} = lnorm_{t,m} - 1/2 |Y_t - mu_{t,m}|^2_{1 / s2_{t,m}}  over the columns
@@ -20,7 +20,6 @@
 // 3.19.
 #include <math_constants.h>
 
-#include "../../include/nnk_mix_gen.h"
 #include "nnk_common.cuh"
 
 namespace nnk {

@@ -26,9 +26,6 @@
 // (nw == NW), with NT <= 5 and rows narrow enough for as_geometry; everything else runs mlpg_kernel.
 #include <type_traits>
 
-#include "../../include/nnk_mlpg_vjp.h"
-#include "../../include/nnk_traj_ll.h"
-#include "../../include/nnk_traj_sample.h"
 #include "nnk_mlpg.cuh"
 #include "nnk_mlpg_as.cuh"
 
@@ -169,7 +166,8 @@ __device__ __forceinline__ double sym_at(const double (&sg)[S + 1][S + 1], int a
 }
 
 // ---- sampling from the trajectory model (MODE_SAMPLE, nnk_mlpg_traj_sample) --------------------------------------
-// include/nnk_traj_sample.h is the normative definition of the noise; these two functions restate it.
+// The comment of nnk_mlpg_traj_sample in include/nnk_b200.h is the normative definition of the noise; these two
+// functions restate it.
 // Philox4x32-10 (Salmon et al. 2011); the key bump after the last round is not used.
 __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
 #pragma unroll

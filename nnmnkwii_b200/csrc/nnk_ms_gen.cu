@@ -1,5 +1,5 @@
 // nnk_ms_gen.cu -- parameter generation considering the modulation spectrum (paramgen.mlpg_ms_batch; C ABI:
-// include/nnk_ms_gen.h, the segment level include/nnk_ms_segment.h; definition in DESIGN.md 3.18).
+// nnk_mlpg_ms and, for the segment level, nnk_mlpg_ms_segment in include/nnk_b200.h; definition in DESIGN.md 3.18).
 //
 // nnk_mlpg_ms chains existing pieces: nnk_mlpg_fwd gives c_m, and every trial's h = P^-1 g is one nnk_mlpg_solve
 // with a float64 right-hand side.  What is new is ms_gen_kernel<LOGN, TRIAL>, one CTA per (utterance, chain):
@@ -15,8 +15,6 @@
 // MS term) are per-thread partials over a fixed index set and a fixed tree: the bits do not depend on the batch.
 #include "nnk_common.cuh"
 #include "nnk_fft.cuh"
-#include "../../include/nnk_ms_gen.h"
-#include "../../include/nnk_ms_segment.h"
 
 namespace nnk {
 
@@ -200,7 +198,7 @@ static int dispatch_ms_gen(int logn, const MsGenParams& p, unsigned n_blocks, cu
   }
 }
 
-// ---- the segment-level MS term (nnk_mlpg_ms_segment, include/nnk_ms_segment.h) --------------------------------
+// ---- the segment-level MS term (nnk_mlpg_ms_segment) --------------------------------------------------------------
 // ms_gen_segment_kernel<LOGN, TRIAL> does ms_gen_kernel's job for the segment-level term, one CTA of 256 threads
 // per (utterance, chain), for chains of any length.  It walks the chain in tiles of P hop blocks (H = L / 2
 // frames each, the tiling of nnk_ms_segment.cu): the tile of blocks [p, p + P) stages frames

@@ -1,6 +1,6 @@
 // nnk_ms_segment.cu -- segment-level modulation spectrum: the log power of every windowed segment (the statistics
 // of postfilters.modspec_statistics(segment=L)) and the segment-level MS post-filter with its overlap-add
-// (postfilters.modspec_post_filter(segment=L)).  C ABI: include/nnk_ms_segment.h.
+// (postfilters.modspec_post_filter(segment=L)).  C ABI: nnk_ms_segment in include/nnk_b200.h.
 //
 // ms_segment_kernel<T, LOGN, FILTER>: one CTA per (utterance, tile of P hop blocks, group of DG adjacent columns).
 // Hop block i is frames [i H, (i + 1) H); it is covered by segments i and i + 1 (segment j starts at (j - 1) H),
@@ -19,7 +19,6 @@
 // The tile is then stored once, with coalesced row stores, zeros past the utterance's length.
 #include "nnk_common.cuh"
 #include "nnk_fft.cuh"
-#include "../../include/nnk_ms_segment.h"
 
 namespace nnk {
 

@@ -23,24 +23,20 @@ Additive, parameter generation considering global variance (Toda, Black & Tokuda
 :func:`gv_statistics` (csrc/nnk_mlpg.cu ``nnk_mlpg_gv``, csrc/nnk_stats.cu ``nnk_segment_moments``).
 
 Additive, parameter generation considering the modulation spectrum (DESIGN.md 3.18): :func:`mlpg_ms`,
-:func:`mlpg_ms_batch` (csrc/nnk_ms_gen.cu ``nnk_mlpg_ms``, C ABI include/nnk_ms_gen.h; with ``segment=L``
-``nnk_mlpg_ms_segment``, include/nnk_ms_segment.h).  Not in ``__all__``.
+:func:`mlpg_ms_batch` (csrc/nnk_ms_gen.cu ``nnk_mlpg_ms``; with ``segment=L`` ``nnk_mlpg_ms_segment``).
 
 Additive, parameter generation from per-frame mixture outputs over all components (DESIGN.md 3.19):
-:func:`mlpg_mixture`, :func:`mlpg_mixture_batch` (csrc/nnk_mix_gen.cu ``nnk_mix_gen``, C ABI
-include/nnk_mix_gen.h).  Not in ``__all__``.
+:func:`mlpg_mixture`, :func:`mlpg_mixture_batch` (csrc/nnk_mix_gen.cu ``nnk_mix_gen``).
 
 Additive, the log-likelihood of target trajectories under the trajectory model of the MLPG inputs (DESIGN.md
 3.20): :func:`trajectory_log_likelihood`, :func:`trajectory_log_likelihood_batch` (csrc/nnk_mlpg.cu
-``nnk_mlpg_traj_ll``, C ABI include/nnk_traj_ll.h).  Not in ``__all__``.
+``nnk_mlpg_traj_ll``).
 
 Additive, samples from that trajectory model with counter-based noise (DESIGN.md 3.21): :func:`trajectory_sample`,
-:func:`trajectory_sample_batch` (csrc/nnk_mlpg.cu ``nnk_mlpg_traj_sample``, C ABI include/nnk_traj_sample.h).  Not
-in ``__all__``.
+:func:`trajectory_sample_batch` (csrc/nnk_mlpg.cu ``nnk_mlpg_traj_sample``).
 
 Additive, the gradient of :func:`mlpg_batch` in its means and its variances for minimum-generation-error training
-(DESIGN.md 3.22): :func:`mlpg_vjp_batch` (csrc/nnk_mlpg.cu ``nnk_mlpg_vjp``, C ABI include/nnk_mlpg_vjp.h).  Not in
-``__all__``.
+(DESIGN.md 3.22): :func:`mlpg_vjp_batch` (csrc/nnk_mlpg.cu ``nnk_mlpg_vjp``).
 """
 import ctypes
 
@@ -54,6 +50,9 @@ __all__ = [
     "build_win_mats", "mlpg", "mlpg_grad", "full_window_mat", "unit_variance_mlpg_matrix", "reshape_means",
     "StreamLayout", "merlin_layout", "mlpg_batch",
     "mlpg_gv", "mlpg_gv_batch", "global_variance", "gv_statistics",
+    "mlpg_ms", "mlpg_ms_batch", "mlpg_mixture", "mlpg_mixture_batch",
+    "trajectory_log_likelihood", "trajectory_log_likelihood_batch", "trajectory_sample", "trajectory_sample_batch",
+    "mlpg_vjp_batch",
 ]
 
 
@@ -456,19 +455,6 @@ def gv_statistics(x, lengths=None, offsets=None):
 # ---------------------------------------------------------------------------------------------------
 # modulation spectrum (additive)
 # ---------------------------------------------------------------------------------------------------
-class _NnkMlpgMs(ctypes.Structure):
-    """ctypes mirror of ``nnk_mlpg_ms_t`` (include/nnk_ms_gen.h)."""
-    _fields_ = [
-        ("ms_mean", ctypes.c_void_p),
-        ("ms_var", ctypes.c_void_p),
-        ("n", ctypes.c_int32),
-        ("n_iter", ctypes.c_int32),
-        ("step", ctypes.c_double),
-        ("weight", ctypes.c_double),
-        ("n_rows", ctypes.c_int64),
-    ]
-
-
 _MS_GEN_N = (256, 512, 1024, 2048, 4096)
 _MS_SEG_N = (32, 64, 128, 256, 512)  # the segment level's DFT lengths (postfilters.SEGMENT_NS)
 
@@ -667,7 +653,7 @@ def _mlpg_ms_device(means, variances, windows, lengths, offsets, layout, padded,
         a.chains, a.n_chain, a.max_T, a.go_f64, a.win = chains_d.data_ptr(), layout.n_chain, max_T, 0, wc
         a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
         a.status_word, a.out_off = status.data_ptr(), None
-        p = _NnkMlpgMs()
+        p = _lib.NnkMlpgMs()
         p.ms_mean, p.ms_var, p.n, p.n_iter, p.step, p.weight = (mean_d.data_ptr(), var_d.data_ptr(), ms[2], ms[3],
                                                                 ms[4], ms[5])
         p.n_rows = n_rows
@@ -700,40 +686,12 @@ def mlpg_ms(mean_frames, variance_frames, windows, ms_mean, ms_var, n_iter=20, s
 # ---------------------------------------------------------------------------------------------------
 # mixture outputs (additive)
 # ---------------------------------------------------------------------------------------------------
-class _NnkMixGenArgs(ctypes.Structure):
-    """ctypes mirror of ``nnk_mix_gen_args_t`` (include/nnk_mix_gen.h)."""
-    _fields_ = [
-        ("log_weights", ctypes.c_void_p),
-        ("means", ctypes.c_void_p),
-        ("vars", ctypes.c_void_p),
-        ("dtype", ctypes.c_int32),
-        ("M", ctypes.c_int32),
-        ("D", ctypes.c_int32),
-        ("n_utt", ctypes.c_int32),
-        ("utt_off", ctypes.c_void_p),
-        ("utt_len", ctypes.c_void_p),
-        ("tile_off", ctypes.c_void_p),
-        ("n_tiles", ctypes.c_int32),
-        ("col_map", ctypes.c_void_p),
-        ("win", _lib.NnkWindows),
-        ("mode", ctypes.c_int32),
-        ("c", ctypes.c_void_p),
-        ("c_ld", ctypes.c_int64),
-        ("c_cols", ctypes.c_int32),
-        ("lnorm", ctypes.c_void_p),
-        ("E", ctypes.c_void_p),
-        ("V", ctypes.c_void_p),
-        ("ll_part", ctypes.c_void_p),
-        ("status_word", ctypes.c_void_p),
-    ]
-
-
 _MIX_DATA_ERRORS = {1: "a NaN or +inf log-weight", 2: "every log-weight is -inf",
                     3: "a variance that is not positive and finite"}
 
 
 def _mix_column_map(layout, nw):
-    """int32 ``(D_in,)`` column map of nnk_mix_gen (include/nnk_mix_gen.h): ``-1`` for a column no chain reads,
+    """int32 ``(D_in,)`` column map of nnk_mix_gen (include/nnk_b200.h): ``-1`` for a column no chain reads,
     ``out_col << 3`` for a copied column, ``(out_col << 3) | (w + 1)`` for window ``w`` of a smoothed one."""
     cmap = np.full(layout.D_in, -1, dtype=np.int32)
     for in_col, stride, out_col, flags in layout.chains.tolist():
@@ -897,7 +855,7 @@ def _mlpg_mixture_device(lw, mu, s2, windows, lens, layout, cmap, padded, n_iter
     V = torch.empty((n_rows, D), dtype=torch.float64, device=device)
     lnorm = torch.empty((n_rows, M), dtype=torch.float64, device=device)
     ll = torch.zeros((n_iter + 1, n_tiles), dtype=torch.float64, device=device) if want_ll else None
-    a = _NnkMixGenArgs()
+    a = _lib.NnkMixGenArgs()
     a.log_weights, a.means, a.vars = lw.data_ptr(), mu.data_ptr(), s2.data_ptr()
     a.dtype, a.M, a.D, a.n_utt = dev.torch_dtype_code(mu.dtype), M, D, n_utt
     a.utt_off, a.utt_len, a.tile_off, a.n_tiles = utt_off_d.data_ptr(), len_d.data_ptr(), tile_d.data_ptr(), n_tiles
@@ -1148,22 +1106,6 @@ def unit_variance_mlpg_matrix(windows, T):
 # ---------------------------------------------------------------------------------------------------
 # trajectory-model log-likelihood (additive)
 # ---------------------------------------------------------------------------------------------------
-class _NnkTrajLl(ctypes.Structure):
-    """ctypes mirror of nnk_traj_ll_t (include/nnk_traj_ll.h)."""
-    _fields_ = [
-        ("targets", ctypes.c_void_p),
-        ("tgt_ld", ctypes.c_int64),
-        ("ll", ctypes.c_void_p),
-        ("grad", ctypes.c_int32),
-        ("grad_means", ctypes.c_void_p),
-        ("gm_ld", ctypes.c_int64),
-        ("grad_vars", ctypes.c_void_p),
-        ("gv_ld", ctypes.c_int64),
-        ("grad_targets", ctypes.c_void_p),
-        ("gx_ld", ctypes.c_int64),
-    ]
-
-
 def _traj_ll_check(targets, means, variances, windows, lengths, offsets, layout):
     """Checked shapes of :func:`trajectory_log_likelihood_batch`'s arguments: ``(layout, padded, on_device)``.
     Raises ValueError for every argument error, before anything touches the device.  With ``targets=None`` it
@@ -1222,8 +1164,8 @@ def _traj_ll_check(targets, means, variances, windows, lengths, offsets, layout)
 def _traj_ll_device(targets, means, variances, windows, lengths, offsets, layout, padded, grad):
     """One launch of ``nnk_mlpg_traj_ll`` on checked CUDA tensors, on the current stream, with one host
     synchronisation (the status word).  Returns ``(ll (n_utt, n_chain) float64, lens, grads)``; ``grads`` is
-    ``(g_means, g_vars, g_targets)`` in the layouts of nnk_traj_ll.h (``g_vars`` float64 ``(n_utt, D)`` partials
-    for ``(D,)`` variances), or None."""
+    ``(g_means, g_vars, g_targets)`` in the layouts of nnk_mlpg_traj_ll in include/nnk_b200.h (``g_vars`` float64
+    ``(n_utt, D)`` partials for ``(D,)`` variances), or None."""
     import torch
 
     from . import _device as dev
@@ -1243,7 +1185,7 @@ def _traj_ll_device(targets, means, variances, windows, lengths, offsets, layout
     if not (n_utt and max_T and layout.n_chain):
         return ll, lens, grads
     a, keep, status = _traj_args(m, v, windows, table, layout, padded, _lib.lib.nnk_mlpg_traj_ll_workspace_bytes)
-    t = _NnkTrajLl()
+    t = _lib.NnkTrajLl()
     t.targets, t.tgt_ld, t.ll, t.grad = x.data_ptr(), layout.D_out, ll.data_ptr(), int(bool(grad))
     if grad:
         t.grad_means, t.gm_ld = grads[0].data_ptr(), D
@@ -1347,17 +1289,6 @@ def trajectory_log_likelihood(targets, mean_frames, variance_frames, windows):
 # ---------------------------------------------------------------------------------------------------
 # sampling from the trajectory model (additive)
 # ---------------------------------------------------------------------------------------------------
-class _NnkTrajSample(ctypes.Structure):
-    """ctypes mirror of nnk_traj_sample_t (include/nnk_traj_sample.h)."""
-    _fields_ = [
-        ("sample_stride", ctypes.c_int64),
-        ("n_samples", ctypes.c_int32),
-        ("seed", ctypes.c_uint64),
-        ("keys", ctypes.c_void_p),
-        ("scale", ctypes.c_double),
-    ]
-
-
 def _is_int(x):
     return isinstance(x, (int, np.integer)) and not isinstance(x, (bool, np.bool_))
 
@@ -1401,7 +1332,7 @@ def _traj_sample_device(means, variances, windows, table, layout, padded, n_samp
     a, keep, status = _traj_args(m, v, windows, table, layout, padded, _lib.lib.nnk_mlpg_traj_sample_workspace_bytes)
     a.out, a.out_ld = out.data_ptr(), layout.D_out
     keys_d = torch.from_numpy(keys.view(np.int32)).to(device) if keys is not None else None
-    t = _NnkTrajSample()
+    t = _lib.NnkTrajSample()
     t.sample_stride, t.n_samples, t.seed, t.scale = out[0].numel(), n_samples, seed, scale
     t.keys = keys_d.data_ptr() if keys_d is not None else None
     _lib.check(_lib.lib.nnk_mlpg_traj_sample(ctypes.byref(a), ctypes.byref(t), dev.current_stream_ptr(device)),
@@ -1420,10 +1351,10 @@ def trajectory_sample_batch(means, variances, windows, n_samples=1, seed=0, keys
     that :func:`trajectory_log_likelihood_batch` scores spreads around its mode.  ``scale = 0`` gives
     :func:`mlpg_batch`'s result in every sample.  See DESIGN.md 3.21.
 
-    The noise is counter-based (Philox4x32-10, Box-Muller; include/nnk_traj_sample.h defines it bit for bit): a
-    draw is a pure function of ``(seed, key, sample index, frame, output column)``.  It does not depend on the
-    batch around an utterance, its padding, the dtype or ``n_samples``: the first ``k`` of 16 samples are the
-    ``k`` samples of ``n_samples = k``.
+    The noise is counter-based (Philox4x32-10, Box-Muller; the comment of nnk_mlpg_traj_sample in include/nnk_b200.h
+    defines it bit for bit): a draw is a pure function of ``(seed, key, sample index, frame, output column)``.  It
+    does not depend on the batch around an utterance, its padding, the dtype or ``n_samples``: the first ``k`` of 16
+    samples are the ``k`` samples of ``n_samples = k``.
 
     Args:
         means, variances, windows, lengths, offsets, layout: as :func:`mlpg_batch` (flat or padded, per-frame or
@@ -1468,18 +1399,6 @@ def trajectory_sample(mean_frames, variance_frames, windows, n_samples=1, seed=0
 # ---------------------------------------------------------------------------------------------------
 # gradient of MLPG in means and variances (additive)
 # ---------------------------------------------------------------------------------------------------
-class _NnkMlpgVjp(ctypes.Structure):
-    """ctypes mirror of nnk_mlpg_vjp_t (include/nnk_mlpg_vjp.h)."""
-    _fields_ = [
-        ("grad_out", ctypes.c_void_p),
-        ("go_ld", ctypes.c_int64),
-        ("grad_means", ctypes.c_void_p),
-        ("gm_ld", ctypes.c_int64),
-        ("grad_vars", ctypes.c_void_p),
-        ("gv_ld", ctypes.c_int64),
-    ]
-
-
 def _mlpg_vjp_device(means, variances, windows, grad_output, table, layout, padded):
     """One launch of ``nnk_mlpg_vjp`` per workspace wave on checked CUDA tensors, on the current stream, with one
     host synchronisation (the status word).  Returns ``(grad_means, grad_variances)`` shaped like the inputs, in
@@ -1497,7 +1416,7 @@ def _mlpg_vjp_device(means, variances, windows, grad_output, table, layout, padd
     g_v = torch.zeros((n_utt, D), dtype=torch.float64, device=device) if var1d else torch.zeros_like(v)
     if n_utt and max_T and layout.n_chain:
         a, keep, status = _traj_args(m, v, windows, table, layout, padded, _lib.lib.nnk_mlpg_vjp_workspace_bytes)
-        t = _NnkMlpgVjp()
+        t = _lib.NnkMlpgVjp()
         t.grad_out, t.go_ld = go.data_ptr(), layout.D_out
         t.grad_means, t.gm_ld = g_m.data_ptr(), D
         t.grad_vars, t.gv_ld = g_v.data_ptr(), D

@@ -17,6 +17,9 @@ HOST_ONLY = {
     ("autograd", "unit_variance_mlpg"): "calls UnitVarianceMLPG.apply, which the UnitVarianceMLPG cases run",
     ("autograd", "modspec"): "calls ModSpec.apply, which the ModSpec case runs",
     ("autograd", "modspec_batch"): "calls ModSpecBatch.apply, which the ModSpecBatch case runs",
+    ("autograd", "trajectory_log_likelihood"): "calls TrajectoryLogLikelihood.apply, which the "
+                                               "TrajectoryLogLikelihood case runs",
+    ("autograd", "mlpg_with_variances"): "calls MLPGWithVariances.apply, which the MLPGWithVariances case runs",
     ("preprocessing", "trim_zeros_frames"): "NumPy on the host; the device trim runs inside DTWAligner and "
                                             "apply_each2d_trim",
     ("preprocessing", "remove_zeros_frames"): "NumPy on the host, the reference's semantics",
@@ -44,8 +47,12 @@ COVERED = {
     ("paramgen", "mlpg"), ("paramgen", "mlpg_batch"), ("paramgen", "mlpg_grad"), ("paramgen", "mlpg_grad_batch"),
     ("paramgen", "unit_variance_mlpg_matrix"), ("paramgen", "mlpg_gv"), ("paramgen", "mlpg_gv_batch"),
     ("paramgen", "global_variance"), ("paramgen", "gv_statistics"),
+    ("paramgen", "mlpg_ms"), ("paramgen", "mlpg_ms_batch"), ("paramgen", "mlpg_mixture"),
+    ("paramgen", "mlpg_mixture_batch"), ("paramgen", "trajectory_log_likelihood"),
+    ("paramgen", "trajectory_log_likelihood_batch"), ("paramgen", "trajectory_sample"),
+    ("paramgen", "trajectory_sample_batch"), ("paramgen", "mlpg_vjp_batch"),
     ("autograd", "MLPG"), ("autograd", "MLPGBatch"), ("autograd", "UnitVarianceMLPG"), ("autograd", "ModSpec"),
-    ("autograd", "ModSpecBatch"),
+    ("autograd", "ModSpecBatch"), ("autograd", "TrajectoryLogLikelihood"), ("autograd", "MLPGWithVariances"),
     ("metrics", "melcd"), ("metrics", "mean_squared_error"), ("metrics", "lf0_mean_squared_error"),
     ("metrics", "vuv_error"),
     ("preprocessing", "delta_features"), ("preprocessing", "meanvar"), ("preprocessing", "meanstd"),
@@ -82,6 +89,10 @@ EXPORTS_NOT_LAUNCHING = {
     "nnk_frame_stats_workspace_bytes": "sizing",
     "nnk_f0_interp_workspace_bytes": "sizing",
     "nnk_preemphasis_workspace_bytes": "sizing",
+    "nnk_mlpg_ms_workspace_bytes": "sizing",
+    "nnk_mlpg_traj_ll_workspace_bytes": "sizing",
+    "nnk_mlpg_traj_sample_workspace_bytes": "sizing",
+    "nnk_mlpg_vjp_workspace_bytes": "sizing",
 }
 
 # launching symbols that only multi-GPU sharding calls: tests/test_sharding_gpu.py covers what one GPU can

@@ -35,7 +35,8 @@ def test_every_export_is_sorted():
     # the symbols the kernel families launch through, by header name
     for name in ("nnk_mlpg_fwd", "nnk_mlpg_grad", "nnk_mlpg_solve", "nnk_mlpg_gv", "nnk_dtw_align",
                  "nnk_postfilter_apply", "nnk_gmm_em_estep", "nnk_kmeans_seed", "nnk_mlpg_host", "nnk_modspec",
-                 "nnk_gmm_traj_em"):
+                 "nnk_gmm_traj_em", "nnk_mlpg_ms", "nnk_mlpg_ms_segment", "nnk_ms_segment", "nnk_mix_gen",
+                 "nnk_mlpg_traj_ll", "nnk_mlpg_traj_sample", "nnk_mlpg_vjp"):
         assert name in launching, name
     assert not any(n.endswith("_workspace_bytes") for n in launching)
 

@@ -424,6 +424,219 @@ def _c():
     return make, call, check
 
 
+MS_MARGIN = 1e-9  # an accept decision whose relative margin is below this could flip under rounding
+
+
+def _ms_walk(rng, T, sd):
+    """Means (T, 3 sd) whose static part is a smooth walk, per-frame variances (tests/test_ms_gen_gpu.py)."""
+    m = np.concatenate([np.cumsum(rng.standard_normal((T, sd)), 0) * 0.1, 0.05 * rng.standard_normal((T, 2 * sd))], 1)
+    return m, rng.random((T, 3 * sd)) + 0.5
+
+
+def _ms_clear(ref_fn):
+    """The restatement's result, asserting that every accept decision on its path is clear of rounding (margin
+    inf: the trial moves c by at most 1e-11 of its size, so either decision gives the same result)."""
+    traces = []
+    ref = ref_fn(traces)
+    worst = min(t[2] for tr in traces for t in tr)
+    _bar(worst > MS_MARGIN)
+    return ref
+
+
+def _ms_check(i, o, ref_fn):
+    """Every utterance of the batch (o[0]) and the single-utterance call (o[1], utterance i["one"]) within 1e-9
+    of the restatement ``ref_fn(m, v, traces)``."""
+    m, v, y = _h(i["m"]), _h(i["v"]), _h(o[0])
+    off = np.concatenate([[0], np.cumsum(i["lens"])])
+    for u in range(len(i["lens"])):
+        a, b = off[u], off[u + 1]
+        if b > a:
+            ref = _ms_clear(lambda tr: ref_fn(m[a:b], v[a:b], tr))
+            _bar(np.abs(y[a:b] - ref).max() <= 1e-9 * np.abs(ref).max())
+            if u == i["one"]:
+                _bar(np.abs(_h(o[1]) - ref).max() <= 1e-9 * np.abs(ref).max())
+
+
+MS_ARGS = dict(n_iter=4, step=0.1, weight=1.0)  # on these inputs some trials are accepted and some rejected
+
+
+def _ms_call(i, **kw):
+    G = _G()
+    a, b = (int(x) for x in np.cumsum(i["lens"])[i["one"] - 1:i["one"] + 1])
+    return [G.mlpg_ms_batch(i["m"], i["v"], W3, i["mm"], i["mv"], lengths=i["lens"], **MS_ARGS, **kw),
+            G.mlpg_ms(i["m"][a:b], i["v"][a:b], W3, i["mm"], i["mv"], **MS_ARGS, **kw)]
+
+
+@case("mlpg_ms_batch_and_mlpg_ms_f64", [("paramgen", "mlpg_ms_batch"), ("paramgen", "mlpg_ms")], ws=True)
+def _c():
+    import oracle.ms_gen as OMS
+
+    def make(rng, big):
+        n, sd = (2048, 8) if big else (1024, 6)
+        lens = [1500, 30, 0, 2000, 40] if big else [900, 17, 0, 1024]
+        m, v = _ms_walk(rng, sum(lens), sd)
+        nat = rng.standard_normal((8, n, sd)) * 0.3 + np.cumsum(rng.standard_normal((8, n, sd)), 1) * 0.05
+        s = np.log(np.maximum(np.abs(np.fft.rfft(nat, n, axis=1)) ** 2, OMS.TINY))
+        return {"m": _cuda(m), "v": _cuda(v), "lens": lens, "one": 3, "mm": s.mean(0), "mv": s.var(0) + 0.5}
+
+    return make, _ms_call, lambda i, o: _ms_check(
+        i, o, lambda m, v, tr: OMS.mlpg_ms(m, v, W3, i["mm"], i["mv"], traces=tr, **MS_ARGS))
+
+
+@case("mlpg_ms_batch_and_mlpg_ms_segment_f64", [("paramgen", "mlpg_ms_batch"), ("paramgen", "mlpg_ms")], ws=True)
+def _c():
+    import ms_gen_segment_oracle as OMSS
+    import oracle.ms_segment as oseg
+    n = L = 128
+
+    def make(rng, big):
+        sd = 8 if big else 6
+        lens = [9500, 30, 0, 1100, 40] if big else [9000, 17, 0, 1024]
+        m, v = _ms_walk(rng, sum(lens), sd)
+        nat = rng.standard_normal((4, 4 * n, sd)) * 0.3 + np.cumsum(rng.standard_normal((4, 4 * n, sd)), 1) * 0.05
+        mean, var = oseg.statistics(list(nat), n, L)
+        return {"m": _cuda(m), "v": _cuda(v), "lens": lens, "one": 3, "mm": mean, "mv": var + 0.5}
+
+    return make, lambda i: _ms_call(i, segment=L), lambda i, o: _ms_check(
+        i, o, lambda m, v, tr: OMSS.mlpg_ms(m, v, W3, i["mm"], i["mv"], L, traces=tr, **MS_ARGS))
+
+
+def _merlin_like(D):
+    """The Merlin layout with D - 7 mgc columns (D = 187: merlin_layout()); the larger calls use D = 211."""
+    mgc = D - 7
+    return _G().StreamLayout(D, [(0, mgc // 3), (mgc, 1), (mgc + 3, 1, "copy"), (mgc + 4, 1)])
+
+
+MERLIN_STREAMS = [(0, 60), (180, 1), (183, 1, "copy"), (184, 1)]
+
+
+@case("mlpg_mixture_batch_and_mlpg_mixture_merlin_f64", [("paramgen", "mlpg_mixture_batch"),
+                                                          ("paramgen", "mlpg_mixture")], ws=True)
+def _c():
+    def make(rng, big):
+        lens, M, D = ([1000, 30, 0, 400, 20], 8, 211) if big else ([900, 17, 0, 300], 8, 187)
+        T = sum(lens)
+        lw = rng.standard_normal((T, M)) * 0.5
+        mu = np.cumsum(rng.standard_normal((T, M, D)), axis=0) * 0.1 + rng.standard_normal((1, M, D))
+        s2 = rng.random((T, M, D)) * 0.5 + 0.1
+        return {"lw": _cuda(lw), "mu": _cuda(mu), "s2": _cuda(s2), "lens": lens, "D": D}
+
+    def call(i):
+        G = _G()
+        y, L = G.mlpg_mixture_batch(i["lw"], i["mu"], i["s2"], W3, lengths=i["lens"],
+                                    layout=_merlin_like(i["D"]), n_iter=4, return_log_likelihood=True)
+        T, mgc = i["lens"][0], i["D"] - 7
+        y1, L1 = G.mlpg_mixture(i["lw"][:T], i["mu"][:T, :, :mgc].contiguous(), i["s2"][:T, :, :mgc].contiguous(),
+                                W3, n_iter=4, return_log_likelihood=True)
+        return [y, L, y1, L1]
+
+    def check(i, o):
+        import mix_gen_oracle as OMG
+        lw, mu, s2, y, L = _h(i["lw"]), _h(i["mu"]), _h(i["s2"]), _h(o[0]), _h(o[1])
+        off = np.concatenate([[0], np.cumsum(i["lens"])])
+        for u in range(len(i["lens"])):
+            a, b = off[u], off[u + 1]
+            if a == b:
+                _bar(np.all(L[u] == 0.0))
+                continue
+            want, Lw = OMG.mlpg_mixture(lw[a:b], mu[a:b], s2[a:b], W3, 4, streams=MERLIN_STREAMS)
+            _bar(rel_err(y[a:b], want) <= 1e-9 and np.all(np.abs(L[u] - Lw) <= 1e-10 * np.abs(Lw)))
+        T = i["lens"][0]
+        want, Lw = OMG.mlpg_mixture(lw[:T], mu[:T, :, :180], s2[:T, :, :180], W3, 4)
+        _bar(rel_err(_h(o[2]), want) <= 1e-9 and np.all(np.abs(_h(o[3]) - Lw) <= 1e-10 * np.abs(Lw)))
+    return make, call, check
+
+
+def _traj_data(rng, lens, D, D_out):
+    """Targets, means and per-frame variances of the trajectory-model tests, float64."""
+    n = sum(lens)
+    m = np.cumsum(rng.standard_normal((n, D)), axis=0) * 0.05 + rng.standard_normal((n, D)) * 0.3
+    v = rng.random((n, D)) + 0.5
+    x = np.cumsum(rng.standard_normal((n, D_out)), axis=0) * 0.05 + rng.standard_normal((n, D_out)) * 0.2
+    return x, m, v
+
+
+def _traj_make(rng, big):
+    lens, D = ([1000, 30, 400, 20], 211) if big else ([900, 17, 300], 187)
+    x, m, v = _traj_data(rng, lens, D, (D - 7) // 3 + 3)
+    go = rng.standard_normal((sum(lens), (D - 7) // 3 + 3))
+    return {"x": _cuda(x), "m": _cuda(m), "v": _cuda(v), "vg": _cuda(rng.random(D) + 0.5), "go": _cuda(go),
+            "lens": lens, "D": D}
+
+
+def _one(i, k):
+    """Utterance 0 of input ``k`` in the single-stream layout: the mgc columns (the static ones of targets)."""
+    T, mgc = i["lens"][0], i["D"] - 7
+    return i[k][:T, :mgc // 3 if k == "x" else mgc].contiguous()
+
+
+@case("trajectory_log_likelihood_batch_single_and_autograd_merlin_f64",
+      [("paramgen", "trajectory_log_likelihood_batch"), ("paramgen", "trajectory_log_likelihood"),
+       ("autograd", "TrajectoryLogLikelihood")], ws=True)
+def _c():
+    def call(i):
+        import torch
+        G, lay = _G(), _merlin_like(i["D"])
+        ll = G.trajectory_log_likelihood_batch(i["x"], i["m"], i["v"], W3, lengths=i["lens"], layout=lay)
+        ll1 = G.trajectory_log_likelihood(_one(i, "x"), _one(i, "m"), _one(i, "v"), W3)
+        x, m, v = (i[k].clone().requires_grad_(True) for k in ("x", "m", "v"))
+        la = _AF().TrajectoryLogLikelihood.apply(x, m, v, W3, i["lens"], lay)
+        la.backward(torch.ones_like(la))
+        return [ll, ll1, la.detach(), x.grad, m.grad, v.grad]
+
+    def check(i, o):
+        from test_traj_ll_gpu import _compare, _oracle_batch
+        x, m, v = (_h(i[k]) for k in ("x", "m", "v"))
+        ll, gm, gv, gx = _oracle_batch(x, m, v, W3, i["lens"], MERLIN_STREAMS)
+        _compare([_h(o[2]), _h(o[4]), _h(o[5]), _h(o[3])], (ll, gm, gv, gx), "autograd")
+        _bar(np.all(np.abs(_h(o[0]) - ll) <= 1e-11 * np.maximum(1.0, np.abs(ll))))
+        T = i["lens"][0]
+        ll1 = _oracle_batch(x[:T, :60], m[:T, :180], v[:T, :180], W3, [T])[0][0]
+        _bar(np.all(np.abs(_h(o[1]) - ll1) <= 1e-11 * np.maximum(1.0, np.abs(ll1))))
+    return _traj_make, call, check
+
+
+@case("trajectory_sample_batch_and_single_merlin_f64", [("paramgen", "trajectory_sample_batch"),
+                                                         ("paramgen", "trajectory_sample")], ws=True)
+def _c():
+    def call(i):
+        G = _G()
+        return [G.trajectory_sample_batch(i["m"], i["v"], W3, n_samples=3, seed=16, lengths=i["lens"],
+                                          layout=_merlin_like(i["D"])),
+                G.trajectory_sample(_one(i, "m"), _one(i, "v"), W3, n_samples=3, seed=16)]
+
+    def check(i, o):
+        from test_traj_sample_gpu import _compare, _oracle
+        m, v = _h(i["m"]), _h(i["v"])
+        _compare(_h(o[0]), _oracle(m, v, W3, i["lens"], 3, 16, streams=MERLIN_STREAMS), "batch")
+        T = i["lens"][0]
+        _compare(_h(o[1]), _oracle(m[:T, :180], v[:T, :180], W3, [T], 3, 16), "single")
+    return _traj_make, call, check
+
+
+@case("mlpg_vjp_batch_and_MLPGWithVariances_merlin_f64", [("paramgen", "mlpg_vjp_batch"),
+                                                           ("autograd", "MLPGWithVariances")], ws=True)
+def _c():
+    def call(i):
+        G, lay = _G(), _merlin_like(i["D"])
+        out = list(G.mlpg_vjp_batch(i["m"], i["v"], W3, i["go"], lengths=i["lens"], layout=lay))
+        out += list(G.mlpg_vjp_batch(i["m"], i["vg"], W3, i["go"], lengths=i["lens"], layout=lay))
+        m, v = i["m"].clone().requires_grad_(True), i["v"].clone().requires_grad_(True)
+        y = _AF().MLPGWithVariances.apply(m, v, W3, i["lens"], lay)
+        y.backward(i["go"])
+        return out + [y.detach(), m.grad, v.grad]
+
+    def check(i, o):
+        from test_mlpg_vjp_gpu import _compare, _oracle_batch
+        m, v, vg, go = (_h(i[k]) for k in ("m", "v", "vg", "go"))
+        want = _oracle_batch(m, v, W3, go, i["lens"], MERLIN_STREAMS)
+        _compare([_h(o[0]), _h(o[1])], want, "per-frame")
+        _compare([_h(o[2]), _h(o[3])], _oracle_batch(m, vg, W3, go, i["lens"], MERLIN_STREAMS), "(D,)")
+        _merlin_ref(m, v, i["lens"], _h(o[4]))
+        _compare([_h(o[5]), _h(o[6])], want, "autograd")
+    return _traj_make, call, check
+
+
 # ---- autograd ----
 def _AF():
     from nnmnkwii_b200 import autograd
@@ -876,6 +1089,41 @@ def _c():
             _bar(not y[L:].any() and (L == 0 or rel_err(y[:L], OM.post_filter(x[b, :L], o[2:4], o[0:2], 0.8, MS_N))
                                       < 1e-10))
     return make, call, check
+
+
+def _ms_segment_case(dt):
+    n, L, tol = 64, 50, 1e-4 if dt == np.float32 else 1e-10
+
+    def make(rng, big):
+        T, D = (1000, 10) if big else (900, 9)
+        lens = np.array([1000, 30, 0, 600, 5] if big else [900, 17, 0, 512])
+        w = rng.standard_normal((3, 401, D))
+        return {"x": _cuda(_nan_padded(rng, lens, T, D, dt)), "lens": lens,
+                "nat": _cuda((13.0 * (w[:, 1:] + 0.2 * w[:, :-1])).astype(dt))}
+
+    def call(i):
+        from nnmnkwii_b200.postfilters import modspec_post_filter, modspec_statistics
+        G = modspec_statistics(i["x"], n=n, lengths=i["lens"], segment=L)
+        N = modspec_statistics(i["nat"], n=n, segment=L)
+        return list(G) + list(N) + [modspec_post_filter(i["x"], N, G, k=0.8, n=n, lengths=i["lens"], segment=L)]
+
+    def check(i, o):
+        import oracle.ms_segment as OS
+        from test_ms_segment_gpu import _check_stats
+        x = _h(i["x"])
+        for got, utts in ((o[0:2], [x[b, :Lb] for b, Lb in enumerate(i["lens"]) if Lb]), (o[2:4], list(_h(i["nat"])))):
+            _check_stats(got, OS.statistics(utts, n, L), dt, utts, n, L)
+        G, N = [_h(t).astype(np.float64) for t in o[0:2]], [_h(t).astype(np.float64) for t in o[2:4]]
+        for b, Lb in enumerate(i["lens"]):  # the filter against the restatement given the device's statistics
+            y = _h(o[4])[b]
+            _bar(not y[Lb:].any() and (Lb == 0 or rel_err(y[:Lb], OS.post_filter(x[b, :Lb], N, G, 0.8, n, L)) <= tol))
+    return make, call, check
+
+
+for _dt in (np.float32, np.float64):
+    CATALOGUE.append(Case("modspec_statistics_and_post_filter_segment_%s" % np.dtype(_dt).name,
+                          [("postfilters", "modspec_statistics"), ("postfilters", "modspec_post_filter")],
+                          *_ms_segment_case(_dt)))
 
 
 # ---- baseline.gmm ----

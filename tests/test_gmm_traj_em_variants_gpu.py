@@ -106,7 +106,9 @@ def launch(S, name, ll):
 
 
 def test_every_instance_is_launched_by_name():
-    cases = [([S, name, ll], r"\bgmm_traj_em_kernel<") for S, name in INSTANCES for ll in (False, True)]
+    # each kernel the test asserts on is named, so that a profile that lost one of them is taken again
+    cases = [([S, name, ll], [r"\bgmm_traj_em_kernel<", r"\bgmm_traj_em_kernel<\d, true>"]
+              + ([r"\bgmm_traj_em_kernel<\d, false>"] if ll else [])) for S, name in INSTANCES for ll in (False, True)]
     res = VM.profiled_in_child("test_gmm_traj_em_variants_gpu", "launch", cases)
     seen = set()
     for (case, _), (names, err) in zip(cases, res):

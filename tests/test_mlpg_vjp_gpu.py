@@ -254,7 +254,7 @@ def test_autograd_forward_is_mlpg_batch_and_expand_gets_frame_gradients():
     assert np.all(np.abs(vt2.grad.cpu().numpy() - want) <= 1e-5 * np.abs(gv).sum(axis=0))
 
 
-# ---- kernels, launches, errors and streams -------------------------------------------------------------------------
+# ---- kernels, launches and errors ----------------------------------------------------------------------------------
 SETS_K = dict(SETS, static=[(0, 0, np.array([1.0]))])
 # window set -> (NW, L, U, PF) of the instance that serves it; "static" is the static window alone (instance 0)
 INST = {"static": (1, 0, 0, 4), "nw3": (3, 1, 1, 4), "hw2": (3, 2, 2, 2), "hw4": (4, 4, 4, 2)}
@@ -307,25 +307,3 @@ def test_non_positive_variance_raises():
     with pytest.raises(np.linalg.LinAlgError) as e_vjp:
         G.mlpg_vjp_batch(m, v, STD, go, lengths=[30, 20])
     assert str(e_vjp.value) == str(e_fwd.value)
-
-
-def test_poisoned_allocations_and_side_stream():
-    import torch
-    G = _G()
-    lens = [900, 17, 300]
-    m, v, go = (_cuda(a) for a in _data(np.random.default_rng(17), sum(lens), 187, 63))
-    kw = dict(lengths=lens, layout=G.merlin_layout())
-    g0 = G.mlpg_vjp_batch(m, v, STD, go, **kw)
-    torch.cuda.synchronize()
-    for _ in range(2):
-        junk = [torch.full((1 << 22,), float("nan"), dtype=torch.float64, device="cuda") for _ in range(8)]
-        del junk
-        g = G.mlpg_vjp_batch(m, v, STD, go, **kw)
-        assert all(torch.equal(a, b) for a, b in zip(g, g0))
-    side = torch.cuda.Stream()
-    with torch.cuda.stream(side):
-        torch.cuda._sleep(20_000_000)
-        ms, vs, gs = m.clone(), v.clone(), go.clone()
-        g = G.mlpg_vjp_batch(ms, vs, STD, gs, **kw)
-    torch.cuda.current_stream().wait_stream(side)
-    assert all(torch.equal(a, b) for a, b in zip(g, g0))

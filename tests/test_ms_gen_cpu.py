@@ -1,18 +1,13 @@
 """Without a GPU: parameter generation considering the modulation spectrum.  The float64 restatement
 (oracle/ms_gen.py) the GPU tests compare against has the definition's properties (analytic gradient, an objective
 that never decreases, plain MLPG for n_iter = 0 or exempt bins); paramgen.mlpg_ms / mlpg_ms_batch and
-baseline.gmm.MLPG(ms=...) refuse bad arguments before any device work; and include/nnk_ms_gen.h matches its
-binding table."""
-import ctypes
-import os
-import re
-
+baseline.gmm.MLPG(ms=...) refuse bad arguments before any device work."""
 import numpy as np
 import pytest
 
 import oracle.gv as ogv
 import oracle.ms_gen as O
-from conftest import ROOT, windows_set
+from conftest import windows_set
 
 STD = windows_set()[2]
 
@@ -173,53 +168,3 @@ def test_gmm_mlpg_ms_argument_errors():
     assert MLPG(gmm).ms is None and model.ms is not None
     with pytest.raises(ValueError, match="modulation spectrum"):
         model.transform_em(rng.standard_normal((20, 4)))
-
-
-# ---- the C ABI header --------------------------------------------------------------------------------------------
-def _code():
-    src = open(os.path.join(ROOT, "include", "nnk_ms_gen.h")).read()
-    return re.sub(r"/\*.*?\*/|//[^\n]*", "", src, flags=re.S)
-
-
-def _kind(c_type):
-    if "*" in c_type:
-        return "ptr"
-    return {"int": "i4", "int32_t": "i4", "int64_t": "i8", "size_t": "i8", "double": "f8"}[
-        c_type.replace("const", "").strip()]
-
-
-def _ctypes_kind(t):
-    if issubclass(t, (ctypes._Pointer, ctypes.c_void_p)):
-        return "ptr"
-    return "f8" if t is ctypes.c_double else "i%d" % ctypes.sizeof(t)
-
-
-def test_header_prototypes_match_the_binding_table():
-    from nnmnkwii_b200 import _lib
-    protos = re.findall(r"([A-Za-z_][\w ]*\**)\s*\b(nnk_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", _code())
-    assert sorted(name for _, name, _ in protos) == sorted(_lib.MS_GEN_SIGNATURES) == [
-        "nnk_mlpg_ms", "nnk_mlpg_ms_workspace_bytes"]
-    L = ctypes.CDLL(_lib.LIB_PATH)
-    for ret, name, params in protos:
-        assert hasattr(L, name), name
-        restype, argtypes = _lib.MS_GEN_SIGNATURES[name]
-        assert _ctypes_kind(restype) == _kind(ret), name
-        params = [p.strip() for p in params.split(",")]
-        assert [_ctypes_kind(t) for t in argtypes] == [_kind(p.rsplit(None, 1)[0]) for p in params], name
-    # the new symbols stay out of the core table
-    assert not set(_lib.MS_GEN_SIGNATURES) & set(_lib.EXPORTS)
-
-
-def test_struct_matches_its_mirror():
-    from nnmnkwii_b200 import paramgen as G
-    body = re.search(r"typedef struct nnk_mlpg_ms \{(.*?)\} nnk_mlpg_ms_t;", _code(), re.S).group(1)
-    want = []
-    for decl in (d.strip() for d in body.split(";") if d.strip()):
-        c_type, name = re.match(r"((?:const\s+)?[A-Za-z_]\w*\s*\**)\s*(\w+)", decl).groups()
-        want.append((name, _kind(c_type)))
-    assert [(f, _ctypes_kind(t)) for f, t in G._NnkMlpgMs._fields_] == want
-
-
-def test_public_names_unchanged():
-    from nnmnkwii_b200 import paramgen as G
-    assert "mlpg_ms" not in G.__all__ and "mlpg_ms_batch" not in G.__all__

@@ -3,18 +3,14 @@
 gradient is the derivative of its MS term, checked by central differences and by torch autograd of the
 definition; its objective never decreases; n_iter = 0 is plain MLPG); paramgen.mlpg_ms / mlpg_ms_batch with
 ``segment`` and baseline.gmm.MLPG(ms_segment=...) refuse bad arguments before any device work while
-``segment=None`` keeps its refusals; and include/nnk_ms_segment.h matches its binding table."""
-import ctypes
-import os
-import re
-
+``segment=None`` keeps its refusals."""
 import numpy as np
 import pytest
 
 import ms_gen_segment_oracle as S
 import oracle.gv as ogv
 import oracle.ms_segment as oseg
-from conftest import ROOT, windows_set
+from conftest import windows_set
 
 STD = windows_set()[2]
 
@@ -222,43 +218,3 @@ def test_gmm_mlpg_ms_segment_argument_errors():
     assert model.ms_segment == 20 and MLPG(gmm).ms_segment is None
     with pytest.raises(ValueError, match="modulation spectrum"):
         model.transform_em(rng.standard_normal((20, 4)))
-
-
-# ---- the C ABI header --------------------------------------------------------------------------------------------
-def _code():
-    src = open(os.path.join(ROOT, "include", "nnk_ms_segment.h")).read()
-    return re.sub(r"/\*.*?\*/|//[^\n]*", "", src, flags=re.S)
-
-
-def _kind(c_type):
-    if "*" in c_type:
-        return "ptr"
-    return {"int": "i4", "int32_t": "i4", "int64_t": "i8", "size_t": "i8", "double": "f8"}[
-        c_type.replace("const", "").strip()]
-
-
-def _ctypes_kind(t):
-    if issubclass(t, (ctypes._Pointer, ctypes.c_void_p)):
-        return "ptr"
-    return "f8" if t is ctypes.c_double else "i%d" % ctypes.sizeof(t)
-
-
-def test_header_prototypes_match_the_binding_table():
-    from nnmnkwii_b200 import _lib
-    assert '#include "nnk_ms_gen.h"' in _code()
-    protos = re.findall(r"([A-Za-z_][\w ]*\**)\s*\b(nnk_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", _code())
-    assert sorted(name for _, name, _ in protos) == sorted(_lib.MS_SEGMENT_SIGNATURES) == [
-        "nnk_mlpg_ms_segment", "nnk_ms_segment"]
-    L = ctypes.CDLL(_lib.LIB_PATH)
-    for ret, name, params in protos:
-        assert hasattr(L, name), name
-        restype, argtypes = _lib.MS_SEGMENT_SIGNATURES[name]
-        assert _ctypes_kind(restype) == _kind(ret), name
-        params = [p.strip() for p in params.split(",")]
-        assert [_ctypes_kind(t) for t in argtypes] == [_kind(p.rsplit(None, 1)[0]) for p in params], name
-    assert "nnk_mlpg_ms_segment" not in _lib.EXPORTS and "nnk_mlpg_ms_segment" not in _lib.MS_GEN_SIGNATURES
-
-
-def test_public_names_unchanged():
-    from nnmnkwii_b200 import paramgen as G
-    assert "mlpg_ms" not in G.__all__ and "mlpg_ms_batch" not in G.__all__

@@ -1,12 +1,10 @@
 """Sampling from the trajectory model without a GPU: the float64 restatement (tests/traj_sample_oracle.py) -- its
 Philox against the published known answers, its banded recurrence against the dense Cholesky form, its samples
 against the model's mean and covariance, and its normals against N(0, 1); the argument errors of
-paramgen.trajectory_sample_batch, raised before any launch; and the C ABI header include/nnk_traj_sample.h against
-its binding table and ctypes mirror."""
+paramgen.trajectory_sample_batch, raised before any launch, and those of the C entry point."""
 import ctypes
 import importlib.util
 import os
-import re
 
 import numpy as np
 import pytest
@@ -180,63 +178,11 @@ def test_argument_errors_raise_before_any_launch(monkeypatch):
         f(torch.from_numpy(m), torch.from_numpy(v), w, lengths=[30])
 
 
-# ---- the C ABI header ------------------------------------------------------------------------------------------
-def _code():
-    src = open(os.path.join(ROOT, "include", "nnk_traj_sample.h")).read()
-    return re.sub(r"/\*.*?\*/|//[^\n]*", "", src, flags=re.S)
-
-
-def _kind(c_type):
-    if "*" in c_type:
-        return "ptr"
-    return {"int": "i4", "int32_t": "i4", "int64_t": "i8", "uint64_t": "u8", "size_t": "u8", "double": "f8",
-            "nnk_windows_t": "windows"}[c_type.replace("const", "").strip()]
-
-
-def _ctypes_kind(t):
-    from nnmnkwii_b200 import _lib
-    if t is _lib.NnkWindows:
-        return "windows"
-    if issubclass(t, (ctypes._Pointer, ctypes.c_void_p)):
-        return "ptr"
-    if t is ctypes.c_double:
-        return "f8"
-    signed = t(-1).value == -1
-    return ("i%d" if signed else "u%d") % ctypes.sizeof(t)
-
-
-def test_header_prototypes_match_the_binding_table():
-    from nnmnkwii_b200 import _lib
-    from nnmnkwii_b200 import paramgen as G
-    protos = re.findall(r"([A-Za-z_][\w ]*\**)\s*\b(nnk_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", _code())
-    assert sorted(name for _, name, _ in protos) == sorted(_lib.TRAJ_SAMPLE_SIGNATURES)
-    L = ctypes.CDLL(_lib.LIB_PATH)
-    for ret, name, params in protos:
-        assert hasattr(L, name), name
-        restype, argtypes = _lib.TRAJ_SAMPLE_SIGNATURES[name]
-        assert _ctypes_kind(restype) == _kind(ret), name
-        params = [p.strip() for p in params.split(",")]
-        assert [_ctypes_kind(t) for t in argtypes] == [_kind(p.rsplit(None, 1)[0]) for p in params], name
-    assert not set(_lib.TRAJ_SAMPLE_SIGNATURES) & set(_lib.EXPORTS)
-    for n in ("trajectory_sample", "trajectory_sample_batch"):
-        assert n not in G.__all__
-
-
-def test_struct_matches_its_mirror():
-    from nnmnkwii_b200 import paramgen as G
-    body = re.search(r"typedef struct nnk_traj_sample \{(.*?)\} nnk_traj_sample_t;", _code(), re.S).group(1)
-    want = []
-    for decl in (d.strip() for d in body.split(";") if d.strip()):
-        c_type, name = re.match(r"((?:const\s+)?[A-Za-z_]\w*\s*\**)\s*(\w+)", decl).groups()
-        want.append((name, _kind(c_type)))
-    assert [(f, _ctypes_kind(t)) for f, t in G._NnkTrajSample._fields_] == want
-
-
+# ---- the C entry point ------------------------------------------------------------------------------------
 def test_c_argument_checks():
     from nnmnkwii_b200 import _lib
-    from nnmnkwii_b200 import paramgen as G
     fn = _lib.lib.nnk_mlpg_traj_sample
-    a, t = _lib.NnkMlpgArgs(), G._NnkTrajSample()
+    a, t = _lib.NnkMlpgArgs(), _lib.NnkTrajSample()
     t.n_samples, t.scale = 1, 1.0
     assert fn(None, ctypes.byref(t), None) == _lib.NNK_ERR_ARG
     assert fn(ctypes.byref(a), None, None) == _lib.NNK_ERR_ARG
@@ -244,7 +190,7 @@ def test_c_argument_checks():
     assert fn(ctypes.byref(a), ctypes.byref(t), None) == _lib.NNK_OK  # empty batch
     for field, value in (("n_samples", 0), ("sample_stride", -1), ("scale", -1.0), ("scale", float("nan")),
                          ("scale", float("inf"))):
-        bad = G._NnkTrajSample()
+        bad = _lib.NnkTrajSample()
         ctypes.memmove(ctypes.byref(bad), ctypes.byref(t), ctypes.sizeof(t))
         setattr(bad, field, value)
         assert fn(ctypes.byref(a), ctypes.byref(bad), None) == _lib.NNK_ERR_ARG, field

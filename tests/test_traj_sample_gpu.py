@@ -254,7 +254,7 @@ def test_different_seeds_and_keys_give_different_draws():
             assert diff.all(), kw
 
 
-# ---- kernels, launches, errors and streams -------------------------------------------------------------------------
+# ---- kernels, launches and errors ----------------------------------------------------------------------------------
 def launch(kind, name, dt):
     import torch
     w = SETS_K[name]
@@ -307,24 +307,3 @@ def test_non_positive_variance_raises():
     with pytest.raises(np.linalg.LinAlgError) as e_s:
         G.trajectory_sample_batch(m, v, STD, n_samples=2, lengths=[30, 20])
     assert str(e_s.value) == str(e_fwd.value)
-
-
-def test_poisoned_allocations_and_side_stream():
-    import torch
-    G = _G()
-    lens = [900, 17, 300]
-    m, v = (_cuda(a) for a in _data(np.random.default_rng(16), sum(lens), 187))
-    kw = dict(lengths=lens, layout=G.merlin_layout(), n_samples=3, seed=16)
-    y0 = G.trajectory_sample_batch(m, v, STD, **kw)
-    torch.cuda.synchronize()
-    for _ in range(2):
-        junk = [torch.full((1 << 22,), float("nan"), dtype=torch.float64, device="cuda") for _ in range(8)]
-        del junk
-        assert torch.equal(G.trajectory_sample_batch(m, v, STD, **kw), y0)
-    side = torch.cuda.Stream()
-    with torch.cuda.stream(side):
-        torch.cuda._sleep(20_000_000)
-        ms, vs = m.clone(), v.clone()
-        y = G.trajectory_sample_batch(ms, vs, STD, **kw)
-    torch.cuda.current_stream().wait_stream(side)
-    assert torch.equal(y, y0)

@@ -1,5 +1,5 @@
 """Float64 NumPy / SciPy restatement of sampling from the trajectory model (paramgen.trajectory_sample_batch,
-DESIGN.md 3.21; include/nnk_traj_sample.h).  TEST INFRASTRUCTURE, NOT PRODUCT.
+DESIGN.md 3.21; the comment of nnk_mlpg_traj_sample in include/nnk_b200.h).  TEST INFRASTRUCTURE, NOT PRODUCT.
 
 Three parts:
 

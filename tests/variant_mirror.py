@@ -32,7 +32,9 @@ def profiled(fn, family=r"\b(mlpg|uv|dtw|fastdtw|trim_len)_\w*kernel\b", attempt
     while 180 profiles of the same call in a fresh process lost none.  At that rate three attempts still
     miss about once in 300 calls, and the suite makes hundreds; eight miss about once in 4 million.
     Pass a ``family`` that names the kernel the caller asserts on, so that a profile that kept only the
-    call's other kernels is repeated too."""
+    call's other kernels is repeated too.  A caller that asserts on several kernels of one call passes a list
+    of patterns: the call is repeated until the profile holds a kernel of each, since a profile can also lose
+    the record of one kernel of a call and keep another's."""
     import torch
     from torch.autograd import DeviceType
     from torch.profiler import ProfilerActivity, profile
@@ -47,15 +49,15 @@ def profiled(fn, family=r"\b(mlpg|uv|dtw|fastdtw|trim_len)_\w*kernel\b", attempt
                 err = e
             torch.cuda.synchronize()
         names = [e.name for e in prof.events() if e.device_type == DeviceType.CUDA]
-        if launched(names, family):
+        if all(launched(names, p) for p in ([family] if isinstance(family, str) else family)):
             return out, err, names
     raise AssertionError("the profiler collected no kernel names of %r in %d attempts: %s" % (family, attempts, names))
 
 
 def launched(names, pattern):
-    """Names matching the regular expression ``pattern``."""
-    rx = re.compile(pattern)
-    return [n for n in names if rx.search(n)]
+    """Names matching the regular expression ``pattern`` (a list of them: any of them)."""
+    rx = [re.compile(p) for p in ([pattern] if isinstance(pattern, str) else pattern)]
+    return [n for n in names if any(r.search(n) for r in rx)]
 
 
 # ---- MLPG ------------------------------------------------------------------------------------------------------
